@@ -11,9 +11,11 @@ memset + 256 MiB clean read) before each step so no step runs out of a warm cach
 times (max over ranks).  Inputs (particle state, maps) are resident in HBM; the per-step control + observation list (~300 B)
 rides in the launch parameters.  `e2e` repeats K steps through the public API with host buffers, one host synchronisation
 and a host read-back of the step's result record (best particle, gate, N_eff) every step.
-Second key `c4_strong`: BASELINE config 4 — 2^20 particles x 1024 landmarks sharded over the N GPUs (strong scaling; at
-N = 1 the whole 103 GB of landmark state lives on the one GPU), same timing rules, fewer steps.  `--config c4` makes it the
-primary line instead.
+Second key `c4_strong`: BASELINE config 4 — 2^19 particles x 1024 landmarks sharded over the N GPUs (strong scaling; at
+N = 1 the whole 52 GB of landmark state lives on the one 80 GB GPU), same timing rules, fewer steps.  `--config c4` makes it
+the primary line instead.
+`--dump-outputs DIR`: after the measurement, what the last step of the primary configuration returned to its caller is
+written as DIR/<name>.npy (float64; rank 0's particles), so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -23,6 +25,8 @@ import subprocess
 import sys
 import tempfile
 import time
+
+import numpy as np
 
 # stdout carries exactly one JSON line: whatever NCCL wants to say (its version banner when NCCL_DEBUG is set) goes to stderr
 os.environ.setdefault("NCCL_DEBUG_FILE", "/dev/stderr")
@@ -92,7 +96,37 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
+
+
+def gpu_info(index):
+    """name, power limit and top SM clock of the card the numbers are measured on"""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+        return {"name": out[0], "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except (OSError, subprocess.SubprocessError, IndexError, ValueError):
+        return None
+
+
+def dump_outputs(out_dir, arrays):
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
+def fastslam_outputs(g, n_local):
+    """what a caller of fastslam_update reads back after the step: particle poses + weights, the best particle, N_eff, the
+    resample gate, the ancestor of every slot (its own index when the step did not resample; rank 0 holds slots 0 ..
+    n_local - 1), and the maps of a fixed, seeded sample of 256 particles (all maps are up to 52 GB)"""
+    pose_w, _ = g.state(landmarks=False)
+    best_idx, best_pose = g.get_best_particle()
+    gate = g.last_gate()
+    ancestors = g.last_indices() if gate else np.arange(n_local)
+    slots = np.sort(np.random.default_rng(0).choice(n_local, size=min(256, n_local), replace=False))
+    return {"pose_weight": pose_w, "best_particle": np.concatenate([[best_idx], best_pose]), "neff": np.array([g.last_neff()]),
+            "resampled": np.array([float(gate)]), "resample_indices": ancestors,
+            "landmark_sample_slots": slots, "landmark_sample": np.stack([g.particle_landmarks(int(i)) for i in slots])}
 
 
 def make_scenario(total_steps):
@@ -211,7 +245,7 @@ def load_traffic():
 CONFIGS = {   # SURVEY.md §8(d)
     "c3": dict(name="FastSLAM 1.0 (fs1.rs fastslam_update), BASELINE config 3", particles_per_gpu=N_PARTICLES, particles_total=None,
                scenario="c3_scenario", scaling="weak"),
-    "c4": dict(name="FastSLAM 1.0 (fs1.rs fastslam_update), BASELINE config 4", particles_per_gpu=None, particles_total=1 << 20,
+    "c4": dict(name="FastSLAM 1.0 (fs1.rs fastslam_update), BASELINE config 4", particles_per_gpu=None, particles_total=1 << 19,
                scenario="c4_scenario", scaling="strong"),
 }
 
@@ -237,8 +271,9 @@ def make_engine(rr, grp, cfg_key, rank, world, local_rank):
     return cfg, n_global, scenarios, rdist
 
 
-def measure(rr, grp, cfg_key, K, W, rank, world, local_rank, with_e2e, sampler_cb=None):
-    """one configuration: warm-up, K flushed + event-timed steps, K un-flushed steps, (optionally) K end-to-end steps"""
+def measure(rr, grp, cfg_key, K, W, rank, world, local_rank, with_e2e, sampler_cb=None, dump_dir=None):
+    """one configuration: warm-up, K flushed + event-timed steps, K un-flushed steps, (optionally) K end-to-end steps;
+    dump_dir: rank 0 writes what the last step returned there"""
     from rust_robotics_b200 import dist as rdist, scenarios
     cfg = CONFIGS[cfg_key]
     n_global = cfg["particles_total"] or cfg["particles_per_gpu"] * world
@@ -284,7 +319,7 @@ def measure(rr, grp, cfg_key, K, W, rank, world, local_rank, with_e2e, sampler_c
         g.time_main_kernel(False)
         return first, ms, s0, s1
 
-    # pass A: the K steps `value` is quoted on.  No events inside a step: an event pair around the EKF launch costs ~8 us per step (it
+    # pass A: the K steps `value` is quoted on.  No events inside a step: an event pair around the EKF launch costs microseconds per step (it
     # breaks the programmatic dependent launch of the kernel behind it), so the kernel is timed on its own pass below.
     first, step_ms, st0, st1 = flushed_pass(False)
     if os.environ.get("BENCH_VERBOSE") and rank == 0:
@@ -351,6 +386,8 @@ def measure(rr, grp, cfg_key, K, W, rank, world, local_rank, with_e2e, sampler_c
     res = {"cfg": cfg, "sc": sc, "n_global": n_global, "t_flushed": t_flushed, "t_noflush": t_noflush, "launches": int(launches),
            "resamples": int(resamples), "kernel_ms": kernel_ms, "t_flushed_kernel_pass": t_flushed_b, "alg_bytes": alg_bytes, "obs_timed": obs_timed, "e2e": e2e,
            "serial_fallbacks": int(st1.serial_fallbacks), "K": K}
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, fastslam_outputs(g, n_local))
     g.close()
     return res
 
@@ -361,7 +398,7 @@ def run_ours(args, rank, world, local_rank):
     grp = rdist.TcpGroup()
     K, W = args.steps, args.warmup
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    primary = measure(rr, grp, args.config, K, W, rank, world, local_rank, True)
+    primary = measure(rr, grp, args.config, K, W, rank, world, local_rank, True, dump_dir=args.dump_outputs)
     second_key = "c4" if args.config == "c3" else "c3"
     second = None
     if not args.no_second:
@@ -386,7 +423,7 @@ def run_ours(args, rank, world, local_rank):
                                          "%.4f ms each (the event pairs break the programmatic dependent launch), so `value` is quoted on the pass without them"
                                          % (r["t_flushed_kernel_pass"] / K * 1e3),
                              "note": "per GPU; algorithmic bytes = particles x (64 + 96 x observations of the step), SURVEY.md 8(d)"},
-                "clocks": clocks, "serial_fallbacks": r["serial_fallbacks"]}
+                "clocks": clocks, "gpu": gpu_info(local_rank), "serial_fallbacks": r["serial_fallbacks"]}
         if second:
             q = second
             line[{"c4": "c4_strong", "c3": "c3_weak"}[second_key]] = {
@@ -468,8 +505,13 @@ def run_pf(args):
                          # SURVEY.md 8(d): config 2 is bounded by the FP64 pipe, not HBM: the reference's formula costs 12 f64 operations per
                          # (particle, beam) counting sqrt / exp / div as one each (pf.rs:317-328,476-479) + 13 per particle for predict
                          "fp64_algorithmic_tflops": n * (12.0 * kobs + 13.0) / (kms * 1e-3) / 1e12,
-                         "fp64_peak_tflops_nominal": 37.2},
-            "clocks": clocks, "serial_fallbacks": int(st1.serial_fallbacks)}
+                         "fp64_peak_tflops_nominal": 34.0},          # H100 SXM data sheet, FP64 without tensor cores
+            "clocks": clocks, "gpu": gpu_info(0), "serial_fallbacks": int(st1.serial_fallbacks)}
+    if args.dump_outputs:        # what the last step returned: its estimate, and the particles (a seeded sample of 2^20 rows beyond that)
+        parts = g.get_particles()
+        if parts.shape[0] > (1 << 20):
+            parts = parts[np.sort(np.random.default_rng(0).choice(parts.shape[0], size=1 << 20, replace=False))]
+        dump_outputs(args.dump_outputs, {"estimate": est, "covariance": g.calc_covariance(), "particles": parts})
     if not args.no_cpu_baseline:
         sys.path.insert(0, os.path.join(ROOT, "tests"))
         import _oracle
@@ -508,6 +550,8 @@ def main():
                     help="fastslam workload: 1 = FastSLAM 1.0 (the headline), 2 = FastSLAM 2.0 (fastslam2.rs) on the same configurations")
     ap.add_argument("--particles", type=int, default=1 << 20, help="mcl / pf workloads only")
     ap.add_argument("--threshold", type=float, default=1.0, help="pf workload: resample_threshold (1.0 = resample every step)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last step of the timed workload returned as DIR/<name>.npy (float64, < 64 MB in all)")
     args = ap.parse_args()
     global NTH_MODE, VARIANT
     NTH_MODE = args.nth

@@ -11,7 +11,7 @@
  *
  * To make "GPU result == oracle result" a BIT-EXACT statement for every particle, weight and resample
  * index, both sides must evaluate the same correctly-specified arithmetic.  + - * / sqrt and fma are
- * correctly rounded by IEEE-754 on x86-64 and on sm_100a, so every function below is written ONLY in
+ * correctly rounded by IEEE-754 on x86-64 and on sm_90a, so every function below is written ONLY in
  * terms of those operations (explicit fma(), never compiler contraction) plus integer bit manipulation.
  * Build rules that make this hold:
  *     device:  nvcc --fmad=false            (no implicit a*b+c fusion)

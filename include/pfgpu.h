@@ -1,5 +1,5 @@
 /*
- * pfgpu.h — C ABI of the B200-native particle-filter / FastSLAM 1.0 engine (libpfgpu.so).
+ * pfgpu.h — C ABI of the H100-native particle-filter / FastSLAM 1.0 engine (libpfgpu.so).
  *
  * This is the drop-in boundary.  The reference (rsasaki0109/rust_robotics) has no FFI of its own: its
  * boundary is the public Rust API of rust_robotics_localization::{ParticleFilterLocalizer,

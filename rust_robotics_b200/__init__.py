@@ -1,4 +1,4 @@
-"""rust_robotics_b200 — B200-native particle-filter / FastSLAM 1.0 engine behind the rust_robotics API.
+"""rust_robotics_b200 — H100-native particle-filter / FastSLAM 1.0 engine behind the rust_robotics API.
 
 The product is the CUDA library (csrc/ -> libpfgpu.so, C ABI in include/pfgpu.h).  `api` mirrors the
 reference's public types (ParticleFilterLocalizer, MonteCarloLocalizer, fastslam1) over that ABI with

@@ -1,4 +1,4 @@
-"""Builds rust_robotics_b200/libpfgpu.so (sm_100a only) with nvcc.  Used by __graft_entry__.build()."""
+"""Builds rust_robotics_b200/libpfgpu.so (sm_90a, H100) with nvcc.  Used by __graft_entry__.build()."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ SRC = os.path.join(PKG, "csrc", "pfgpu.cu")
 LIB = os.path.join(PKG, "libpfgpu.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--fmad=false",                               # the numerical contract: no implicit a*b+c fusion (pf_contract_math.h)
     "-Xcompiler", "-fPIC,-ffp-contract=off",
@@ -17,9 +17,10 @@ NVCC_FLAGS = [
 
 
 def sources():
+    """everything the library depends on, this file included (a change of the flags above rebuilds it)"""
     d = os.path.join(PKG, "csrc")
     inc = os.path.join(os.path.dirname(PKG), "include")
-    return [os.path.join(d, f) for f in os.listdir(d)] + [os.path.join(inc, f) for f in os.listdir(inc)]
+    return [os.path.join(d, f) for f in os.listdir(d)] + [os.path.join(inc, f) for f in os.listdir(inc)] + [os.path.abspath(__file__)]
 
 
 def needs_build():

@@ -8,7 +8,7 @@
 #include "../../include/pf_contract_math.h"
 
 #ifndef PFGPU_NUM_SMS
-#define PFGPU_NUM_SMS 148          // B200: 2 dies x 74 SMs
+#define PFGPU_NUM_SMS 132          // H100 SXM; ctx_open reads the device's own count
 #endif
 
 extern thread_local char g_pfgpu_err[512];

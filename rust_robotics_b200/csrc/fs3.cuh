@@ -8,7 +8,7 @@
 //                     sum to EVERY rank.
 //   fs3_post_kernel   everything after the per-particle work (fs1.rs:258-265, resample fs1.rs:206-234): exact sequential
 //                     sums S, S2, the CDF (x3_core.h), normalisation, N_eff gate, the comb in closed form, index search,
-//                     pose clone and the lazy clone of the maps — one launch of <= 148 co-resident CTAs that synchronise
+//                     pose clone and the lazy clone of the maps — one launch of at most one co-resident CTA per SM, synchronised
 //                     through a counter in global memory (one such barrier for a step that does not resample, four for one
 //                     that does).  Every rank runs it on ALL n_glob weights (they are 8 B per particle), so the ranks never
 //                     wait for each other inside it.

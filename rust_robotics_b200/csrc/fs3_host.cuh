@@ -19,8 +19,8 @@ struct pfgpu_fs {
     Fs3Rec* h_rec = nullptr;          // pinned + mapped
     double* stage = nullptr; size_t stage_bytes = 0;   // device staging buffer for upload / download / seed_map
     bool pdl = true;
-    bool early = false;               // PFGPU_EARLY_LAUNCH=1: release the dependent kernel at the START of the previous grid (measured: 2 % slower;
-                                      // releasing the next EKF launch when the post kernel's CTAs are through their phases: also 1.7 % slower)
+    bool early = false;               // PFGPU_EARLY_LAUNCH=1: release the dependent kernel at the START of the previous grid (experiment;
+                                      // off by default)
     bool ekf_attr[2] = { false, false };
     int variant = 1;                  // 1 = FastSLAM 1.0 (fs1.rs), 2 = FastSLAM 2.0 (fs2.rs); pfgpu_fs_set_variant
     int ekf_helpers = 0;              // PFGPU_EKF_HELPERS: cap on the helper warps per CTA (0 = as many as fit, at most 3)
@@ -69,13 +69,12 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
     // post kernel shape: <= 128 tiles (one CTA each, co-resident), NT threads x K values
     {
         // below 65 536 weights: up to 128 tiles of 256 threads (latency matters, not throughput); at 65 536: 128 tiles of 512 threads,
-        // one value per thread (measured 1.3 % faster than 256 x 2; fewer, fatter tiles are slower: 64 x 512 x 2 -2 %, 32 x 512 x 4
-        // -13 %); beyond that the per-value phases (classify, normalise, emit: ~100 instructions per value and sum) dominate, so
-        // every SM gets a tile of 512 threads
+        // one value per thread; beyond that the per-value phases (classify, normalise, emit: ~100 instructions per value and sum)
+        // dominate, so every SM gets a tile of 512 threads
         const char* env = getenv("PFGPU_POST_NT");
         const bool big = n_global > (size_t)128 * 256 * 2;
         h->post_nt = env ? (atoi(env) == 512 ? 512 : 256) : (n_global >= (size_t)128 * 512 ? 512 : 256);
-        unsigned want = (unsigned)std::min<int>(big ? 148 : 128, h->ctx.num_sms);
+        unsigned want = (unsigned)std::min<int>(big ? FS3_MAX_TILES : 128, h->ctx.num_sms);
         { const char* ew = getenv("PFGPU_POST_TILES"); if (ew && atoi(ew) >= 1 && atoi(ew) <= (int)want) want = (unsigned)atoi(ew); }   // tests: several values per thread at small n
         unsigned K = (unsigned)((n_global + (size_t)want * h->post_nt - 1) / ((size_t)want * h->post_nt));
         if (K == 0) K = 1;

@@ -5,8 +5,8 @@
 // (pf.rs:337-345, 416-423; MCL resamples every step, mcl.rs:298), build the cumulative weights (pf.rs:448-453; MCL forces the
 // last entry to 1, mcl.rs:334-336), draw one uniform per output slot and search it (pf.rs:456-470, mcl.rs:344-361, 387-392),
 // clone the poses, and refresh the cached estimate + covariance (pf.rs:382-413, 499-503).  Run as separate kernels that is ~21
-// launches of a few microseconds each — the step is launch-latency bound below ~10^5 particles (profiles/r02_sweep).  Here the
-// same arithmetic runs in one kernel of <= 148 co-resident CTAs built on the FastSLAM post kernel's machinery: the exact
+// launches of a few microseconds each — the step is launch-latency bound below ~10^5 particles.  Here the
+// same arithmetic runs in one kernel of <= one co-resident CTA per SM, built on the FastSLAM post kernel's machinery: the exact
 // sequential sums are fs3_xsum (fs3.cuh) over tiles held in shared memory, grid barriers are arrival counters.
 //
 // Bit-exactness: the three sums (S = sum w_raw, Q = sum w^2, the cumulative weights) are the reference's sequential f64 sums,

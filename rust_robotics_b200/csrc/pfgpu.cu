@@ -1,5 +1,5 @@
 // pfgpu.cu — the C ABI of include/pfgpu.h: handles, step orchestration, upload/download.
-// Single translation unit: nvcc -gencode arch=compute_100a,code=sm_100a --fmad=false (see __graft_entry__.build()).
+// Single translation unit: nvcc -gencode arch=compute_90a,code=sm_90a --fmad=false (see __graft_entry__.build()).
 #include "common.cuh"
 #include "xsum.cuh"
 #include "pf_kernels.cuh"
@@ -63,7 +63,7 @@ struct Marks {
     std::vector<cudaEvent_t> ev = std::vector<cudaEvent_t>(PF_MARK_SLOTS, nullptr);
     void* l2buf = nullptr;
     void* l2buf_rd = nullptr;
-    size_t l2bytes = (size_t)256 << 20;      // > 126 MB L2
+    size_t l2bytes = (size_t)256 << 20;      // several times the 50 MB L2
 };
 static int marks_mark(Ctx& ctx, Marks& m, int slot) {
     if (slot < 0 || slot >= PF_MARK_SLOTS) return PFGPU_ERR_INVALID;
@@ -272,8 +272,8 @@ static int pf3_setup(pfgpu_pf* h) {
     const char* e = getenv("PFGPU_PF_FUSED");
     if (e && e[0] == '0') return 0;
     const size_t n = h->d.n;
-    // measured (profiles/r02_sweep): 2.0x at 2^10, 1.4x at 2^14, 1.15x at 2^16, even at 2^18, slower at 2^20 (there the separate
-    // kernels fill the GPU and their launch latency is hidden behind the graph replay)
+    // up to 2^18 particles (H100 SXM at 400 W, resample every step: 1.44x at 2^16, 1.10x at 2^18 against the separate kernels);
+    // beyond that the separate kernels fill the GPU and their launch latency is hidden behind the graph replay
     if (h->world != 1 || h->adaptive || n < 1 || n > ((size_t)1 << 18)) return 0;
     const unsigned NT = 256;
     unsigned tiles = (unsigned)std::min<size_t>((size_t)std::min(h->ctx.num_sms, FS3_MAX_TILES), (n + NT - 1) / NT);
@@ -828,7 +828,7 @@ extern "C" int pfgpu_test_div(unsigned long long n, uint64_t seed, unsigned long
     unsigned long long* d = nullptr;
     PF_CUDA(cudaMalloc(&d, sizeof(*d)));
     PF_CUDA(cudaMemset(d, 0, sizeof(*d)));
-    pf_test_div_kernel<<<148 * 8, 256>>>(n, seed, d);
+    pf_test_div_kernel<<<PFGPU_NUM_SMS * 8, 256>>>(n, seed, d);
     PF_CUDA(cudaDeviceSynchronize());
     PF_CUDA(cudaMemcpy(mismatches, d, sizeof(*d), cudaMemcpyDeviceToHost));
     cudaFree(d);
