@@ -30,7 +30,7 @@ extern "C" {
 
 #define PFGPU_OK                 0
 #define PFGPU_ERR_INVALID      (-1)   /* RoboticsError::InvalidParameter                       */
-#define PFGPU_ERR_UNSUPPORTED  (-2)   /* valid in the reference, not built here (KLD-adaptive MCL on more than one GPU, > 1024 landmarks, ...) */
+#define PFGPU_ERR_UNSUPPORTED  (-2)   /* valid in the reference, not built here (KLD-adaptive MCL on more than one GPU, ...) */
 #define PFGPU_ERR_NO_DEVICE     1000  /* no CUDA device / extension cannot run: fail loudly      */
 #define PFGPU_ERR_CUDA          1001
 #define PFGPU_ERR_NCCL          1002
@@ -107,7 +107,8 @@ typedef struct { double d, angle; uint64_t lm_id; } pfgpu_fs_obs;
 typedef struct pfgpu_fs pfgpu_fs;
 
 void pfgpu_fs_default_config(pfgpu_fs_config* cfg);
-/* create_particles(n, m) fs1.rs:302-306 */
+/* create_particles(n, m) fs1.rs:302-306.  0 <= n_landmarks <= 65536 (this and both sharded create calls); more returns
+ * PFGPU_ERR_UNSUPPORTED with a message in pfgpu_last_error. */
 int  pfgpu_fs_create(const pfgpu_fs_config* cfg, size_t n_particles, size_t n_landmarks, uint64_t seed,
                      int device, pfgpu_fs** out);
 /* Sharded over `world` (<= 8) GPUs of one NVLink domain, one process per GPU; collective over all ranks (same arguments

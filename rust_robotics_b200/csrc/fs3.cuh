@@ -45,6 +45,10 @@
 #define FS3_ENT_CAP 512           // dirty values itemised per sum (more: that sum takes the serial walk)
 #define FS3_SLOTS 5               // S, Q (border only), S2, cdf, comb (n not a power of two)
 #define FS3_SPIN_LIMIT (1u << 27)
+#define FS3_MAX_LM 65536          // landmarks per particle: row ids (< m) fit the u16 row list
+
+__host__ __device__ __forceinline__ unsigned fs3_bm_words(unsigned m) { return (m + 31u) / 32u; }
+__host__ __device__ __forceinline__ unsigned fs3_bm_ld(unsigned m) { return fs3_bm_words(m) + FS3_MAX_TILES; }
 
 struct Fs3Obs { double d, angle; int lm_id; int pad; };
 struct Fs3ObsParam { Fs3Obs o[32]; };
@@ -97,6 +101,8 @@ struct Fs3Dev {
     unsigned long long* resTP; unsigned* resKey; unsigned long long* resP; double* resAft;   // [8][tiles] / [8][FS3_ENT_CAP] for the scans
     double* tileEnd;                                           // [FS3_MAX_TILES] last CDF value of every tile (coarse level of the index search)
     unsigned short* rowlist; int* rowinfo;                     // live ancestry rows ([m]), [0] their count, [1] new row id or -1
+    unsigned* rowbm;                                           // [2][fs3_bm_ld(m)] by step parity: live-row bitmap ([ceil(m/32)] words),
+                                                               // then one "has an identity landmark" flag per post-kernel CTA
     double* tileBw; unsigned* tileBi;         // [FS3_MAX_TILES] best (weight, global slot) per tile
     int* flagsg;                              // [FS3_SLOTS] "bad value seen" per sum (reset by the post kernel's last CTA)
     Fs3Rec* rec;
@@ -452,12 +458,6 @@ __global__ void fs3_signal_kernel(const __grid_constant__ Fs3Dev d, int which, u
     pf_grid_dep_sync();
     fs3_signal_peers(d, which, value);
 }
-__device__ __forceinline__ void fs3_mark_updated_warp(const Fs3Dev& d, const Fs3ObsParam& po, int k_obs, int lane) {
-    for (int j = lane; j < k_obs; j += 32) {
-        const int l = po.o[j].lm_id, s = d.lmst[l];
-        if (s >> 1) d.lmst[l] = (s & 1) ^ 1;
-    }
-}
 __global__ void fs3_mark_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3ObsParam po, int k_obs) {
     pf_grid_dep_sync();
     fs3_mark_updated(d, po, k_obs);
@@ -482,7 +482,7 @@ struct Fs3Sh {
     unsigned long long Ptot;
     int D, fail, last;
     unsigned jr[2];
-    unsigned rowbits[32];                                     // bitmap of the live ancestry rows (CTA 0)
+    unsigned rowscan[2][NT / 32];                             // row-list compaction (CTA 0): live rows / first free row per warp
     double tend[FS3_MAX_TILES];                               // last CDF value of every tile
     x3_comb_table comb;
 };
@@ -592,10 +592,103 @@ __device__ __noinline__ void fs3_serial_walk(const Fs3Dev& d, Fs3Sh<NT>& sh, uns
 __device__ __noinline__ int fs3_classify(double v, double a0, double a1, unsigned m32, unsigned long long* inc, int* lvl) {
     return x3_classify(v, a0, a1, m32, inc, lvl);            // one copy of the code for the three passes of fs3_xsum
 }
-// Work that hides inside the first exact sum of a launch, on warps that would otherwise sleep at a block barrier while warp 0
-// waits for the grid and evaluates the chain: the lazy-clone bookkeeping + live-row list (CTA 0), the comb table, and the
-// N(0,1) pairs of the next predict.
-struct Fs3Hook { unsigned long long comb_n; uint64_t seed; uint32_t noise_call; int k_last; const Fs3ObsParam* po; };
+// Work that hides inside an exact sum, on warps that would otherwise sleep at a block barrier while warp 0 waits for the grid
+// and evaluates the chain.  First sum of a launch: the lazy-clone bookkeeping of every CTA's landmark slice, the comb table and
+// the N(0,1) pairs of the next predict.  CDF sum of a resample (compact = 1): the live-row list, in CTA 0.
+struct Fs3Hook { unsigned long long comb_n; uint64_t seed; uint32_t noise_call; int k_last; const Fs3ObsParam* po; int par; int compact; };
+
+// Landmarks [lo, hi) belong to post-kernel CTA b: it applies their marks, records their rows and retargets them at a resample.
+__device__ __forceinline__ void fs3_lm_slice(const Fs3Dev& d, unsigned b, unsigned nt, unsigned* lo, unsigned* hi) {
+    const unsigned per = (d.m + nt - 1) / nt;
+    *lo = min(d.m, b * per); *hi = min(d.m, *lo + per);
+}
+// Threads 32 .. NT-1 of CTA b.  (1) The lazy-clone bookkeeping of the EKF launch that just ran, for this CTA's landmarks: those it
+// updated through a row now live in own columns of the other buffer.  (2) One bit per row some landmark of the slice still reads
+// through, OR-ed into the live-row bitmap of this step's parity, and this CTA's "has an identity landmark" flag.  (3) This CTA's
+// share of the OTHER parity's bitmap and its flag are zeroed for the next step (nobody reads them in this launch).
+// Thread h owns landmarks lo + h, lo + h + NH, ...; it applies the marks of its own landmarks, so it reads back its own stores.
+template <int NT>
+__device__ __forceinline__ void fs3_row_scan(const Fs3Dev& d, const Fs3ObsParam& po, int k_last, int par, unsigned b, unsigned nt) {
+    constexpr unsigned NH = NT - 32;
+    const unsigned h = threadIdx.x - 32u, lane = threadIdx.x & 31u;
+    const unsigned W = fs3_bm_words(d.m), ldb = fs3_bm_ld(d.m);
+    unsigned* bm = d.rowbm + (size_t)par * ldb;
+    unsigned* bmo = d.rowbm + (size_t)(par ^ 1) * ldb;
+    unsigned lo, hi;
+    fs3_lm_slice(d, b, nt, &lo, &hi);
+#pragma unroll 1
+    for (int j = 0; j < k_last; ++j) {
+        const unsigned l = (unsigned)po.o[j].lm_id;
+        if (l >= lo && l < hi && (l - lo) % NH == h) { const int s = d.lmst[l]; if (s >> 1) d.lmst[l] = (s & 1) ^ 1; }
+    }
+    {
+        const unsigned wper = (W + nt - 1) / nt, w0 = min(W, b * wper), w1 = min(W, w0 + wper);
+#pragma unroll 1
+        for (unsigned w = w0 + h; w < w1; w += NH) bmo[w] = 0u;
+        if (h == 0) bmo[W + b] = 0u;
+    }
+    // consecutive landmarks mostly share a row: a thread ORs its bits per bitmap word and stores a word only when it changes,
+    // and a warp whose lanes all ended on the same word stores it once
+    unsigned cw = 0xFFFFFFFFu, acc = 0u;
+    int ident = 0;
+#pragma unroll 4
+    for (unsigned l = lo + h; l < hi; l += NH) {
+        const int s = d.lmst[l];
+        if (s >> 1) {
+            const unsigned r = (unsigned)((s >> 1) - 1), w = r >> 5;
+            if (w != cw) { if (acc) atomicOr(bm + cw, acc); cw = w; acc = 0u; }
+            acc |= 1u << (r & 31u);
+        } else ident = 1;
+    }
+    const unsigned has = __ballot_sync(0xffffffffu, acc != 0u);
+    if (has) {
+        const unsigned src = (unsigned)__ffs(has) - 1u;
+        const unsigned wl = __shfl_sync(0xffffffffu, cw, src);
+        if (__all_sync(0xffffffffu, acc == 0u || cw == wl)) {
+            const unsigned all = __reduce_or_sync(0xffffffffu, acc);
+            if (lane == src) atomicOr(bm + wl, all);
+        } else if (acc) atomicOr(bm + cw, acc);
+    }
+    if (__any_sync(0xffffffffu, ident) && lane == 0) bm[W + b] = 1u;
+}
+// Threads 32 .. NT-1 of CTA 0, on a resample step, after every CTA's fs3_row_scan of this step is visible: the bitmap compacted
+// into rowlist (ascending row ids), rowinfo[0] = their count, rowinfo[1] = the row the identity landmarks get (the first free id:
+// with an identity landmark at most m - 1 rows are live) or -1 when there is none.  Block-wide scan over the NT - 32 threads.
+template <int NT>
+__device__ __forceinline__ void fs3_row_compact(const Fs3Dev& d, Fs3Sh<NT>& sh, int par, unsigned nt) {
+    constexpr unsigned NH = NT - 32;
+    const unsigned h = threadIdx.x - 32u, lane = threadIdx.x & 31u, wh = h >> 5;
+    const unsigned W = fs3_bm_words(d.m);
+    const unsigned* bm = d.rowbm + (size_t)par * fs3_bm_ld(d.m);
+    const unsigned per = (W + NH - 1) / NH, w0 = min(W, h * per), w1 = min(W, w0 + per);
+    int cnt = 0;
+    unsigned ff = 0xFFFFFFFFu;                                 // first free row id among my words
+#pragma unroll 1
+    for (unsigned w = w0; w < w1; ++w) {
+        const unsigned x = __ldcg(bm + w);
+        cnt += __popc(x);
+        if (ff == 0xFFFFFFFFu && ~x) ff = w * 32u + (unsigned)__ffs(~x) - 1u;
+    }
+    int incl = cnt;
+#pragma unroll 1
+    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane >= o) incl += y; }
+    const unsigned wff = __reduce_min_sync(0xffffffffu, ff);
+    if (lane == 31) { sh.rowscan[0][wh] = (unsigned)incl; sh.rowscan[1][wh] = wff; }
+    int any = 0;
+    if (wh == 0) {
+#pragma unroll 1
+        for (unsigned t = lane; t < nt; t += 32) any |= __ldcg(bm + W + t) != 0u ? 1 : 0;
+        any = __any_sync(0xffffffffu, any);
+    }
+    asm volatile("bar.sync 1, %0;" :: "r"(NH) : "memory");    // the hook warps only: warp 0 is busy with the chain
+    unsigned pos = (unsigned)(incl - cnt), tot = 0, mf = 0xFFFFFFFFu;
+#pragma unroll 1
+    for (unsigned v = 0; v < NH / 32; ++v) { const unsigned c = sh.rowscan[0][v]; if (v < wh) pos += c; tot += c; mf = min(mf, sh.rowscan[1][v]); }
+#pragma unroll 1
+    for (unsigned w = w0; w < w1; ++w)
+        for (unsigned x = __ldcg(bm + w); x; x &= x - 1) d.rowlist[pos++] = (unsigned short)(w * 32u + (unsigned)__ffs(x) - 1u);
+    if (h == 0) { d.rowinfo[0] = (int)tot; d.rowinfo[1] = any ? (int)mf : -1; }
+}
 
 // One exact sequential sum over the n_glob values held tile-wise in shared memory (thread t owns values t*K .. t*K+K-1 of its
 // tile, stored at vals[k*NT + t]).  toff = approximate sum of everything in front of this tile.  Returns the exact total
@@ -665,40 +758,13 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
     // ---- grid barrier + chain.  The LAST CTA to arrive evaluates the chain (every aggregate is published by then and it reads
     // them uncontended: 128 CTAs fetching the same few sectors at once serialise in L2) and publishes the results; the others
     // wait for its flag.  Warp 0 only; the other warps wait at the block barrier below. ----
-    if (hook && tid >= 32) {
+    if (hook && tid >= 32 && hook->compact) {
+        // the live-row list of this resample.  Every CTA's fs3_row_scan (in the first sum) is ordered before its arrival at the
+        // S2 sum's barrier, which this CTA has passed; the other CTAs read the list only after the grid barriers behind this sum.
+        if (b == 0) fs3_row_compact<NT>(d, sh, hook->par, nt);
+    } else if (hook && tid >= 32) {
+        fs3_row_scan<NT>(d, *hook->po, hook->k_last, hook->par, b, nt);
         if (tid < 64) {                            // warp 1
-            if (b == 0) {
-                // lazy-clone bookkeeping of the EKF launch that just ran, then the rows a resample would have to compose: one bit per
-                // row some landmark still reads through; the identity landmarks would get ONE new row (the first free id: with an
-                // identity landmark at most m - 1 rows are live).  Other CTAs read the list only after >= 3 grid barriers.
-                unsigned* s_bits = sh.rowbits;
-                fs3_mark_updated_warp(d, *hook->po, hook->k_last, lane);
-                __syncwarp();
-                int any_ident = 0;
-                s_bits[lane] = 0u;                                       // 32-word bitmap of the live rows (m <= 1024)
-                __syncwarp();
-#pragma unroll 1
-                for (unsigned l = lane; l < d.m; l += 32) {
-                    const int st_l = d.lmst[l];
-                    if (st_l >> 1) { const unsigned r = (unsigned)((st_l >> 1) - 1); atomicOr(&s_bits[r >> 5], 1u << (r & 31)); } else any_ident = 1;
-                }
-                any_ident = __any_sync(0xffffffffu, any_ident);
-                __syncwarp();
-                const unsigned bits = s_bits[lane];
-                const int cntb = __popc(bits);
-                int incl = cntb;
-#pragma unroll 1
-                for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += y; }
-                int pos = incl - cntb;
-#pragma unroll 1
-                for (unsigned x = bits; x; x &= x - 1) d.rowlist[pos++] = (unsigned short)(lane * 32 + __ffs(x) - 1);
-                const unsigned fr = ~bits;
-                const unsigned has = __ballot_sync(0xffffffffu, fr != 0u);
-                if (lane == 31) d.rowinfo[0] = incl;
-                if (lane == 0) d.rowinfo[1] = -1;
-                __syncwarp();
-                if (any_ident && lane == __ffs(has) - 1) d.rowinfo[1] = lane * 32 + __ffs(fr) - 1;
-            }
             if (hook->comb_n && lane == 0) x3_comb_build(&sh.comb, r0, inv, (double)hook->comb_n, hook->comb_n);
         } else {                                   // warps 2..: the N(0,1) pairs of the next predict for this CTA's share of the local slots
             const unsigned per = (d.n + nt - 1) / nt, t_lo = b * per, t_hi = min(d.n, t_lo + per);
@@ -981,6 +1047,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     // ---------------- S = sum w_raw (normalize_weights fs1.rs:196-203) ----------------
     Fs3Hook hook;
     hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.noise_call = step + 1u; hook.k_last = k_last; hook.po = &po;
+    hook.par = par; hook.compact = 0;
     const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, m32, nullptr, par, 0.0, r0, inv, q, &hook);
     FS3_TRACE(1);
     // w = w_raw / S; best particle of the tile (LAST maximum, fs1.rs:269-274)
@@ -1048,7 +1115,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         }
         // ---------------- cum_sum fs1.rs:213-216 ----------------
         const double toff3 = S2 > 0.0 ? fs3_div(toff2, S2) : toff2;
-        (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0);
+        hook.compact = 1;
+        (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, &hook);
         FS3_TRACE(4);
         // ---------------- the comb r, r + 1/n, ... accumulated sequentially (fs1.rs:219-230) ----------------
         if (log2n < 0) {                                       // n not a power of two: every add rounds -> exact scan
@@ -1058,13 +1126,18 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             __syncthreads();
             (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff4, 4, 3, m32, d.rcomb_all, par, S2, r0, inv, 0.0);
         }
+        // this CTA's landmark slice (only this CTA writes it, in the first sum): its first entries are loaded in front of the barrier,
+        // so the retarget behind the index walk does not wait for them
+        unsigned lm_lo, lm_hi;
+        fs3_lm_slice(d, b, nt, &lm_lo, &lm_hi);
+        const int s_first = lm_lo + tid < lm_hi ? d.lmst[lm_lo + tid] : 0;
         fs3_grid_sync<NT>(d, 4, nt);                           // the whole CDF (and comb) is visible
         FS3_TRACE(5);
         // ---------------- index walk, pose clone, lazy map clone for this CTA's share of the local slots ----------------
         // j_t = first j with c_j >= r_t, clamped to n - 1: "while r > cum_sum[j+1] && j < n-1 { j += 1 }" (fs1.rs:224-226) with r and
         // j both non-decreasing over the slots.  The CTA's first and last slot bracket all of its answers; the bracketed piece of
         // the CDF is staged in shared memory (it is about as long as the slot range) and every slot searches there.
-        const int nrows = d.rowinfo[0], newrow = d.rowinfo[1];
+        const int nrows = __ldcg(d.rowinfo), newrow = __ldcg(d.rowinfo + 1);     // (fs3_row_compact, in CTA 0 during the CDF sum)
         const int cur = st->cur, rcur = st->rcur;
         const unsigned per = (d.n + nt - 1) / nt;              // local slots per CTA
         const unsigned t_lo = b * per, t_hi = min(d.n, t_lo + per);
@@ -1153,6 +1226,13 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
                 }
             }
         }
+        if (newrow >= 0) {     // the identity landmarks of this CTA's slice now read through the new row (every scan of lmst is over)
+#pragma unroll 1
+            for (unsigned l = lm_lo + tid; l < lm_hi; l += NT) {
+                const int s = l == lm_lo + tid ? s_first : d.lmst[l];
+                if ((s >> 1) == 0) d.lmst[l] = (s & 1) | ((newrow + 1) << 1);
+            }
+        }
         FS3_TRACE(6);
     }
     // ---------------- completion: the last CTA flips the state, writes the record, tells the peers ----------------
@@ -1161,11 +1241,6 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     __syncthreads();
     if (!sh.last) return;
     if (d.trace && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); d.trace[40] += t - d.trace[39]; }   // [40] the last CTA is through
-    if (gate) {
-        const int newrow = d.rowinfo[1];
-#pragma unroll 1
-        for (unsigned l = tid; l < d.m; l += NT) { const int s = d.lmst[l]; if ((s >> 1) == 0) d.lmst[l] = (s & 1) | ((newrow + 1) << 1); }
-    }
     if (tid < FS3_SLOTS) { d.flagsg[tid] = 0; d.entCnt[tid] = 0u; }
     if (tid < 8) { d.bar[tid] = 0u; d.resflag[tid] = 0u; }
     if (tid < 32) {
@@ -1271,13 +1346,15 @@ __global__ void __launch_bounds__(256) fs3_seed_pose_kernel(const __grid_constan
 }
 __global__ void __launch_bounds__(256) fs3_seed_lm_kernel(const __grid_constant__ Fs3Dev d, const double* lm_xy, double sigma, double cov0, uint64_t seed) {
     const unsigned i = blockIdx.x * 256u + threadIdx.x;
-    const size_t l = blockIdx.y;
     if (i >= d.n) return;
-    double z0, z1;
-    pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_INIT_A, 0, ((uint64_t)d.off + i) * d.m + l), &z0, &z1);
-    double* p = d.lm[0] + l * 6 * d.ld + i;
-    p[0] = lm_xy[2 * l] + sigma * z0; p[d.ld] = lm_xy[2 * l + 1] + sigma * z1;
-    p[2 * (size_t)d.ld] = cov0; p[3 * (size_t)d.ld] = 0.0; p[4 * (size_t)d.ld] = 0.0; p[5 * (size_t)d.ld] = cov0;
+#pragma unroll 1
+    for (size_t l = blockIdx.y; l < d.m; l += gridDim.y) {      // (gridDim.y is at most 65 535)
+        double z0, z1;
+        pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_INIT_A, 0, ((uint64_t)d.off + i) * d.m + l), &z0, &z1);
+        double* p = d.lm[0] + l * 6 * d.ld + i;
+        p[0] = lm_xy[2 * l] + sigma * z0; p[d.ld] = lm_xy[2 * l + 1] + sigma * z1;
+        p[2 * (size_t)d.ld] = cov0; p[3 * (size_t)d.ld] = 0.0; p[4 * (size_t)d.ld] = 0.0; p[5 * (size_t)d.ld] = cov0;
+    }
 }
 
 // get_observations fs1.rs:277-299 (the simulator next to the filter): landmarks within max_range of the true pose, in

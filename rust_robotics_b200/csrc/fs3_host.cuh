@@ -53,7 +53,7 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
     if (!out) return PFGPU_ERR_INVALID;
     *out = nullptr;
     if (!cfg || n == 0 || n_global >= (1ull << 28) * (size_t)world || n >= (1ull << 28) || n_global > 0xFFFFFFF0ull) return PFGPU_ERR_INVALID;
-    if (m > 1024) { snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "more than 1024 landmarks per particle are not supported"); return PFGPU_ERR_UNSUPPORTED; }
+    if (m > FS3_MAX_LM) { snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "more than %d landmarks per particle are not supported", FS3_MAX_LM); return PFGPU_ERR_UNSUPPORTED; }
     if (world > 1 && n % 64 != 0) { snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "sharded FastSLAM needs a multiple of 64 particles per GPU"); return PFGPU_ERR_UNSUPPORTED; }
     pfgpu_fs* h = new (std::nothrow) pfgpu_fs();
     if (!h) return PFGPU_ERR_CUDA;
@@ -139,8 +139,10 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         FS_TRY(cudaMalloc(&d.resKey, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned))); FS_TRY(cudaMalloc(&d.resP, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned long long)));
         FS_TRY(cudaMalloc(&d.resAft, (size_t)8 * FS3_ENT_CAP * sizeof(double)));
         FS_TRY(cudaMalloc(&d.tileEnd, FS3_MAX_TILES * sizeof(double)));
-        FS_TRY(cudaMalloc(&d.rowlist, 1024 * sizeof(unsigned short))); FS_TRY(cudaMalloc(&d.rowinfo, 2 * sizeof(int)));
+        FS_TRY(cudaMalloc(&d.rowlist, mm * sizeof(unsigned short))); FS_TRY(cudaMalloc(&d.rowinfo, 2 * sizeof(int)));
         FS_TRY(cudaMemset(d.rowinfo, 0, 2 * sizeof(int)));
+        const size_t nbm = (size_t)2 * fs3_bm_ld((unsigned)m);       // both parities start clear; each post kernel clears the other
+        FS_TRY(cudaMalloc(&d.rowbm, nbm * sizeof(unsigned))); FS_TRY(cudaMemset(d.rowbm, 0, nbm * sizeof(unsigned)));
         FS_TRY(cudaMalloc(&d.tileBw, FS3_MAX_TILES * sizeof(double))); FS_TRY(cudaMalloc(&d.tileBi, FS3_MAX_TILES * sizeof(unsigned)));
         FS_TRY(cudaMalloc(&d.flagsg, 8 * sizeof(int))); FS_TRY(cudaMemset(d.flagsg, 0, 8 * sizeof(int)));
         FS_TRY(cudaHostAlloc(&h->h_rec, sizeof(Fs3Rec), cudaHostAllocMapped));
@@ -237,7 +239,7 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(h->arena);
     cudaFree(d.st); cudaFree(d.lmst); cudaFree(d.w); cudaFree(d.nz[0]); cudaFree(d.nz[1]); cudaFree(d.wn_all); cudaFree(d.cum_all); cudaFree(d.rcomb_all); cudaFree(d.idx);
     cudaFree(d.tileP); cudaFree(d.tileQ); cudaFree(d.entCnt); cudaFree(d.entKey); cudaFree(d.entTile); cudaFree(d.entP); cudaFree(d.entV); cudaFree(d.entL);
-    cudaFree(d.bar); cudaFree(d.rowlist); cudaFree(d.rowinfo); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
+    cudaFree(d.bar); cudaFree(d.rowlist); cudaFree(d.rowinfo); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
     cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->stage);
     if (h->h_rec) cudaFreeHost(h->h_rec);
@@ -329,7 +331,7 @@ extern "C" int pfgpu_fs_seed_map(pfgpu_fs* h, const double pose3[3], const doubl
         int rc = fs_stage(h, m * 2 * sizeof(double));
         if (rc) return rc;
         PF_CUDA(cudaMemcpyAsync(h->stage, lm_xy, m * 2 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
-        dim3 grid(cdiv_u(d.n, 256), (unsigned)m);
+        dim3 grid(cdiv_u(d.n, 256), (unsigned)std::min<size_t>(m, 65535));
         PF_LAUNCH(h->ctx, fs3_seed_lm_kernel, grid, 256, 0, d, h->stage, sigma, cov0, h->seed);
         PF_LAUNCH(h->ctx, fs3_lmst_reset_kernel, 1, 256, 0, d);
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));

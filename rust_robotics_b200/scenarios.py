@@ -72,6 +72,12 @@ def c4_scenario(steps=55, seed=42):
     return FastSlamScenario(32, (155.0, 55.0, 0.0), (1.0, 0.01), steps, seed)
 
 
+def bigmap_scenario(steps=110, seed=42):
+    """16 384 landmarks (128 x 128 grid, 10 m pitch) with C3's 40 m circle moved to the middle of the grid: the robot sits at the
+    same offset from the grid lines as in C3, so it observes the same ~12.7 landmarks per step"""
+    return FastSlamScenario(128, (635.0, 595.0, 0.0), (1.0, 0.025), steps, seed)
+
+
 class PfScenario:
     """C1: the scenario of crates/rust_robotics/examples/render_gif_particle_filter.rs:21-79 (5 landmarks, rounded
     rectangle drive, obs = max(range + N(0, 0.15), 0)); C2: 360 landmarks on a 30 m circle, u = (1.0, 0.03)."""
