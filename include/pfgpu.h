@@ -180,7 +180,8 @@ typedef struct {
 } pfgpu_stats;
 int  pfgpu_pf_stats(pfgpu_pf*, pfgpu_stats*);
 int  pfgpu_fs_stats(pfgpu_fs*, pfgpu_stats*);
-/* debug (PFGPU_POST_TRACE=1): accumulated per-phase times [ns] of the fused post-step kernel; out32[31] = launches */
+/* debug (PFGPU_POST_TRACE=1): accumulated per-phase times [ns] of the fused post-step kernel; out32[31] = launches,
+   out32[11] = resamples that ran the exact S2 and CDF sums instead of the certified CDF (counted with or without the trace) */
 int  pfgpu_fs_post_trace(pfgpu_fs*, unsigned long long* out32);
 /* how the coupled part of the step runs: 0 = one GPU, 2 = sharded over peer memory (NVLink loads / stores inside the kernels;
    no NCCL call and no host sync per step) */

@@ -9,8 +9,8 @@
 //   fs3_post_kernel   everything after the per-particle work (fs1.rs:258-265, resample fs1.rs:206-234): exact sequential
 //                     sums S, S2, the CDF (x3_core.h), normalisation, N_eff gate, the comb in closed form, index search,
 //                     pose clone and the lazy clone of the maps — one launch of at most one co-resident CTA per SM, synchronised
-//                     through a counter in global memory (one such barrier for a step that does not resample, four for one
-//                     that does).  Every rank runs it on ALL n_glob weights (they are 8 B per particle), so the ranks never
+//                     through a counter in global memory (one such barrier for a step that does not resample, two for one
+//                     that resamples from the certified CDF, four or five for one that runs the exact S2 and CDF sums).  Every rank runs it on ALL n_glob weights (they are 8 B per particle), so the ranks never
 //                     wait for each other inside it.
 //
 // HBM layout per rank (n local particles, column stride ld = n rounded up to 64, m landmarks):
@@ -46,6 +46,10 @@
 #define FS3_SLOTS 5               // S, Q (border only), S2, cdf, comb (n not a power of two)
 #define FS3_SPIN_LIMIT (1u << 27)
 #define FS3_MAX_LM 65536          // landmarks per particle: row ids (< m) fit the u16 row list
+#define FS3_ROW_CHUNK 1024        // live rows a post-kernel CTA lists in shared memory at a time (more: several passes)
+#define FS3_CERT_FLAG FS3_SLOTS   // flagsg[FS3_CERT_FLAG]: some CTA could not certify its piece of the CDF
+#define FS3_CERT_MAX_LOG2N 16     // certified CDF up to 2^16 particles: about 4 n^3 2^-53 comb values fall within its bound of a
+                                  // CDF value, 1/8 at 2^16, 1 at 2^17, 64 at 2^19 (where it would almost always be refused)
 
 __host__ __device__ __forceinline__ unsigned fs3_bm_words(unsigned m) { return (m + 31u) / 32u; }
 __host__ __device__ __forceinline__ unsigned fs3_bm_ld(unsigned m) { return fs3_bm_words(m) + FS3_MAX_TILES; }
@@ -61,6 +65,7 @@ struct Fs3State {                 // device-resident; written by the last CTA of
     unsigned bar_count, bar_gen;  // grid barrier of the post kernel
     int err;                      // sticky: 1 = a barrier or a peer flag timed out
     int serial_walks, cert_fail, dirty_last, border_cnt;
+    int cdf_exact;                // resamples that ran the exact S2 and CDF sums (certificate refused, or not applicable)
     unsigned noise_call;          // nz[] holds the predict noise of EKF call `noise_call - 1` (0: none); written by the post kernel
     double S, Q, neff, S2, r0;
 };
@@ -78,6 +83,7 @@ struct Fs3Dev {
     int wait_inline;                          // 1: kernels spin on the peers' flags themselves; 0: the host launches fs3_wait_kernel
                                               // in front of them (ranks sharing one GPU must not hold SMs while they wait)
     unsigned npart;                           // partial sums per rank (= ld / 64)
+    int exact_cdf;                            // 1: every resample runs the exact S2 and CDF sums (PFGPU_FS_EXACT_CDF=1)
     Fs3State* st;
     int* lmst;                                // [m]
     char* peer[FS3_MAXG];                     // arena base of every rank (peer[rank] = own)
@@ -89,7 +95,7 @@ struct Fs3Dev {
     double* nz[2];                            // [ld] each: N(0,1) pair of every local slot for the NEXT predict (fs1.rs:129-130), precomputed
                                               // by idle warps of the post kernel (it depends on seed, call and slot only)
     double* wn_all;                           // [n_glob] normalised weights of all slots (post-kernel scratch, fallback walks)
-    double* cum_all;                          // [n_glob] exact CDF
+    double* cum_all;                          // [n_glob] CDF of the resample: certified fl(P_j / S), or the exact one
     double* rcomb_all;                        // [n_glob] exact comb (only when n_glob is not a power of two)
     unsigned* idx;                            // [ld] global ancestor of local slot t at the last resample
     unsigned long long* tileP; double* tileQ;                  // [FS3_SLOTS][FS3_MAX_TILES] clean-increment sum per tile; [tiles] sum w_raw^2
@@ -100,11 +106,10 @@ struct Fs3Dev {
     Fs3Res* res;                                               // [8] its results: total, entry count, failure
     unsigned long long* resTP; unsigned* resKey; unsigned long long* resP; double* resAft;   // [8][tiles] / [8][FS3_ENT_CAP] for the scans
     double* tileEnd;                                           // [FS3_MAX_TILES] last CDF value of every tile (coarse level of the index search)
-    unsigned short* rowlist; int* rowinfo;                     // live ancestry rows ([m]), [0] their count, [1] new row id or -1
     unsigned* rowbm;                                           // [2][fs3_bm_ld(m)] by step parity: live-row bitmap ([ceil(m/32)] words),
                                                                // then one "has an identity landmark" flag per post-kernel CTA
     double* tileBw; unsigned* tileBi;         // [FS3_MAX_TILES] best (weight, global slot) per tile
-    int* flagsg;                              // [FS3_SLOTS] "bad value seen" per sum (reset by the post kernel's last CTA)
+    int* flagsg;                              // [FS3_SLOTS + 1] "bad value seen" per sum, then the certificate flag (reset by the post kernel's last CTA)
     Fs3Rec* rec;
     unsigned long long* trace;                // optional [32] phase timestamps (PFGPU_POST_TRACE)
 };
@@ -480,9 +485,10 @@ struct Fs3Sh {
     double bef[FS3_ENT_CAP], aft[FS3_ENT_CAP];                // exact sum in front of / right after each dirty value
     double total, tbase, bcast;
     unsigned long long Ptot;
-    int D, fail, last;
+    int D, fail, last, lead, rany;
     unsigned jr[2];
-    unsigned rowscan[2][NT / 32];                             // row-list compaction (CTA 0): live rows / first free row per warp
+    unsigned rowscan[2][NT / 32];                             // live-row list: live rows / first free row per warp
+    unsigned short rowl[FS3_ROW_CHUNK];                       // live rows [base, base + FS3_ROW_CHUNK) of the ascending list
     double tend[FS3_MAX_TILES];                               // last CDF value of every tile
     x3_comb_table comb;
 };
@@ -594,8 +600,13 @@ __device__ __noinline__ int fs3_classify(double v, double a0, double a1, unsigne
 }
 // Work that hides inside an exact sum, on warps that would otherwise sleep at a block barrier while warp 0 waits for the grid
 // and evaluates the chain.  First sum of a launch: the lazy-clone bookkeeping of every CTA's landmark slice, the comb table and
-// the N(0,1) pairs of the next predict.  CDF sum of a resample (compact = 1): the live-row list, in CTA 0.
-struct Fs3Hook { unsigned long long comb_n; uint64_t seed; uint32_t noise_call; int k_last; const Fs3ObsParam* po; int par; int compact; };
+// the N(0,1) pairs of the next predict.
+struct Fs3Hook { unsigned long long comb_n; uint64_t seed; uint32_t noise_call; int k_last; const Fs3ObsParam* po; int par; };
+// what fs3_xsum_emit needs of a thread's pass through fs3_xsum: approximate prefix in front of its first value, clean-increment
+// sum in front of it inside the tile, and the binade of its run (-1: classified value by value)
+struct Fs3Run { double a_first; unsigned long long Pex; int e_run; };
+// the certificate of a CDF emitted as fl(P_j / S) (DESIGN §1): comb r0 + t inv, t < n = 2^p; dl, ab: relative and absolute bound
+struct Fs3Cert { double S, r0, inv, ninv, dl, ab; unsigned long long n; };
 
 // Landmarks [lo, hi) belong to post-kernel CTA b: it applies their marks, records their rows and retargets them at a resample.
 __device__ __forceinline__ void fs3_lm_slice(const Fs3Dev& d, unsigned b, unsigned nt, unsigned* lo, unsigned* hi) {
@@ -651,52 +662,67 @@ __device__ __forceinline__ void fs3_row_scan(const Fs3Dev& d, const Fs3ObsParam&
     }
     if (__any_sync(0xffffffffu, ident) && lane == 0) bm[W + b] = 1u;
 }
-// Threads 32 .. NT-1 of CTA 0, on a resample step, after every CTA's fs3_row_scan of this step is visible: the bitmap compacted
-// into rowlist (ascending row ids), rowinfo[0] = their count, rowinfo[1] = the row the identity landmarks get (the first free id:
-// with an identity landmark at most m - 1 rows are live) or -1 when there is none.  Block-wide scan over the NT - 32 threads.
+// Every thread of a CTA, on a resample step, behind a grid barrier that follows every CTA's fs3_row_scan of this step: the live
+// rows of the bitmap in ascending order.  Thread t owns bitmap words [t per, t per + per) (per <= 8: m <= 65 536, NT >= 256).
+// fs3_row_count: *pos = the position of the thread's first live row in that order, *nrows = how many rows are live, *newrow = the
+// row the identity landmarks get (the first free id: with an identity landmark at most m - 1 rows are live) or -1 when there is
+// none.  Contains one block barrier.
 template <int NT>
-__device__ __forceinline__ void fs3_row_compact(const Fs3Dev& d, Fs3Sh<NT>& sh, int par, unsigned nt) {
-    constexpr unsigned NH = NT - 32;
-    const unsigned h = threadIdx.x - 32u, lane = threadIdx.x & 31u, wh = h >> 5;
+__device__ __forceinline__ void fs3_row_count(const Fs3Dev& d, Fs3Sh<NT>& sh, int par, unsigned nt, unsigned* pos, int* nrows, int* newrow) {
+    const unsigned tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
     const unsigned W = fs3_bm_words(d.m);
     const unsigned* bm = d.rowbm + (size_t)par * fs3_bm_ld(d.m);
-    const unsigned per = (W + NH - 1) / NH, w0 = min(W, h * per), w1 = min(W, w0 + per);
+    const unsigned per = (W + NT - 1) / NT, w0 = min(W, tid * per), w1 = min(W, w0 + per);
+    unsigned x[8];                                             // every load in flight before the first use
+#pragma unroll
+    for (unsigned i = 0; i < 8; ++i) x[i] = w0 + i < w1 ? __ldcg(bm + w0 + i) : 0xFFFFFFFFu;
+    int any = 0;
+    if (wid == 0) {
+#pragma unroll
+        for (unsigned i = 0; i < (FS3_MAX_TILES + 31) / 32; ++i) { const unsigned t = lane + 32u * i; if (t < nt) any |= __ldcg(bm + W + t) != 0u ? 1 : 0; }
+    }
     int cnt = 0;
     unsigned ff = 0xFFFFFFFFu;                                 // first free row id among my words
-#pragma unroll 1
-    for (unsigned w = w0; w < w1; ++w) {
-        const unsigned x = __ldcg(bm + w);
-        cnt += __popc(x);
-        if (ff == 0xFFFFFFFFu && ~x) ff = w * 32u + (unsigned)__ffs(~x) - 1u;
+#pragma unroll
+    for (unsigned i = 0; i < 8; ++i) {
+        if (w0 + i < w1) { cnt += __popc(x[i]); if (ff == 0xFFFFFFFFu && ~x[i]) ff = (w0 + i) * 32u + (unsigned)__ffs(~x[i]) - 1u; }
     }
     int incl = cnt;
 #pragma unroll 1
     for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, incl, o); if ((int)lane >= o) incl += y; }
     const unsigned wff = __reduce_min_sync(0xffffffffu, ff);
-    if (lane == 31) { sh.rowscan[0][wh] = (unsigned)incl; sh.rowscan[1][wh] = wff; }
-    int any = 0;
-    if (wh == 0) {
+    if (lane == 31) { sh.rowscan[0][wid] = (unsigned)incl; sh.rowscan[1][wid] = wff; }
+    if (wid == 0) { any = __any_sync(0xffffffffu, any); if (lane == 0) sh.rany = any; }
+    __syncthreads();
+    unsigned p = (unsigned)(incl - cnt), tot = 0, mf = 0xFFFFFFFFu;
 #pragma unroll 1
-        for (unsigned t = lane; t < nt; t += 32) any |= __ldcg(bm + W + t) != 0u ? 1 : 0;
-        any = __any_sync(0xffffffffu, any);
-    }
-    asm volatile("bar.sync 1, %0;" :: "r"(NH) : "memory");    // the hook warps only: warp 0 is busy with the chain
-    unsigned pos = (unsigned)(incl - cnt), tot = 0, mf = 0xFFFFFFFFu;
+    for (unsigned v = 0; v < NT / 32; ++v) { const unsigned c = sh.rowscan[0][v]; if (v < wid) p += c; tot += c; mf = min(mf, sh.rowscan[1][v]); }
+    *pos = p; *nrows = (int)tot; *newrow = sh.rany ? (int)mf : -1;
+}
+// the live rows at positions [base, base + FS3_ROW_CHUNK) of the ascending order into sh.rowl (pos from fs3_row_count); the caller
+// synchronises before sh.rowl is read
+template <int NT>
+__device__ __forceinline__ void fs3_row_fill(const Fs3Dev& d, Fs3Sh<NT>& sh, int par, unsigned base, unsigned pos) {
+    const unsigned tid = threadIdx.x;
+    const unsigned W = fs3_bm_words(d.m);
+    const unsigned* bm = d.rowbm + (size_t)par * fs3_bm_ld(d.m);
+    const unsigned per = (W + NT - 1) / NT, w0 = min(W, tid * per), w1 = min(W, w0 + per);
+    unsigned p = pos;
 #pragma unroll 1
-    for (unsigned v = 0; v < NH / 32; ++v) { const unsigned c = sh.rowscan[0][v]; if (v < wh) pos += c; tot += c; mf = min(mf, sh.rowscan[1][v]); }
-#pragma unroll 1
-    for (unsigned w = w0; w < w1; ++w)
-        for (unsigned x = __ldcg(bm + w); x; x &= x - 1) d.rowlist[pos++] = (unsigned short)(w * 32u + (unsigned)__ffs(x) - 1u);
-    if (h == 0) { d.rowinfo[0] = (int)tot; d.rowinfo[1] = any ? (int)mf : -1; }
+    for (unsigned w = w0; w < w1 && p < base + FS3_ROW_CHUNK; ++w)
+        for (unsigned x = __ldcg(bm + w); x; x &= x - 1, ++p)
+            if (p >= base && p < base + FS3_ROW_CHUNK) sh.rowl[p - base] = (unsigned short)(w * 32u + (unsigned)__ffs(x) - 1u);
 }
 
 // One exact sequential sum over the n_glob values held tile-wise in shared memory (thread t owns values t*K .. t*K+K-1 of its
 // tile, stored at vals[k*NT + t]).  toff = approximate sum of everything in front of this tile.  Returns the exact total
-// (identical in every CTA); with out != nullptr also stores the exact inclusive prefix of every value to out[global index].
-// Contains ONE grid barrier (`round`).
+// (identical in every CTA).  pub = 1: the chain's leader also publishes the tile prefixes and the sorted dirty values, and *run
+// keeps this thread's state, so that fs3_xsum_emit can store the exact inclusive prefixes afterwards (sh.fail = 0; with
+// sh.fail = 1 the serial walk has already stored them to `out`).  Contains ONE grid barrier (`round`).
 template <int NT>
 __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
-                                        unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, const Fs3Hook* hook = nullptr) {
+                                        unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run,
+                                        const Fs3Hook* hook = nullptr) {
     const int tid = threadIdx.x, lane = tid & 31, pp = round & 1;
     const unsigned b = blockIdx.x;
     const size_t T = (size_t)NT * K;
@@ -758,11 +784,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
     // ---- grid barrier + chain.  The LAST CTA to arrive evaluates the chain (every aggregate is published by then and it reads
     // them uncontended: 128 CTAs fetching the same few sectors at once serialise in L2) and publishes the results; the others
     // wait for its flag.  Warp 0 only; the other warps wait at the block barrier below. ----
-    if (hook && tid >= 32 && hook->compact) {
-        // the live-row list of this resample.  Every CTA's fs3_row_scan (in the first sum) is ordered before its arrival at the
-        // S2 sum's barrier, which this CTA has passed; the other CTAs read the list only after the grid barriers behind this sum.
-        if (b == 0) fs3_row_compact<NT>(d, sh, hook->par, nt);
-    } else if (hook && tid >= 32) {
+    if (hook && tid >= 32) {
         fs3_row_scan<NT>(d, *hook->po, hook->k_last, hook->par, b, nt);
         if (tid < 64) {                            // warp 1
             if (hook->comb_n && lane == 0) x3_comb_build(&sh.comb, r0, inv, (double)hook->comb_n, hook->comb_n);
@@ -891,7 +913,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             total = __shfl_sync(0xffffffffu, total, 0);
             if (slot == 0) FS3_TRACE(19);
             // publish: what the other CTAs need to finish on their own
-            if (out && !fail) {
+            if (pub && !fail) {
 #pragma unroll 1
                 for (unsigned t = lane; t < nt; t += 32) d.resTP[rt + t] = sh.tPoff[t];
 #pragma unroll 1
@@ -899,7 +921,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             }
             if (lane == 0) {
                 res->total = total; res->Ptot = Ptot; res->D = D; res->fail = fail;
-                sh.total = total; sh.Ptot = Ptot; sh.D = D; sh.fail = fail;
+                sh.total = total; sh.Ptot = Ptot; sh.D = D; sh.fail = fail; sh.lead = 1;
                 d.st->dirty_last = (int)cnt;
             }
             __syncwarp();                                          // the other lanes' stores above are ordered before lane 0's release
@@ -914,55 +936,79 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             FS3_TRACE(tb0 + 1);
             const double total = __ldcg(&res->total);
             const int D = __ldcg(&res->D), fail = __ldcg(&res->fail);
-            if (out && !fail) {                                   // the sorted dirty entries + my tile's increment prefix, for the emission
-                if (lane == 0) sh.tPoff[b] = __ldcg(d.resTP + rt + b);
-#pragma unroll 1
-                for (int o = lane; o < D; o += 32) { sh.skey[o] = __ldcg(d.resKey + rb + o); sh.sP[o] = __ldcg(d.resP + rb + o); sh.aft[o] = __ldcg(d.resAft + rb + o); }
-            }
-            if (lane == 0) { sh.total = total; sh.D = D; sh.fail = fail; }
+            if (lane == 0) { sh.total = total; sh.D = D; sh.fail = fail; sh.lead = 0; }
         }
     }
     __syncthreads();
     FS3_TRACE(tb0 + 2);
     if (sh.fail) { fs3_serial_walk<NT>(d, sh, K, slot, out, par, S2, r0, inv); return sh.total; }
-    if (out) {                                                // exact inclusive prefix of every value of this tile
-        const int D = sh.D;
-        const size_t g0 = (size_t)b * T + (size_t)tid * K;
-        int ko = 0;                                            // dirty values in front of this thread's first value
-        {
-            int lo = 0, hi = D;
-#pragma unroll 1
-            while (lo < hi) { const int mid = (lo + hi) >> 1; if ((size_t)sh.skey[mid] < g0) lo = mid + 1; else hi = mid; }
-            ko = lo;
-        }
-        double base = ko ? sh.aft[ko - 1] : 0.0;
-        unsigned long long Pb = ko ? sh.sP[ko - 1] : 0ull, Pc = sh.tPoff[b] + Pex;
-        double a = a_first, c = base;
-        int ok = 1;
-        if (e_run >= 0) {
-#pragma unroll 2
-            for (unsigned k = 0; k < K; ++k) {
-                unsigned long long inc;
-                if (x3_classify_at(vals[k * NT + tid], e_run, &inc)) { base = sh.aft[ko]; Pb = sh.sP[ko]; ko++; c = base; }
-                else { Pc += inc; c = x3_apply(base, Pc - Pb, inc ? e_run : -1, &ok); }
-                if (g0 + k < d.n_glob) out[g0 + k] = c;
-            }
-        } else {
-#pragma unroll 1
-            for (unsigned k = 0; k < K; ++k) {
-                const double v = vals[k * NT + tid], a1 = a + v;
-                unsigned long long inc; int lvl;
-                if (fs3_classify(v, a, a1, m32, &inc, &lvl)) { base = sh.aft[ko]; Pb = sh.sP[ko]; ko++; c = base; }
-                else { Pc += inc; c = x3_apply(base, Pc - Pb, inc ? lvl : -1, &ok); }
-                if (g0 + k < d.n_glob) out[g0 + k] = c;
-                a = a1;
-            }
-        }
-        if (slot == 3 && tid == NT - 1) d.tileEnd[b] = c;      // coarse level of the index search
-        if (!ok) atomicAdd(&d.st->cert_fail, 1);
-        FS3_TRACE(tb0 + 3);
-    }
+    if (run) { run->a_first = a_first; run->Pex = Pex; run->e_run = e_run; }
     return sh.total;
+}
+
+// The exact inclusive prefix c_j of every value of this tile after fs3_xsum(pub = 1) of round `round` (nothing when that sum took
+// the serial walk: it has stored them already).  cert == nullptr: c_j goes to out[j].  Otherwise fl(c_j / cert->S) goes to
+// out[j], and the return value is 1 when some comb value may lie on the other side of it than of the CDF the reference computes
+// (x3_cdf_near_comb), or a clean run failed its certificate.  tend: the tile's last stored value goes to tileEnd[tile].
+// vals must still hold the values the sum saw.  Contains one block barrier.
+template <int NT>
+__device__ __noinline__ int fs3_xsum_emit(const Fs3Dev& d, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
+                                          double* out, int tend, const Fs3Cert* cert, int tslot) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    const unsigned b = blockIdx.x;
+    const size_t T = (size_t)NT * K;
+    unsigned long long t_prev = 0;
+    if (d.trace && b == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_prev));
+    if (sh.fail) return 0;
+    if (tid < 32 && !sh.lead) {                               // the sorted dirty entries + my tile's increment prefix, as the leader published them
+        const size_t rb = (size_t)round * FS3_ENT_CAP, rt = (size_t)round * FS3_MAX_TILES;
+        if (lane == 0) sh.tPoff[b] = __ldcg(d.resTP + rt + b);
+#pragma unroll 1
+        for (int o = lane; o < sh.D; o += 32) { sh.skey[o] = __ldcg(d.resKey + rb + o); sh.sP[o] = __ldcg(d.resP + rb + o); sh.aft[o] = __ldcg(d.resAft + rb + o); }
+    }
+    __syncthreads();
+    const int D = sh.D, e_run = run->e_run;
+    const size_t g0 = (size_t)b * T + (size_t)tid * K;
+    int ko = 0;                                                // dirty values in front of this thread's first value
+    {
+        int lo = 0, hi = D;
+#pragma unroll 1
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if ((size_t)sh.skey[mid] < g0) lo = mid + 1; else hi = mid; }
+        ko = lo;
+    }
+    double base = ko ? sh.aft[ko - 1] : 0.0;
+    unsigned long long Pb = ko ? sh.sP[ko - 1] : 0ull, Pc = sh.tPoff[b] + run->Pex;
+    double a = run->a_first, c = base, o = base;
+    int ok = 1, near = 0;
+    if (e_run >= 0 && !cert) {                                 // the usual exact emission: the whole run inside one binade
+#pragma unroll 2
+        for (unsigned k = 0; k < K; ++k) {
+            unsigned long long inc;
+            if (x3_classify_at(vals[k * NT + tid], e_run, &inc)) { base = sh.aft[ko]; Pb = sh.sP[ko]; ko++; c = base; }
+            else { Pc += inc; c = x3_apply(base, Pc - Pb, inc ? e_run : -1, &ok); }
+            if (g0 + k < d.n_glob) out[g0 + k] = c;
+        }
+        o = c;
+    } else {
+#pragma unroll 1
+        for (unsigned k = 0; k < K; ++k) {
+            const double v = vals[k * NT + tid], a1 = a + v;
+            unsigned long long inc; int lvl = e_run;
+            if (e_run >= 0 ? x3_classify_at(v, e_run, &inc) : fs3_classify(v, a, a1, m32, &inc, &lvl)) { base = sh.aft[ko]; Pb = sh.sP[ko]; ko++; c = base; }
+            else { Pc += inc; c = x3_apply(base, Pc - Pb, inc ? lvl : -1, &ok); }
+            o = c;
+            if (cert) {
+                o = fs3_div(c, cert->S);
+                if (g0 + k < d.n_glob) near |= x3_cdf_near_comb(o, cert->r0, cert->inv, cert->ninv, cert->n, cert->dl, cert->ab);
+            }
+            if (g0 + k < d.n_glob) out[g0 + k] = o;
+            a = a1;
+        }
+    }
+    if (tend && tid == NT - 1) d.tileEnd[b] = o;              // coarse level of the index search
+    if (!ok) { atomicAdd(&d.st->cert_fail, 1); near = 1; }
+    if (tslot >= 0) FS3_TRACE(tslot);
+    return near;
 }
 
 // lower bound of r in the exact CDF, clamped: "while r > cum_sum[j+1] && j < n-1 { j += 1 }" (fs1.rs:224-226) with r and j both
@@ -1045,11 +1091,46 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     const double inv = fs3_div(1.0, (double)ng);
     const double r0 = pfc_u01_52(pfc_blk_u64(pfc_rng_block(seed, PFC_STREAM_FS_RESAMPLE, st->resamples, 0), 0)) * (inv - 0.0) + 0.0;
     // ---------------- S = sum w_raw (normalize_weights fs1.rs:196-203) ----------------
+    // With n = 2^p, p <= FS3_CERT_MAX_LOG2N, the leader also publishes what every CTA needs to emit the exact prefixes P_j of w_raw:
+    // a resample may then use the certified CDF fl(P_j / S) instead of the S2 and CDF sums (see below)
+    const int cert_pub = log2n >= 0 && log2n <= FS3_CERT_MAX_LOG2N && !d.exact_cdf;
     Fs3Hook hook;
     hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.noise_call = step + 1u; hook.k_last = k_last; hook.po = &po;
-    hook.par = par; hook.compact = 0;
-    const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, m32, nullptr, par, 0.0, r0, inv, q, &hook);
+    hook.par = par;
+    Fs3Run run;
+    const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
+    const int S_walked = sh.fail;
     FS3_TRACE(1);
+    // ---------------- gate: neff = 1 / sum w^2 < NTH (compute_neff fs1.rs:186-193, fs1.rs:262-263) ----------------
+    // Only the DECISION feeds back into the state.  Q is first taken from the tree-order sums of w_raw^2 published with the
+    // aggregates of S: sum (w_raw_i / S)^2 differs from the reference's sequential sum of fl(w_raw_i / S)^2 by at most
+    // (n + 64) 2^-51 relatively; only when neff lands that close to NTH is the exact sequential sum walked (below, once wn_all is written).
+    double Q = (unsigned)tid < nt ? __ldcg(d.tileQ + tid) : 0.0, dummy = 0.0;
+    fs3_block_sum2<NT>(Q, dummy, sh.red[1], sh.wd[1]);
+    if (S > 0.0) Q = fs3_div(fs3_div(Q, S), S);
+    double neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
+    const double slack = 16.0 * (double)(ng + 64) * 2.220446049250313e-16;
+    // The error bound of the shortcut assumes that no w_raw^2 that matters under- or overflows: with S inside [1e-120, 1e120] the
+    // squares of all weights within 1e-34 of the largest are normal numbers.  Outside (e.g. an outlier observation that drives
+    // EVERY likelihood to 1e-170: the normalised weights are perfectly ordinary, their raw squares are all zero) the exact sum decides.
+    const bool scale_ok = !(S > 0.0) || (S >= 1e-120 && S <= 1e120);
+    const bool border = !scale_ok || !(fabs(neff - nth) > slack * fmax(fabs(nth), fabs(neff)));     // the same decision in every CTA
+    // ---------------- certified CDF (DESIGN §1) ----------------
+    // The index rule only COMPARES comb values with CDF values.  On a resample of n = 2^p weights with S > 0 in the window above and
+    // no serial walk, every CTA stores c~_j = fl(P_j / S) for its tile to cum_all; |c_j - c~_j| <= dl c~_j + ab for the reference's
+    // CDF c_j (normalise, re-normalise by S2, sequential cum_sum).  A CTA that finds a comb value within that distance of one of
+    // its c~_j raises the certificate flag, and then every CTA runs the exact S2 and CDF sums behind the next grid barrier.
+    const bool cert = cert_pub && !border && neff < nth && S > 0.0 && !S_walked;
+    if (cert) {
+        Fs3Cert cp;
+        const double g = 4.0 * (double)ng * 1.1102230246251565e-16;      // 4 n 2^-53
+        cp.S = S; cp.r0 = r0; cp.inv = inv; cp.ninv = (double)ng; cp.n = ng;
+        cp.dl = g / (1.0 - g) * (1.0 + 9.5367431640625e-07);             // gamma_4n (1 + 2^-20)
+        cp.ab = (4.0 * (double)ng + 4.0) * 4.9406564584124654e-324 + (double)(log2n + 4) * 1.1102230246251565e-16;
+        const int near = fs3_xsum_emit<NT>(d, sh, vals, K, m32, &run, 0, d.cum_all, 1, &cp, -1);
+        if (__syncthreads_or(near) && tid == 0) d.flagsg[FS3_CERT_FLAG] = 1;
+        FS3_TRACE(4);
+    }
     // w = w_raw / S; best particle of the tile (LAST maximum, fs1.rs:269-274)
     double bw = -1.0; unsigned bi = 0;
 #pragma unroll 1
@@ -1070,25 +1151,13 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         if (ow > bw || (ow == bw && oi > bi)) { bw = ow; bi = oi; }
     }
     if ((tid & 31) == 0) { sh.red[0][tid >> 5] = bw; sh.wi[0][tid >> 5] = (int)bi; }
-    // ---------------- gate: neff = 1 / sum w^2 < NTH (compute_neff fs1.rs:186-193, fs1.rs:262-263) ----------------
-    // Only the DECISION feeds back into the state.  Q is first taken from the tree-order sums of w_raw^2 published with the
-    // aggregates of S: sum (w_raw_i / S)^2 differs from the reference's sequential sum of fl(w_raw_i / S)^2 by at most
-    // (n + 64) 2^-51 relatively; only when neff lands that close to NTH is the exact sequential sum walked.
-    double Q = (unsigned)tid < nt ? __ldcg(d.tileQ + tid) : 0.0, dummy = 0.0;
-    fs3_block_sum2<NT>(Q, dummy, sh.red[1], sh.wd[1]);         // (also orders the arg-max partials above)
+    __syncthreads();
     if (tid == 0) {
 #pragma unroll 1
         for (int w = 1; w < NT / 32; ++w) { const double ow = sh.red[0][w]; const unsigned oi = (unsigned)sh.wi[0][w]; if (ow > bw || (ow == bw && oi > bi)) { bw = ow; bi = oi; } }
         d.tileBw[b] = bw; d.tileBi[b] = bi;
     }
-    if (S > 0.0) Q = fs3_div(fs3_div(Q, S), S);
-    double neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
-    const double slack = 16.0 * (double)(ng + 64) * 2.220446049250313e-16;
-    // The error bound of the shortcut assumes that no w_raw^2 that matters under- or overflows: with S inside [1e-120, 1e120] the
-    // squares of all weights within 1e-34 of the largest are normal numbers.  Outside (e.g. an outlier observation that drives
-    // EVERY likelihood to 1e-170: the normalised weights are perfectly ordinary, their raw squares are all zero) the exact sum decides.
-    const bool scale_ok = !(S > 0.0) || (S >= 1e-120 && S <= 1e120);
-    if (!scale_ok || !(fabs(neff - nth) > slack * fmax(fabs(nth), fabs(neff)))) {     // rare; the same decision in every CTA
+    if (border) {                                              // rare
         fs3_grid_sync<NT>(d, 6, nt);                           // wn_all is complete
         if (tid == 0) {
             double s = 0.0;
@@ -1105,46 +1174,58 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     FS3_TRACE(2);
     double S2 = 0.0;
     if (gate) {
-        // ---------------- resample() re-normalises first (fs1.rs:207) ----------------
-        const double toff2 = S > 0.0 ? fs3_div(toff, S) : toff;
-        S2 = fs3_xsum<NT>(d, sh, vals, K, nt, toff2, 2, 1, m32, nullptr, par, 0.0, 0.0, 0.0, 0.0);
-        FS3_TRACE(3);
-        if (S2 > 0.0) {
-#pragma unroll 1
-            for (unsigned k = 0; k < K; ++k) vals[k * NT + tid] = fs3_div(vals[k * NT + tid], S2);
-        }
-        // ---------------- cum_sum fs1.rs:213-216 ----------------
-        const double toff3 = S2 > 0.0 ? fs3_div(toff2, S2) : toff2;
-        hook.compact = 1;
-        (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, &hook);
-        FS3_TRACE(4);
-        // ---------------- the comb r, r + 1/n, ... accumulated sequentially (fs1.rs:219-230) ----------------
-        if (log2n < 0) {                                       // n not a power of two: every add rounds -> exact scan
-        #pragma unroll 1
-    for (unsigned k = 0; k < K; ++k) { const size_t i = g0 + k; vals[k * NT + tid] = i < ng ? (i == 0 ? r0 : inv) : 0.0; }
-            const double toff4 = b == 0 ? 0.0 : r0 + ((double)((size_t)b * T) - 1.0) * inv;
-            __syncthreads();
-            (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff4, 4, 3, m32, d.rcomb_all, par, S2, r0, inv, 0.0);
-        }
         // this CTA's landmark slice (only this CTA writes it, in the first sum): its first entries are loaded in front of the barrier,
         // so the retarget behind the index walk does not wait for them
         unsigned lm_lo, lm_hi;
         fs3_lm_slice(d, b, nt, &lm_lo, &lm_hi);
         const int s_first = lm_lo + tid < lm_hi ? d.lmst[lm_lo + tid] : 0;
-        fs3_grid_sync<NT>(d, 4, nt);                           // the whole CDF (and comb) is visible
-        FS3_TRACE(5);
+        bool exact = !cert;
+        if (cert) {
+            fs3_grid_sync<NT>(d, 4, nt);                       // every c~_j and every CTA's verdict are visible
+            exact = __ldcg(d.flagsg + FS3_CERT_FLAG) != 0;
+            FS3_TRACE(5);
+        }
+        if (exact) {
+            if (b == 0 && tid == 0) st->cdf_exact += 1;
+            // ---------------- resample() re-normalises first (fs1.rs:207) ----------------
+            const double toff2 = S > 0.0 ? fs3_div(toff, S) : toff;
+            S2 = fs3_xsum<NT>(d, sh, vals, K, nt, toff2, 2, 1, m32, nullptr, par, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
+            FS3_TRACE(3);
+            if (S2 > 0.0) {
+#pragma unroll 1
+                for (unsigned k = 0; k < K; ++k) vals[k * NT + tid] = fs3_div(vals[k * NT + tid], S2);
+            }
+            // ---------------- cum_sum fs1.rs:213-216 ----------------
+            const double toff3 = S2 > 0.0 ? fs3_div(toff2, S2) : toff2;
+            (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, 1, &run);
+            (void)fs3_xsum_emit<NT>(d, sh, vals, K, m32, &run, 2, d.cum_all, 1, nullptr, 15);
+            FS3_TRACE(4);
+            // ---------------- the comb r, r + 1/n, ... accumulated sequentially (fs1.rs:219-230) ----------------
+            if (log2n < 0) {                                   // n not a power of two: every add rounds -> exact scan
+#pragma unroll 1
+                for (unsigned k = 0; k < K; ++k) { const size_t i = g0 + k; vals[k * NT + tid] = i < ng ? (i == 0 ? r0 : inv) : 0.0; }
+                const double toff4 = b == 0 ? 0.0 : r0 + ((double)((size_t)b * T) - 1.0) * inv;
+                __syncthreads();
+                (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff4, 4, 3, m32, d.rcomb_all, par, S2, r0, inv, 0.0, 1, &run);
+                (void)fs3_xsum_emit<NT>(d, sh, vals, K, m32, &run, 3, d.rcomb_all, 0, nullptr, -1);
+            }
+            fs3_grid_sync<NT>(d, cert ? 5 : 4, nt);            // the whole CDF (and comb) is visible
+            FS3_TRACE(5);
+        }
         // ---------------- index walk, pose clone, lazy map clone for this CTA's share of the local slots ----------------
         // j_t = first j with c_j >= r_t, clamped to n - 1: "while r > cum_sum[j+1] && j < n-1 { j += 1 }" (fs1.rs:224-226) with r and
         // j both non-decreasing over the slots.  The CTA's first and last slot bracket all of its answers; the bracketed piece of
-        // the CDF is staged in shared memory (it is about as long as the slot range) and every slot searches there.
-        const int nrows = __ldcg(d.rowinfo), newrow = __ldcg(d.rowinfo + 1);     // (fs3_row_compact, in CTA 0 during the CDF sum)
+        // the CDF is staged in shared memory (it is about as long as the slot range) and every slot searches there.  The certified
+        // CDF is monotone and every comparison with a comb value comes out as with the exact one, so the same search serves both.
         const int cur = st->cur, rcur = st->rcur;
         const unsigned per = (d.n + nt - 1) / nt;              // local slots per CTA
         const unsigned t_lo = b * per, t_hi = min(d.n, t_lo + per);
         const double* cdf = d.cum_all;
 #pragma unroll 1
         for (unsigned t = tid; t < nt; t += NT) sh.tend[t] = __ldcg(d.tileEnd + t);
-        __syncthreads();
+        // the live rows: every CTA's fs3_row_scan (inside the S sum) is ordered before the grid barrier this CTA has just passed
+        unsigned rpos; int nrows, newrow;
+        fs3_row_count<NT>(d, sh, par, nt, &rpos, &nrows, &newrow);            // (also orders the tileEnd copy)
         if (t_lo < t_hi) {
             if (tid < 64) {
                 const size_t te = (size_t)d.off + (tid < 32 ? t_lo : t_hi - 1);
@@ -1153,6 +1234,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
                 if ((tid & 31) == 0) sh.jr[tid >> 5] = je;
             }
         }
+        fs3_row_fill<NT>(d, sh, par, 0, rpos);
         __syncthreads();
         if (t_lo < t_hi) {
             FS3_TRACE(22);
@@ -1165,65 +1247,91 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             }
             __syncthreads();
             FS3_TRACE(23);
-            // four slots per thread and trip: their searches, pose gathers and row gathers are independent, so the dependent memory
-            // round trips (index -> ancestor's pose -> ancestor's row entries) overlap four-fold
+            unsigned* drows = d.rows[rcur ^ 1];
+            // rows in chunks of FS3_ROW_CHUNK (one chunk but for very large maps); the first chunk's pass also searches the slots and
+            // clones the poses, later passes take the ancestors from idx (this thread's own stores)
 #pragma unroll 1
-            for (unsigned t0 = t_lo + tid; t0 < t_hi; t0 += 4 * NT) {
-                unsigned jj[4]; int jrk[4]; unsigned jcol[4];
+            for (unsigned rbase = 0; ; rbase += FS3_ROW_CHUNK) {
+                const int nr = min(nrows - (int)rbase, FS3_ROW_CHUNK);
+                // four slots per thread and trip: their searches, pose gathers and row gathers are independent, so the dependent memory
+                // round trips (index -> ancestor's pose -> ancestor's row entries) overlap four-fold
+#pragma unroll 1
+                for (unsigned t0 = t_lo + tid; t0 < t_hi; t0 += 4 * NT) {
+                    unsigned jj[4]; int jrk[4]; unsigned jcol[4];
+                    if (rbase == 0) {
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const unsigned t = t0 + (unsigned)u * NT;
-                    jj[u] = 0; jrk[u] = 0; jcol[u] = 0;
-                    if (t < t_hi) {
-                        const size_t tg = (size_t)d.off + t;
-                        const double r = log2n >= 0 ? x3_comb_eval(&sh.comb, inv, tg) : __ldcg(d.rcomb_all + tg);
-                        unsigned lo = 0, hi = len;
-                        if (staged) {
+                        for (int u = 0; u < 4; ++u) {
+                            const unsigned t = t0 + (unsigned)u * NT;
+                            jj[u] = 0; jrk[u] = 0; jcol[u] = 0;
+                            if (t < t_hi) {
+                                const size_t tg = (size_t)d.off + t;
+                                const double r = log2n >= 0 ? x3_comb_eval(&sh.comb, inv, tg) : __ldcg(d.rcomb_all + tg);
+                                unsigned lo = 0, hi = len;
+                                if (staged) {
 #pragma unroll 1
-                            while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (vals[mid] < r) lo = mid + 1; else hi = mid; }
-                        } else {
+                                    while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (vals[mid] < r) lo = mid + 1; else hi = mid; }
+                                } else {
 #pragma unroll 1
-                            while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (__ldcg(cdf + jlo + mid) < r) lo = mid + 1; else hi = mid; }
+                                    while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (__ldcg(cdf + jlo + mid) < r) lo = mid + 1; else hi = mid; }
+                                }
+                                unsigned j = jlo + lo;
+                                if (j >= ng) j = (unsigned)ng - 1;
+                                jj[u] = j; jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;              // owner rank and column of the ancestor
+                            }
                         }
-                        unsigned j = jlo + lo;
-                        if (j >= ng) j = (unsigned)ng - 1;
-                        jj[u] = j; jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;              // owner rank and column of the ancestor
+                        double gx[4], gy[4], ga[4];
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) {
+                            const double* sx = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_px[cur]) : d.px[cur];
+                            const double* sy = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_py[cur]) : d.py[cur];
+                            const double* sa = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_pyaw[cur]) : d.pyaw[cur];
+                            gx[u] = sx[jcol[u]]; gy[u] = sy[jcol[u]]; ga[u] = sa[jcol[u]];
+                        }
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) {
+                            const unsigned t = t0 + (unsigned)u * NT;
+                            if (t < t_hi) {
+                                d.idx[t] = jj[u];
+                                d.px[cur ^ 1][t] = gx[u]; d.py[cur ^ 1][t] = gy[u]; d.pyaw[cur ^ 1][t] = ga[u];     // particles[j].clone() fs1.rs:227
+                                d.w[t] = inv;                                                            // fs1.rs:228
+                                if (newrow >= 0) drows[(size_t)newrow * d.ld + t] = fs3_ref(jrk[u], jcol[u]);
+                            }
+                        }
+                    } else {
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) {
+                            const unsigned t = t0 + (unsigned)u * NT;
+                            const unsigned j = t < t_hi ? d.idx[t] : 0u;
+                            jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;
+                        }
+                    }
+                    // the ancestors' row entries: eight rows x four slots of independent gathers in flight per batch (the rows were
+                    // written a resample ago; one dependent HBM round trip per batch instead of per row)
+                    const unsigned* srow[4];
+#pragma unroll
+                    for (int u = 0; u < 4; ++u)
+                        srow[u] = (d.G > 1 ? reinterpret_cast<const unsigned*>(d.peer[jrk[u]] + d.o_rows[rcur]) : d.rows[rcur]) + jcol[u];
+#pragma unroll 1
+                    for (int x0 = 0; x0 < nr; x0 += 8) {
+                        unsigned e[8][4];
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) {
+                            const size_t ro = (size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld;
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) e[i][u] = (x0 + i < nr && t0 + (unsigned)u * NT < t_hi) ? srow[u][ro] : 0u;
+                        }
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) {
+                            const size_t ro = (size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld;
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) { const unsigned t = t0 + (unsigned)u * NT; if (x0 + i < nr && t < t_hi) drows[ro + t] = e[i][u]; }
+                        }
                     }
                 }
-                double gx[4], gy[4], ga[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const double* sx = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_px[cur]) : d.px[cur];
-                    const double* sy = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_py[cur]) : d.py[cur];
-                    const double* sa = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_pyaw[cur]) : d.pyaw[cur];
-                    gx[u] = sx[jcol[u]]; gy[u] = sy[jcol[u]]; ga[u] = sa[jcol[u]];
-                }
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const unsigned t = t0 + (unsigned)u * NT;
-                    if (t < t_hi) {
-                        d.idx[t] = jj[u];
-                        d.px[cur ^ 1][t] = gx[u]; d.py[cur ^ 1][t] = gy[u]; d.pyaw[cur ^ 1][t] = ga[u];     // particles[j].clone() fs1.rs:227
-                        d.w[t] = inv;                                                            // fs1.rs:228
-                    }
-                }
-                unsigned* drows = d.rows[rcur ^ 1];
-#pragma unroll 2
-                for (int x = 0; x < nrows; ++x) {
-                    const size_t ro = (size_t)d.rowlist[x] * d.ld;
-                    unsigned e[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const unsigned* srows = d.G > 1 ? reinterpret_cast<const unsigned*>(d.peer[jrk[u]] + d.o_rows[rcur]) : d.rows[rcur];
-                        e[u] = srows[ro + jcol[u]];
-                    }
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) { const unsigned t = t0 + (unsigned)u * NT; if (t < t_hi) drows[ro + t] = e[u]; }
-                }
-                if (newrow >= 0) {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) { const unsigned t = t0 + (unsigned)u * NT; if (t < t_hi) drows[(size_t)newrow * d.ld + t] = fs3_ref(jrk[u], jcol[u]); }
-                }
+                if ((int)(rbase + FS3_ROW_CHUNK) >= nrows) break;
+                __syncthreads();                               // everybody is through this chunk's rows
+                fs3_row_fill<NT>(d, sh, par, rbase + FS3_ROW_CHUNK, rpos);
+                __syncthreads();
             }
         }
         if (newrow >= 0) {     // the identity landmarks of this CTA's slice now read through the new row (every scan of lmst is over)
@@ -1241,7 +1349,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     __syncthreads();
     if (!sh.last) return;
     if (d.trace && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); d.trace[40] += t - d.trace[39]; }   // [40] the last CTA is through
-    if (tid < FS3_SLOTS) { d.flagsg[tid] = 0; d.entCnt[tid] = 0u; }
+    if (tid < FS3_SLOTS) d.entCnt[tid] = 0u;
+    if (tid <= FS3_CERT_FLAG) d.flagsg[tid] = 0;
     if (tid < 8) { d.bar[tid] = 0u; d.resflag[tid] = 0u; }
     if (tid < 32) {
         // best particle: the last maximum over the tiles (no resample) / the last slot (after a resample every weight is 1/n)

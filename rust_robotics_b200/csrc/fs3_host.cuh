@@ -139,8 +139,6 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         FS_TRY(cudaMalloc(&d.resKey, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned))); FS_TRY(cudaMalloc(&d.resP, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned long long)));
         FS_TRY(cudaMalloc(&d.resAft, (size_t)8 * FS3_ENT_CAP * sizeof(double)));
         FS_TRY(cudaMalloc(&d.tileEnd, FS3_MAX_TILES * sizeof(double)));
-        FS_TRY(cudaMalloc(&d.rowlist, mm * sizeof(unsigned short))); FS_TRY(cudaMalloc(&d.rowinfo, 2 * sizeof(int)));
-        FS_TRY(cudaMemset(d.rowinfo, 0, 2 * sizeof(int)));
         const size_t nbm = (size_t)2 * fs3_bm_ld((unsigned)m);       // both parities start clear; each post kernel clears the other
         FS_TRY(cudaMalloc(&d.rowbm, nbm * sizeof(unsigned))); FS_TRY(cudaMemset(d.rowbm, 0, nbm * sizeof(unsigned)));
         FS_TRY(cudaMalloc(&d.tileBw, FS3_MAX_TILES * sizeof(double))); FS_TRY(cudaMalloc(&d.tileBi, FS3_MAX_TILES * sizeof(unsigned)));
@@ -153,6 +151,7 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
     { const char* e5 = getenv("PFGPU_PDL"); h->pdl = !(e5 && e5[0] == '0'); }
     { const char* e7 = getenv("PFGPU_EARLY_LAUNCH"); if (e7 && atoi(e7) == 1) h->early = true; }
     { const char* e6 = getenv("PFGPU_EKF_HELPERS"); if (e6 && atoi(e6) >= 1 && atoi(e6) <= 3) h->ekf_helpers = atoi(e6); }
+    { const char* e8 = getenv("PFGPU_FS_EXACT_CDF"); d.exact_cdf = e8 && atoi(e8) == 1 ? 1 : 0; }   // A/B: every resample runs the exact S2 and CDF sums
     if (world > 1 && uid) {
         ncclUniqueId id;
         memcpy(&id, uid, sizeof(id));
@@ -239,7 +238,7 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(h->arena);
     cudaFree(d.st); cudaFree(d.lmst); cudaFree(d.w); cudaFree(d.nz[0]); cudaFree(d.nz[1]); cudaFree(d.wn_all); cudaFree(d.cum_all); cudaFree(d.rcomb_all); cudaFree(d.idx);
     cudaFree(d.tileP); cudaFree(d.tileQ); cudaFree(d.entCnt); cudaFree(d.entKey); cudaFree(d.entTile); cudaFree(d.entP); cudaFree(d.entV); cudaFree(d.entL);
-    cudaFree(d.bar); cudaFree(d.rowlist); cudaFree(d.rowinfo); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
+    cudaFree(d.bar); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
     cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->stage);
     if (h->h_rec) cudaFreeHost(h->h_rec);
@@ -540,6 +539,11 @@ extern "C" int pfgpu_fs_post_trace(pfgpu_fs* h, unsigned long long* out32) {
     for (int k = 0; k < 32; ++k) out32[k] = 0;
     if (h->d.trace) PF_CUDA(cudaMemcpy(out32, h->d.trace, 32 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     out32[31] = h->steps;
+    {                     // [11] resamples that ran the exact S2 and CDF sums instead of the certified CDF
+        Fs3State st;
+        PF_CUDA(cudaMemcpy(&st, h->d.st, sizeof(st), cudaMemcpyDeviceToHost));
+        out32[11] = (unsigned long long)st.cdf_exact;
+    }
     // step timeline [ns], folded into the free slot pairs: [7] idle before the EKF launch, [24..26] EKF launch, idle between the
     // launches, post launch
     if (h->d.trace) {

@@ -54,7 +54,7 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
     fs3_block_sum2<NT>(toff, qoff, sh.red[0], sh.red[1]);      // (red[] is free again: the grid barrier above is also a block barrier;
                                                                //  wd[] is the first scratch fs3_xsum writes, with no barrier in between)
     // ---------------- S = sum w_raw, sequential (normalize_weights pf.rs:426-439) ----------------
-    const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0);
+    const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
     const double unif = 1.0 / (double)pd.n_global;
 #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) {
@@ -83,7 +83,7 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
         if (!scale_ok || !(fabs(neff - thr) > slack * fmax(fabs(thr), fabs(neff)))) {     // rare; the same decision in every CTA
             const double toffq = S > 0.0 ? fs3_div(fs3_div(qoff, S), S) : (double)((size_t)b * T) * unif * unif;
             __syncthreads();
-            Q = fs3_xsum<NT>(d, sh, vals2, K, nt, toffq, 1, 1, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0);
+            Q = fs3_xsum<NT>(d, sh, vals2, K, nt, toffq, 1, 1, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
             neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
         }
         gate = neff < thr ? 1 : 0;
@@ -93,7 +93,9 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
         // ---------------- cumulative weights (pf.rs:448-453 / mcl.rs:328-336), exact inclusive prefix of every weight ----------------
         const double toffc = S > 0.0 ? fs3_div(toff, S) : (double)((size_t)b * T) * unif;
         __syncthreads();
-        ctot = fs3_xsum<NT>(d, sh, vals, K, nt, toffc, 3, 2, a.m32, pd.cum, 0, 0.0, 0.0, 0.0, 0.0);
+        Fs3Run run;
+        ctot = fs3_xsum<NT>(d, sh, vals, K, nt, toffc, 3, 2, a.m32, pd.cum, 0, 0.0, 0.0, 0.0, 0.0, 1, &run);
+        (void)fs3_xsum_emit<NT>(d, sh, vals, K, a.m32, &run, 2, pd.cum, 1, nullptr, 15);
         __syncthreads();                                       // every prefix of this tile is stored before the last one is overridden
         if (a.mode == 1 && b == (unsigned)((n - 1) / T) && tid == 0) { pd.cum[n - 1] = 1.0; d.tileEnd[b] = 1.0; }   // *last = 1.0 mcl.rs:334-336
         fs3_grid_sync<NT>(d, 4, nt);                           // the whole CDF is visible

@@ -133,4 +133,20 @@ PFC_HD double x3_comb_eval(const x3_comb_table* tb, double inv, unsigned long lo
     return tb->V[k] + (double)(t - tb->T[k]) * inv;
 }
 
+/* Certified CDF (DESIGN §1).  c is fl(P_j / S); the CDF value the reference computes lies within dl * c + ab of it.  Returns 1
+ * when a comb value r_t (n = 2^p values, r_0 = r0, step inv = 2^-p, ninv = 2^p) may lie within that distance of c, i.e. when
+ * "c_j >= r_t" might come out differently for c than for the reference's value.  r0 + t inv stands in for the sequential r_t:
+ * the accumulation rounds at most p + 3 times (once per binade it enters), by at most 2^-54 each, and the stand-in once more;
+ * ab carries that (p + 4) 2^-53.  A comb value within distance 1 / (2n) of c has t within one of (c - r0) n: four candidates. */
+PFC_HD int x3_cdf_near_comb(double c, double r0, double inv, double ninv, unsigned long long n, double dl, double ab) {
+    const double lim = dl * c + ab;
+    const double t0 = floor((c - r0) * ninv) - 1.0;
+    int near = 0;
+    for (int i = 0; i < 4; ++i) {
+        const double t = t0 + (double)i;
+        if (t >= 0.0 && t < (double)n && fabs((r0 + t * inv) - c) <= lim) near = 1;
+    }
+    return near;
+}
+
 #endif
