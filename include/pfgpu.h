@@ -108,7 +108,8 @@ typedef struct pfgpu_fs pfgpu_fs;
 
 void pfgpu_fs_default_config(pfgpu_fs_config* cfg);
 /* create_particles(n, m) fs1.rs:302-306.  0 <= n_landmarks <= 65536 (this and both sharded create calls); more returns
- * PFGPU_ERR_UNSUPPORTED with a message in pfgpu_last_error. */
+ * PFGPU_ERR_UNSUPPORTED with a message in pfgpu_last_error.  n_particles < 2^28 (per GPU when sharded); beyond that the limit
+ * is device memory (about 104 * n_landmarks + 140 bytes per particle), and an allocation that fails returns PFGPU_ERR_CUDA. */
 int  pfgpu_fs_create(const pfgpu_fs_config* cfg, size_t n_particles, size_t n_landmarks, uint64_t seed,
                      int device, pfgpu_fs** out);
 /* Sharded over `world` (<= 8) GPUs of one NVLink domain, one process per GPU; collective over all ranks (same arguments
@@ -183,6 +184,9 @@ int  pfgpu_fs_stats(pfgpu_fs*, pfgpu_stats*);
 /* debug (PFGPU_POST_TRACE=1): accumulated per-phase times [ns] of the fused post-step kernel; out32[31] = launches,
    out32[11] = resamples that ran the exact S2 and CDF sums instead of the certified CDF (counted with or without the trace) */
 int  pfgpu_fs_post_trace(pfgpu_fs*, unsigned long long* out32);
+/* shape of the fused post-step kernel: tiles (one co-resident CTA each) x threads x values per thread, and whether the tiles
+   live in shared memory (*global_tile = 0) or, for particle counts whose tile does not fit on chip, in global memory (1) */
+int  pfgpu_fs_post_shape(pfgpu_fs*, unsigned* tiles, unsigned* threads, unsigned* values_per_thread, int* global_tile);
 /* how the coupled part of the step runs: 0 = one GPU, 2 = sharded over peer memory (NVLink loads / stores inside the kernels;
    no NCCL call and no host sync per step) */
 int  pfgpu_fs_shard_mode(pfgpu_fs*, int* mode);

@@ -62,7 +62,7 @@ EXPORTS = [
     "pfgpu_fs_get_observations", "pfgpu_fs_last_indices", "pfgpu_fs_last_neff", "pfgpu_fs_last_gate", "pfgpu_fs_set_variant", "pfgpu_fs_count", "pfgpu_fs_sync",
     "pfgpu_nccl_unique_id", "pfgpu_pf_stats", "pfgpu_fs_stats", "pfgpu_pf_time_main_kernel",
     "pfgpu_fs_time_main_kernel", "pfgpu_pf_mark", "pfgpu_pf_elapsed_ms", "pfgpu_fs_mark", "pfgpu_fs_elapsed_ms",
-    "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_shard_mode",
+    "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
 ]
 
 
@@ -133,6 +133,7 @@ def load_library():
         getattr(L, f"pfgpu_{k}_elapsed_ms").argtypes = [vp, C.c_int, C.c_int, c_dp]
         getattr(L, f"pfgpu_{k}_flush_l2").argtypes = [vp]
     L.pfgpu_fs_post_trace.argtypes = [vp, C.POINTER(C.c_ulonglong)]
+    L.pfgpu_fs_post_shape.argtypes = [vp, C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_int)]
     L.pfgpu_fs_shard_mode.argtypes = [vp, C.POINTER(C.c_int)]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
@@ -545,6 +546,13 @@ class FastSlam1:
         m = C.c_int()
         _check(self.L, self.L.pfgpu_fs_shard_mode(self.h, C.byref(m)))
         return m.value
+
+    def post_shape(self):
+        """(tiles, threads, values per thread, "shared" or "global"): the fused post-step kernel's shape, and where its weight
+        tiles live (global memory for particle counts whose tile does not fit in shared memory)."""
+        t, nt, k, gl = C.c_uint(), C.c_uint(), C.c_uint(), C.c_int()
+        _check(self.L, self.L.pfgpu_fs_post_shape(self.h, C.byref(t), C.byref(nt), C.byref(k), C.byref(gl)))
+        return t.value, nt.value, k.value, "global" if gl.value else "shared"
 
     def time_main_kernel(self, on=True):
         _check(self.L, self.L.pfgpu_fs_time_main_kernel(self.h, int(on)))

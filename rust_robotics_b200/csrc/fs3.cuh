@@ -574,7 +574,7 @@ __device__ __forceinline__ double fs3_value(const Fs3Dev& d, int slot, size_t i,
     return i == 0 ? r0 : inv;
 }
 // exact by construction: one thread walks all values in order (bad values, too many dirty ones, failed certificate)
-template <int NT>
+template <int NT, bool GT = false>
 __device__ __noinline__ void fs3_serial_walk(const Fs3Dev& d, Fs3Sh<NT>& sh, unsigned K, int slot, double* out, int par, double S2, double r0, double inv) {
     if (threadIdx.x == 0) {
         const size_t T = (size_t)NT * K, lo = (size_t)blockIdx.x * T;
@@ -719,7 +719,7 @@ __device__ __forceinline__ void fs3_row_fill(const Fs3Dev& d, Fs3Sh<NT>& sh, int
 // (identical in every CTA).  pub = 1: the chain's leader also publishes the tile prefixes and the sorted dirty values, and *run
 // keeps this thread's state, so that fs3_xsum_emit can store the exact inclusive prefixes afterwards (sh.fail = 0; with
 // sh.fail = 1 the serial walk has already stored them to `out`).  Contains ONE grid barrier (`round`).
-template <int NT>
+template <int NT, bool GT = false>
 __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
                                         unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run,
                                         const Fs3Hook* hook = nullptr) {
@@ -941,7 +941,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
     }
     __syncthreads();
     FS3_TRACE(tb0 + 2);
-    if (sh.fail) { fs3_serial_walk<NT>(d, sh, K, slot, out, par, S2, r0, inv); return sh.total; }
+    if (sh.fail) { fs3_serial_walk<NT, GT>(d, sh, K, slot, out, par, S2, r0, inv); return sh.total; }
     if (run) { run->a_first = a_first; run->Pex = Pex; run->e_run = e_run; }
     return sh.total;
 }
@@ -951,7 +951,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
 // out[j], and the return value is 1 when some comb value may lie on the other side of it than of the CDF the reference computes
 // (x3_cdf_near_comb), or a clean run failed its certificate.  tend: the tile's last stored value goes to tileEnd[tile].
 // vals must still hold the values the sum saw.  Contains one block barrier.
-template <int NT>
+template <int NT, bool GT = false>
 __device__ __noinline__ int fs3_xsum_emit(const Fs3Dev& d, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
                                           double* out, int tend, const Fs3Cert* cert, int tslot) {
     const int tid = threadIdx.x, lane = tid & 31;
@@ -1046,13 +1046,19 @@ __device__ __forceinline__ unsigned fs3_cdf_search(const double* cdf, const doub
     return base + fs3_warp_search(cdf + base, len, r);
 }
 
-template <int NT>
+// GTILE = false: the tile of K x NT weights lives in dynamic shared memory.  GTILE = true: it lives in this CTA's slice of vtile
+// ([tiles][K][NT] doubles of global memory, the same layout: every access stays coalesced), for particle counts whose tile does not
+// fit on chip.  A value stored by one thread is read by another only behind a __syncthreads(), which orders global memory inside
+// a CTA too.
+template <int NT, bool GTILE>
 __global__ void __launch_bounds__(NT, 1)
 fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3ObsParam po, int k_last, double nth, uint64_t seed, unsigned step,
-                unsigned K, unsigned m32, int log2n, int early_launch) {
+                unsigned K, unsigned m32, int log2n, int early_launch, double* vtile) {
     pf_grid_dep_sync();
     if (early_launch) pf_grid_launch_dependents();
-    extern __shared__ __align__(16) double vals[];            // [K][NT]
+    double* vt;
+    { extern __shared__ __align__(16) double vals[]; vt = GTILE ? vtile + (size_t)blockIdx.x * NT * K : vals; }
+    double* const vals = vt;                                  // [K][NT]
     __shared__ Fs3Sh<NT> sh;
     Fs3State* st = d.st;
     const int tid = threadIdx.x;
@@ -1098,7 +1104,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.noise_call = step + 1u; hook.k_last = k_last; hook.po = &po;
     hook.par = par;
     Fs3Run run;
-    const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
+    const double S = fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff, 0, 0, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
     const int S_walked = sh.fail;
     FS3_TRACE(1);
     // ---------------- gate: neff = 1 / sum w^2 < NTH (compute_neff fs1.rs:186-193, fs1.rs:262-263) ----------------
@@ -1127,7 +1133,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         cp.S = S; cp.r0 = r0; cp.inv = inv; cp.ninv = (double)ng; cp.n = ng;
         cp.dl = g / (1.0 - g) * (1.0 + 9.5367431640625e-07);             // gamma_4n (1 + 2^-20)
         cp.ab = (4.0 * (double)ng + 4.0) * 4.9406564584124654e-324 + (double)(log2n + 4) * 1.1102230246251565e-16;
-        const int near = fs3_xsum_emit<NT>(d, sh, vals, K, m32, &run, 0, d.cum_all, 1, &cp, -1);
+        const int near = fs3_xsum_emit<NT, GTILE>(d, sh, vals, K, m32, &run, 0, d.cum_all, 1, &cp, -1);
         if (__syncthreads_or(near) && tid == 0) d.flagsg[FS3_CERT_FLAG] = 1;
         FS3_TRACE(4);
     }
@@ -1161,8 +1167,22 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         fs3_grid_sync<NT>(d, 6, nt);                           // wn_all is complete
         if (tid == 0) {
             double s = 0.0;
+            if constexpr (GTILE) {       // millions of values: sixteen loads in flight per trip, the adds in the same order
+                size_t i = 0;
 #pragma unroll 1
-            for (size_t i = 0; i < ng; ++i) { const double w = __ldcg(d.wn_all + i); s = s + w * w; }
+                for (; i + 16 <= ng; i += 16) {
+                    double2 w[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) w[u] = __ldcg(reinterpret_cast<const double2*>(d.wn_all + i) + u);
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) { s = s + w[u].x * w[u].x; s = s + w[u].y * w[u].y; }
+                }
+#pragma unroll 1
+                for (; i < ng; ++i) { const double w = __ldcg(d.wn_all + i); s = s + w * w; }
+            } else {
+#pragma unroll 1
+                for (size_t i = 0; i < ng; ++i) { const double w = __ldcg(d.wn_all + i); s = s + w * w; }
+            }
             sh.bcast = s;
             if (b == 0) st->border_cnt += 1;
         }
@@ -1189,7 +1209,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             if (b == 0 && tid == 0) st->cdf_exact += 1;
             // ---------------- resample() re-normalises first (fs1.rs:207) ----------------
             const double toff2 = S > 0.0 ? fs3_div(toff, S) : toff;
-            S2 = fs3_xsum<NT>(d, sh, vals, K, nt, toff2, 2, 1, m32, nullptr, par, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
+            S2 = fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff2, 2, 1, m32, nullptr, par, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
             FS3_TRACE(3);
             if (S2 > 0.0) {
 #pragma unroll 1
@@ -1197,8 +1217,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             }
             // ---------------- cum_sum fs1.rs:213-216 ----------------
             const double toff3 = S2 > 0.0 ? fs3_div(toff2, S2) : toff2;
-            (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, 1, &run);
-            (void)fs3_xsum_emit<NT>(d, sh, vals, K, m32, &run, 2, d.cum_all, 1, nullptr, 15);
+            (void)fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, 1, &run);
+            (void)fs3_xsum_emit<NT, GTILE>(d, sh, vals, K, m32, &run, 2, d.cum_all, 1, nullptr, 15);
             FS3_TRACE(4);
             // ---------------- the comb r, r + 1/n, ... accumulated sequentially (fs1.rs:219-230) ----------------
             if (log2n < 0) {                                   // n not a power of two: every add rounds -> exact scan
@@ -1206,8 +1226,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
                 for (unsigned k = 0; k < K; ++k) { const size_t i = g0 + k; vals[k * NT + tid] = i < ng ? (i == 0 ? r0 : inv) : 0.0; }
                 const double toff4 = b == 0 ? 0.0 : r0 + ((double)((size_t)b * T) - 1.0) * inv;
                 __syncthreads();
-                (void)fs3_xsum<NT>(d, sh, vals, K, nt, toff4, 4, 3, m32, d.rcomb_all, par, S2, r0, inv, 0.0, 1, &run);
-                (void)fs3_xsum_emit<NT>(d, sh, vals, K, m32, &run, 3, d.rcomb_all, 0, nullptr, -1);
+                (void)fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff4, 4, 3, m32, d.rcomb_all, par, S2, r0, inv, 0.0, 1, &run);
+                (void)fs3_xsum_emit<NT, GTILE>(d, sh, vals, K, m32, &run, 3, d.rcomb_all, 0, nullptr, -1);
             }
             fs3_grid_sync<NT>(d, cert ? 5 : 4, nt);            // the whole CDF (and comb) is visible
             FS3_TRACE(5);

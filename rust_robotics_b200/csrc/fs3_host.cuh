@@ -25,6 +25,8 @@ struct pfgpu_fs {
     int variant = 1;                  // 1 = FastSLAM 1.0 (fs1.rs), 2 = FastSLAM 2.0 (fs2.rs); pfgpu_fs_set_variant
     int ekf_helpers = 0;              // PFGPU_EKF_HELPERS: cap on the helper warps per CTA (0 = as many as fit, at most 3)
     int post_nt = 256; unsigned post_K = 1, post_tiles = 1, m32 = 0; int log2n = -1; size_t post_smem = 0;
+    bool post_global = false;         // the post kernel keeps its weight tiles in global memory (fs3_post_kernel<512, true>) ...
+    double* vtile = nullptr;          // ... here: [post_tiles][post_K][512]
 };
 
 extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.rs:13-23
@@ -32,11 +34,11 @@ extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.
     c->init_weight = 1.0 / 100.0;
 }
 
-template <int NT>
+template <int NT, bool GTILE>
 static int fs3_post_prepare(pfgpu_fs* h) {
-    if (cudaFuncSetAttribute(fs3_post_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
+    if (cudaFuncSetAttribute(fs3_post_kernel<NT, GTILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
     int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fs3_post_kernel<NT>, NT, h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fs3_post_kernel<NT, GTILE>, NT, h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
     return (size_t)nb * (size_t)h->ctx.num_sms >= h->post_tiles ? 0 : 1;
 }
 
@@ -84,10 +86,24 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         h->m32 = x3_margin32(n_global);
         h->log2n = -1;
         for (int p = 0; p < 32; ++p) if (((size_t)1 << p) == n_global) h->log2n = p;
-        int bad = h->post_nt == 512 ? fs3_post_prepare<512>(h) : fs3_post_prepare<256>(h);
+        // PFGPU_POST_SMEM_CAP=<bytes> (tests): the most dynamic shared memory the weight tile may take (default: what the device allows)
+        const char* ec = getenv("PFGPU_POST_SMEM_CAP");
+        const bool capped = ec && ec[0] && (size_t)strtoull(ec, nullptr, 10) < h->post_smem;
+        int bad = capped || (h->post_nt == 512 ? fs3_post_prepare<512, false>(h) : fs3_post_prepare<256, false>(h));
         if (bad || h->post_tiles > FS3_MAX_TILES || h->post_tiles > (unsigned)h->post_nt) {
-            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "%zu particles do not fit the fused post-step kernel (%u tiles x %zu B of shared memory)", n_global, h->post_tiles, h->post_smem);
-            return fail(PFGPU_ERR_UNSUPPORTED);
+            // the tile does not fit on chip: one tile of 512 threads per SM, its K x 512 weights in global memory (vtile)
+            h->post_global = true;
+            h->post_nt = 512;
+            unsigned tiles = (unsigned)std::min<int>(FS3_MAX_TILES, h->ctx.num_sms);
+            { const char* ew = getenv("PFGPU_POST_TILES"); if (ew && atoi(ew) >= 1 && atoi(ew) <= (int)tiles) tiles = (unsigned)atoi(ew); }
+            K = (unsigned)((n_global + (size_t)tiles * 512 - 1) / ((size_t)tiles * 512));
+            h->post_K = K;
+            h->post_tiles = (unsigned)((n_global + (size_t)512 * K - 1) / ((size_t)512 * K));
+            h->post_smem = 0;
+            if (fs3_post_prepare<512, true>(h)) {
+                snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "the post-step kernel cannot keep %u CTAs co-resident on this device", h->post_tiles);
+                return fail(PFGPU_ERR_UNSUPPORTED);
+            }
         }
     }
     // ONE allocation for everything a peer may touch, same layout on every rank: one IPC mapping per peer exposes all of it
@@ -146,6 +162,7 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         FS_TRY(cudaHostAlloc(&h->h_rec, sizeof(Fs3Rec), cudaHostAllocMapped));
         memset(h->h_rec, 0, sizeof(Fs3Rec));
         FS_TRY(cudaHostGetDevicePointer((void**)&d.rec, h->h_rec, 0));
+        if (h->post_global) FS_TRY(cudaMalloc(&h->vtile, (size_t)h->post_tiles * h->post_K * 512 * sizeof(double)));
         if (getenv("PFGPU_POST_TRACE")) { FS_TRY(cudaMalloc(&d.trace, 48 * sizeof(unsigned long long))); FS_TRY(cudaMemset(d.trace, 0, 48 * sizeof(unsigned long long))); }
     }
     { const char* e5 = getenv("PFGPU_PDL"); h->pdl = !(e5 && e5[0] == '0'); }
@@ -240,7 +257,7 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(d.tileP); cudaFree(d.tileQ); cudaFree(d.entCnt); cudaFree(d.entKey); cudaFree(d.entTile); cudaFree(d.entP); cudaFree(d.entV); cudaFree(d.entL);
     cudaFree(d.bar); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
-    cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->stage);
+    cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage);
     if (h->h_rec) cudaFreeHost(h->h_rec);
     if (h->comm) ncclCommDestroy(h->comm);
     marks_free(h->marks);
@@ -417,10 +434,12 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
         PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
     }
     // normalise, N_eff gate and (when it opens) the whole resample: one launch
-    if (h->post_nt == 512)
-        PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_post_kernel<512>, h->post_tiles, 512, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0);
+    if (h->post_global)
+        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, true>), h->post_tiles, 512, 0, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    else if (h->post_nt == 512)
+        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, false>), h->post_tiles, 512, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
     else
-        PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_post_kernel<256>, h->post_tiles, 256, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0);
+        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<256, false>), h->post_tiles, 256, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
     h->n_step++;
     h->steps++;
     if (did) {     // the gate lives on the device; only a caller who asks pays a sync
@@ -551,6 +570,14 @@ extern "C" int pfgpu_fs_post_trace(pfgpu_fs* h, unsigned long long* out32) {
         PF_CUDA(cudaMemcpy(t8, h->d.trace + 32, 9 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
         out32[7] = t8[0]; out32[24] = t8[1]; out32[25] = t8[2]; out32[26] = t8[3]; out32[27] = t8[8];
     }
+    return 0;
+}
+extern "C" int pfgpu_fs_post_shape(pfgpu_fs* h, unsigned* tiles, unsigned* threads, unsigned* values_per_thread, int* global_tile) {
+    if (!h) return PFGPU_ERR_INVALID;
+    if (tiles) *tiles = h->post_tiles;
+    if (threads) *threads = (unsigned)h->post_nt;
+    if (values_per_thread) *values_per_thread = h->post_K;
+    if (global_tile) *global_tile = h->post_global ? 1 : 0;
     return 0;
 }
 extern "C" int pfgpu_fs_time_main_kernel(pfgpu_fs* h, int on) {

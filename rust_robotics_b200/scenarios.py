@@ -78,6 +78,12 @@ def bigmap_scenario(steps=110, seed=42):
     return FastSlamScenario(128, (635.0, 595.0, 0.0), (1.0, 0.025), steps, seed)
 
 
+def particles_scenario(steps=110, seed=42):
+    """the particle-count sweep (bench_particles.py): 36 landmarks (6 x 6 grid, 10 m pitch); the robot drives a 20 m circle
+    (u = (1.0, 0.05)) about the middle of the grid, so it sees most of the map every step"""
+    return FastSlamScenario(6, (25.0, 5.0, 0.0), (1.0, 0.05), steps, seed)
+
+
 class PfScenario:
     """C1: the scenario of crates/rust_robotics/examples/render_gif_particle_filter.rs:21-79 (5 landmarks, rounded
     rectangle drive, obs = max(range + N(0, 0.15), 0)); C2: 360 landmarks on a 30 m circle, u = (1.0, 0.03)."""
