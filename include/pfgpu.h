@@ -161,6 +161,29 @@ int  pfgpu_fs_last_gate(pfgpu_fs*, int* did_resample);     /* whether the last s
  * between steps; every rank of a sharded engine must make the same call. */
 int  pfgpu_fs_set_variant(pfgpu_fs*, int variant);
 int  pfgpu_fs_count(pfgpu_fs*, size_t* n_local, size_t* n_global, size_t* n_landmarks);
+/* Estimate (not in the reference, whose callers read the best particle's map, keeping landmarks with cov00 < 100).  With W the sum
+ * of the stored weights (never assumed to be 1):
+ *   pose      weighted mean and 3x3 covariance of (x, y, yaw); yaw deviations are wrapped differences from a centre c, the mean
+ *             yaw is wrapped to [-pi, pi].  c = the current pose of the last particle (global index n - 1), read from the state at
+ *             every call (after upload / seed_map too), so it is always a member of the cloud.
+ *   landmark  over the particles whose copy passes cov00 < cov00_max: mass = (sum of their weights) / W, mean = weighted mean of
+ *             the copies' (x, y), cov = sum w (P + (mu - mean)(mu - mean)^T) / sum w in (c00, c01, c10, c11) order.
+ * mass 0: mean and cov are NaN.  W <= 0 or not finite: everything NaN, every mass 0 (a status of 0: the state has no mean).
+ * Two steps, so that a sharded engine needs no cross-rank synchronisation inside the library:
+ * pfgpu_fs_moments: moments of the particles this handle owns (one GPU: all of them) of the deviations from the centre c, which
+ *   every rank reads bit for bit (through the peer mapping when sharded): total weight, weighted mean, and central second
+ *   moments m2 = sum w (d - mean)(d - mean)^T.  lm (nullable: pose only) receives n_landmarks entries.  Synchronises and returns through host memory.  Valid
+ *   where pfgpu_fs_download is: on a sharded engine no rank may step until every rank's call has returned.  cov00_max = INFINITY
+ *   takes every copy; NaN is invalid. */
+typedef struct { double w; double c[3]; double mean[3]; double m2[6]; } pfgpu_fs_pose_moments; /* m2: xx xy xyaw yy yyaw yawyaw */
+typedef struct { double w; double mean[2]; double m2[4]; } pfgpu_fs_lm_moments;               /* m2 = sum w (P + d d^T), lm6 order */
+int  pfgpu_fs_moments(pfgpu_fs*, double cov00_max, pfgpu_fs_pose_moments* pose, pfgpu_fs_lm_moments* lm);
+/* Host only: merge `world` ranks' moments in rank order and finalise.  lm: [world] pointers to n_landmarks entries each, or NULL
+ * (pose only).  Every output is nullable; pose_cov9_colmajor is column-major (nalgebra Matrix3), lm_mean2 n_landmarks x 2,
+ * lm_cov4 n_landmarks x 4 (c00, c01, c10, c11).  Ranks merge with the pairwise (Chan) update; moments about different centres
+ * are invalid. */
+int  pfgpu_fs_estimate_merge(const pfgpu_fs_pose_moments* pose, const pfgpu_fs_lm_moments* const* lm, int world, size_t n_landmarks,
+                             double pose_mean3[3], double pose_cov9_colmajor[9], double* lm_mass, double* lm_mean2, double* lm_cov4);
 int  pfgpu_fs_sync(pfgpu_fs*);
 
 /* ============================================ plumbing ============================================== */

@@ -7,6 +7,7 @@ Names and argument meanings follow the Rust reference so the parity tests read l
 Errors: status < 0 -> InvalidParameter (RoboticsError::InvalidParameter, rust_robotics_core/src/error.rs:8-24);
 status > 0 -> PfgpuError (CUDA/NCCL).  No CPU fallback exists.
 """
+import collections
 import ctypes as C
 import math
 import os
@@ -51,6 +52,15 @@ class Stats(C.Structure):
                 ("imported_particles", C.c_uint64)]
 
 
+class _FsPoseMoments(C.Structure):
+    _fields_ = [("w", C.c_double), ("c", C.c_double * 3), ("mean", C.c_double * 3), ("m2", C.c_double * 6)]
+
+
+# FastSlam1.estimate(): pose (3,) mean of (x, y, yaw), pose_cov (3, 3); per landmark (None when not asked for) mass (m,),
+# mean (m, 2), cov (m, 2, 2)
+FsEstimate = collections.namedtuple("FsEstimate", ["pose", "pose_cov", "mass", "mean", "cov"])
+
+
 EXPORTS = [
     "pfgpu_strerror", "pfgpu_last_error", "pfgpu_device_count",
     "pfgpu_pf_default_config", "pfgpu_pf_config_validate", "pfgpu_pf_create", "pfgpu_pf_create_sharded",
@@ -63,6 +73,7 @@ EXPORTS = [
     "pfgpu_nccl_unique_id", "pfgpu_pf_stats", "pfgpu_fs_stats", "pfgpu_pf_time_main_kernel",
     "pfgpu_fs_time_main_kernel", "pfgpu_pf_mark", "pfgpu_pf_elapsed_ms", "pfgpu_fs_mark", "pfgpu_fs_elapsed_ms",
     "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
+    "pfgpu_fs_moments", "pfgpu_fs_estimate_merge",
 ]
 
 
@@ -135,6 +146,8 @@ def load_library():
     L.pfgpu_fs_post_trace.argtypes = [vp, C.POINTER(C.c_ulonglong)]
     L.pfgpu_fs_post_shape.argtypes = [vp, C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_int)]
     L.pfgpu_fs_shard_mode.argtypes = [vp, C.POINTER(C.c_int)]
+    L.pfgpu_fs_moments.argtypes = [vp, C.c_double, C.POINTER(_FsPoseMoments), c_dp]
+    L.pfgpu_fs_estimate_merge.argtypes = [C.POINTER(_FsPoseMoments), C.POINTER(c_dp), C.c_int, C.c_size_t, c_dp, c_dp, c_dp, c_dp, c_dp]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
     _LIB = L
@@ -553,6 +566,43 @@ class FastSlam1:
         t, nt, k, gl = C.c_uint(), C.c_uint(), C.c_uint(), C.c_int()
         _check(self.L, self.L.pfgpu_fs_post_shape(self.h, C.byref(t), C.byref(nt), C.byref(k), C.byref(gl)))
         return t.value, nt.value, k.value, "global" if gl.value else "shared"
+
+    # -- estimate (no reference counterpart: fs1.rs's callers read the best particle's map, keeping landmarks with cov00 < 100) --
+    def moments(self, cov00_max=100.0, landmarks=True):
+        """pfgpu_fs_moments: (pose moments, (m, 7) landmark moments or None) of the particles this handle owns"""
+        pose = _FsPoseMoments()
+        lm = np.empty((self.m, 7)) if landmarks else None
+        _check(self.L, self.L.pfgpu_fs_moments(self.h, float(cov00_max), C.byref(pose), _dp(lm) if lm is not None else None))
+        return pose, lm
+
+    @staticmethod
+    def merge_moments(moments):
+        """pfgpu_fs_estimate_merge over [(pose moments, landmark moments or None)] in rank order -> FsEstimate"""
+        L = load_library()
+        world = len(moments)
+        poses = (_FsPoseMoments * world)(*[p for p, _ in moments])
+        lms = [l for _, l in moments]
+        with_lm = lms[0] is not None
+        m = lms[0].shape[0] if with_lm else 0
+        mean, cov = np.empty(3), np.empty(9)
+        mass, lmean, lcov = (np.empty(m), np.empty((m, 2)), np.empty((m, 2, 2))) if with_lm else (None, None, None)
+        ptrs = (c_dp * world)(*[_dp(l) for l in lms]) if with_lm else None
+        _check(L, L.pfgpu_fs_estimate_merge(poses, ptrs, world, m, _dp(mean), _dp(cov), *(_dp(a) if a is not None else None for a in (mass, lmean, lcov))))
+        return FsEstimate(mean, cov.reshape(3, 3).T, mass, lmean, lcov)
+
+    def estimate(self, cov00_max=100.0, landmarks=True):
+        """Weighted posterior estimate (DESIGN §3.4): FsEstimate(pose (3,), pose_cov (3, 3), mass (m,), mean (m, 2), cov (m, 2, 2));
+        the landmark fields are None with landmarks=False.  Only landmark copies with cov00 < cov00_max count (the examples'
+        filter; inf takes every copy).  Synchronises."""
+        return self.merge_moments([self.moments(cov00_max, landmarks)])
+
+    @staticmethod
+    def estimate_all(ranks, cov00_max=100.0, landmarks=True):
+        """estimate() of an in-process sharded engine (create_sharded_local): synchronises every rank, then collects their moments
+        and merges them in rank order"""
+        for g in ranks:
+            g.sync()
+        return FastSlam1.merge_moments([g.moments(cov00_max, landmarks) for g in ranks])
 
     def time_main_kernel(self, on=True):
         _check(self.L, self.L.pfgpu_fs_time_main_kernel(self.h, int(on)))

@@ -2,6 +2,7 @@
 // Included by pfgpu.cu after the shared helpers (Ctx, Marks, KernelTimer, PF_NCCL, ...).
 #pragma once
 #include "fs3.cuh"
+#include "fs3_est.cuh"
 
 struct pfgpu_fs {
     Ctx ctx;
@@ -27,6 +28,7 @@ struct pfgpu_fs {
     int post_nt = 256; unsigned post_K = 1, post_tiles = 1, m32 = 0; int log2n = -1; size_t post_smem = 0;
     bool post_global = false;         // the post kernel keeps its weight tiles in global memory (fs3_post_kernel<512, true>) ...
     double* vtile = nullptr;          // ... here: [post_tiles][post_K][512]
+    char* est = nullptr; size_t est_bytes = 0;   // pfgpu_fs_moments scratch, allocated by the first call (fs3_est.cuh)
 };
 
 extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.rs:13-23
@@ -257,7 +259,7 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(d.tileP); cudaFree(d.tileQ); cudaFree(d.entCnt); cudaFree(d.entKey); cudaFree(d.entTile); cudaFree(d.entP); cudaFree(d.entV); cudaFree(d.entL);
     cudaFree(d.bar); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
-    cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage);
+    cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage); cudaFree(h->est);
     if (h->h_rec) cudaFreeHost(h->h_rec);
     if (h->comm) ncclCommDestroy(h->comm);
     marks_free(h->marks);
@@ -586,5 +588,101 @@ extern "C" int pfgpu_fs_time_main_kernel(pfgpu_fs* h, int on) {
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     timer_drain(h->timer);
     h->timer.on = on != 0; h->timer.ms_sum = 0.0; h->timer.count = 0;
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// estimate (DESIGN §3.4): pfgpu_fs_moments on the device, pfgpu_fs_estimate_merge on the host
+// ---------------------------------------------------------------------------------------------------------------------
+static_assert(sizeof(pfgpu_fs_lm_moments) == sizeof(Fs3LmMom), "pfgpu_fs_lm_moments is Fs3LmMom");
+static_assert(sizeof(pfgpu_fs_pose_moments) == sizeof(double) * 3 + sizeof(Fs3PoseMom), "pfgpu_fs_pose_moments: w, c[3], mean[3], m2[6]");
+static_assert(sizeof(Fs3PoseMom) == FS3_EST_POSE_SUMS * sizeof(double) && FS3_EST_POSE_MAX_BLOCKS <= FS3_EST_NT, "pose partials");
+
+// chunks of the map pass: enough (chunk, landmark) warps to fill the GPU, at least 32 slots per chunk, and at most
+// FS3_EST_SCRATCH_CAP bytes of chunk partials; depends on (n, m) only
+static void fs3_est_shape(size_t n, size_t m, unsigned* chunk, unsigned* nchunks) {
+    size_t nc = (FS3_EST_TARGET_WARPS + m - 1) / m;
+    nc = std::min(nc, (n + 31) / 32);
+    nc = std::min(nc, std::max<size_t>(1, FS3_EST_SCRATCH_CAP / (m * sizeof(Fs3LmMom))));
+    if (nc < 1) nc = 1;
+    const size_t ch = ((n + nc - 1) / nc + 31) / 32 * 32;
+    *chunk = (unsigned)ch;
+    *nchunks = (unsigned)((n + ch - 1) / ch);
+}
+
+extern "C" int pfgpu_fs_moments(pfgpu_fs* h, double cov00_max, pfgpu_fs_pose_moments* pose, pfgpu_fs_lm_moments* lm) {
+    if (!h || !pose || std::isnan(cov00_max)) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));          // (a time-out of the last step surfaces here)
+    int rc = fs_check_err(h);
+    if (rc) return rc;
+    const Fs3Dev& d = h->d;
+    const bool map = lm && d.m;
+    unsigned chunk = 0, nch = 0;
+    if (map) fs3_est_shape(d.n, d.m, &chunk, &nch);
+    const unsigned pblocks = std::min<unsigned>(cdiv_u(d.n, 4 * FS3_EST_NT), FS3_EST_POSE_MAX_BLOCKS);
+    // scratch: ticket | pose block partials | pose moments | map chunk partials | map moments
+    const size_t o_part = 256, o_pose = o_part + (size_t)FS3_EST_POSE_MAX_BLOCKS * FS3_EST_POSE_SUMS * sizeof(double), o_lmp = o_pose + 256;
+    const size_t o_lmo = o_lmp + (map ? (size_t)d.m * nch * sizeof(Fs3LmMom) : 0), need = o_lmo + (map ? (size_t)d.m * sizeof(Fs3LmMom) : 0);
+    if (need > h->est_bytes) {
+        if (h->est) { cudaFree(h->est); h->est = nullptr; h->est_bytes = 0; }
+        PF_CUDA(cudaMalloc(&h->est, need));
+        PF_CUDA(cudaMemset(h->est, 0, 256));
+        h->est_bytes = need;
+    }
+    char* E = h->est;
+    PF_LAUNCH(h->ctx, fs3_est_pose_kernel, pblocks, FS3_EST_NT, 0, d, reinterpret_cast<Fs3PoseMom*>(E + o_part), reinterpret_cast<unsigned*>(E),
+              reinterpret_cast<double*>(E + o_pose));
+    if (map) {
+        dim3 grid(nch, cdiv_u(d.m, FS3_EST_NT / 32));
+        PF_LAUNCH(h->ctx, fs3_est_map_kernel, grid, FS3_EST_NT, 0, d, cov00_max, chunk, reinterpret_cast<Fs3LmMom*>(E + o_lmp));
+        PF_LAUNCH(h->ctx, fs3_est_merge_kernel, cdiv_u(d.m, FS3_EST_NT / 32), FS3_EST_NT, 0, reinterpret_cast<const Fs3LmMom*>(E + o_lmp), nch, d.m,
+                  reinterpret_cast<Fs3LmMom*>(E + o_lmo));
+        PF_CUDA(cudaMemcpyAsync(lm, E + o_lmo, (size_t)d.m * sizeof(Fs3LmMom), cudaMemcpyDeviceToHost, h->ctx.stream));
+    }
+    PF_CUDA(cudaMemcpyAsync(pose, E + o_pose, sizeof(*pose), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return fs_check_err(h);
+}
+
+extern "C" int pfgpu_fs_estimate_merge(const pfgpu_fs_pose_moments* pose, const pfgpu_fs_lm_moments* const* lm, int world, size_t m,
+                                       double pose_mean3[3], double pose_cov9_colmajor[9], double* lm_mass, double* lm_mean2, double* lm_cov4) {
+    if (!pose || world < 1) return PFGPU_ERR_INVALID;
+    for (int g = 0; g < world; ++g) {
+        if (memcmp(pose[g].c, pose[0].c, sizeof(pose[0].c)) != 0) return PFGPU_ERR_INVALID;   // moments about different centres
+        if (lm && m && !lm[g]) return PFGPU_ERR_INVALID;
+    }
+    Fs3PoseMom acc = {0.0, {0.0, 0.0, 0.0}, {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}};
+    for (int g = 0; g < world; ++g) {
+        Fs3PoseMom b;
+        b.w = pose[g].w;
+        for (int k = 0; k < 3; ++k) b.m[k] = pose[g].mean[k];
+        for (int k = 0; k < 6; ++k) b.q[k] = pose[g].m2[k];
+        fs3_pose_merge(acc, b);
+    }
+    const double W = acc.w;
+    const bool ok = W > 0.0 && std::isfinite(W);
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    if (pose_mean3 || pose_cov9_colmajor) {
+        double mean[3], cov[9];
+        mean[0] = pose[0].c[0] + acc.m[0]; mean[1] = pose[0].c[1] + acc.m[1]; mean[2] = fs3_wrap_angle(pose[0].c[2] + acc.m[2]);
+        static const int ix[3][3] = {{0, 1, 2}, {1, 3, 4}, {2, 4, 5}};
+        for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j) cov[3 * j + i] = acc.q[ix[i][j]] / W;
+        if (pose_mean3) for (int k = 0; k < 3; ++k) pose_mean3[k] = ok ? mean[k] : nan;
+        if (pose_cov9_colmajor) for (int k = 0; k < 9; ++k) pose_cov9_colmajor[k] = ok ? cov[k] : nan;
+    }
+    if (!lm) return 0;
+    for (size_t l = 0; l < m; ++l) {
+        Fs3LmMom acc = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int g = 0; g < world; ++g) fs3_mom_merge(acc, reinterpret_cast<const Fs3LmMom*>(lm[g])[l]);
+        const bool some = ok && acc.w != 0.0;
+        if (lm_mass) lm_mass[l] = some ? acc.w / W : 0.0;
+        if (lm_mean2) { lm_mean2[2 * l] = some ? acc.mx : nan; lm_mean2[2 * l + 1] = some ? acc.my : nan; }
+        if (lm_cov4) {
+            lm_cov4[4 * l] = some ? acc.m00 / acc.w : nan; lm_cov4[4 * l + 1] = some ? acc.m01 / acc.w : nan;
+            lm_cov4[4 * l + 2] = some ? acc.m10 / acc.w : nan; lm_cov4[4 * l + 3] = some ? acc.m11 / acc.w : nan;
+        }
+    }
     return 0;
 }

@@ -13,6 +13,12 @@ namespace rust_robotics_b200 { namespace fastslam1 {
 struct Landmark { double x, y; std::array<double, 4> cov; };              // fs1.rs:27-31 (cov row-major c00 c01 c10 c11)
 struct Particle { double weight, x, y, yaw; std::vector<Landmark> landmarks; };   // fs1.rs:45-51
 using Observation = std::tuple<double, double, size_t>;                   // (distance, angle, landmark_id) fs1.rs:240
+// weighted posterior estimate (no reference counterpart; include/pfgpu.h pfgpu_fs_moments): pose mean (x, y, yaw) and covariance
+// (column-major), per landmark the weight mass of the copies with cov00 < cov00_max, their mean and mixture covariance
+struct Estimate {
+    std::array<double, 3> pose; std::array<double, 9> pose_cov;
+    std::vector<double> mass; std::vector<std::array<double, 2>> mean; std::vector<std::array<double, 4>> cov;
+};
 
 class FastSlam {
     pfgpu_fs* h_ = nullptr;
@@ -54,6 +60,19 @@ public:
             for (size_t l = 0; l < m_; ++l) { const double* q = &lm[(i * m_ + l) * 6]; out[i].landmarks.push_back({q[0], q[1], {q[2], q[3], q[4], q[5]}}); }
         }
         return out;
+    }
+    // pfgpu_fs_moments + pfgpu_fs_estimate_merge on this (one-GPU) engine; landmarks = false: pose only
+    Estimate estimate(double cov00_max = 100.0, bool landmarks = true) const {
+        pfgpu_fs_pose_moments pm;
+        std::vector<pfgpu_fs_lm_moments> lm(landmarks ? m_ : 0);
+        check(pfgpu_fs_moments(h_, cov00_max, &pm, landmarks ? lm.data() : nullptr), "estimate");
+        Estimate e;
+        const size_t m = lm.size();
+        e.mass.resize(m); e.mean.resize(m); e.cov.resize(m);
+        const pfgpu_fs_lm_moments* one = lm.data();
+        check(pfgpu_fs_estimate_merge(&pm, landmarks ? &one : nullptr, 1, m, e.pose.data(), e.pose_cov.data(), e.mass.data(),
+                                      m ? e.mean[0].data() : nullptr, m ? e.cov[0].data() : nullptr), "estimate");
+        return e;
     }
     size_t len() const { return n_; }
     // 1 = fastslam1::fastslam_update, 2 = fastslam2::fastslam2_update (crates/rust_robotics_slam/src/fastslam2.rs:376-383)

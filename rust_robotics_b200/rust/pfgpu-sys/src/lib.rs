@@ -22,6 +22,15 @@ pub struct pfgpu_pf_config {
     pub kld_epsilon: f64,
     pub kld_z: f64,
 }
+/// pfgpu_fs_moments: weight, mean and central second moments (m2: xx xy xyaw yy yyaw yawyaw) of one handle's pose deviations
+/// from the centre `c`
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct pfgpu_fs_pose_moments { pub w: f64, pub c: [f64; 3], pub mean: [f64; 3], pub m2: [f64; 6] }
+/// per landmark: weight of the copies that passed cov00 < cov00_max, their mean, sum w (P + d d^T) in (c00, c01, c10, c11) order
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct pfgpu_fs_lm_moments { pub w: f64, pub mean: [f64; 2], pub m2: [f64; 4] }
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct pfgpu_fs_config {
@@ -79,6 +88,11 @@ extern "C" {
     pub fn pfgpu_fs_particle_landmarks(h: *mut pfgpu_fs, index_local: usize, lm6: *mut f64) -> c_int;
     pub fn pfgpu_fs_count(h: *mut pfgpu_fs, n_local: *mut usize, n_global: *mut usize, n_landmarks: *mut usize) -> c_int;
     pub fn pfgpu_fs_sync(h: *mut pfgpu_fs) -> c_int;
+    // estimate (no reference counterpart): moments per handle, then a host-only merge over the ranks in rank order
+    pub fn pfgpu_fs_moments(h: *mut pfgpu_fs, cov00_max: f64, pose: *mut pfgpu_fs_pose_moments, lm: *mut pfgpu_fs_lm_moments) -> c_int;
+    pub fn pfgpu_fs_estimate_merge(pose: *const pfgpu_fs_pose_moments, lm: *const *const pfgpu_fs_lm_moments, world: c_int, n_landmarks: usize,
+                                   pose_mean3: *mut f64, pose_cov9_colmajor: *mut f64, lm_mass: *mut f64, lm_mean2: *mut f64,
+                                   lm_cov4: *mut f64) -> c_int;
     pub fn pfgpu_pf_sync(h: *mut pfgpu_pf) -> c_int;
     // multi-GPU: one process per GPU; rank 0 makes the id, the host program broadcasts its 128 bytes, every rank creates
     // its shard with the GLOBAL particle count (INTEGRATION.md "Multi-GPU")

@@ -1,13 +1,17 @@
 //! FastSLAM 1.0 over the GPU engine — mirrors crates/rust_robotics_slam/src/fastslam1.rs.
 //! The reference's functions mutate a caller-owned `Vec<Particle>`; here the particles live on the device inside
 //! `FastSlam` (SURVEY.md §8b) and `download()` materialises the reference's `Vec<Particle>` when a caller wants it.
-use nalgebra::{Matrix2, Vector2};
+use nalgebra::{Matrix2, Matrix3, Vector2, Vector3};
 use pfgpu_sys as sys;
 
 #[derive(Clone)]
 pub struct Landmark { pub x: f64, pub y: f64, pub cov: Matrix2<f64> }                  // fs1.rs:27-31
 #[derive(Clone)]
 pub struct Particle { pub weight: f64, pub x: f64, pub y: f64, pub yaw: f64, pub landmarks: Vec<Landmark> }   // fs1.rs:45-51
+
+/// FastSlam::estimate (no reference counterpart; include/pfgpu.h pfgpu_fs_moments): weighted pose mean (x, y, yaw) and covariance;
+/// per landmark the weight mass of the copies with cov00 < cov00_max, their weighted mean and mixture covariance (NaN at mass 0)
+pub struct Estimate { pub pose: Vector3<f64>, pub pose_cov: Matrix3<f64>, pub mass: Vec<f64>, pub mean: Vec<Vector2<f64>>, pub cov: Vec<Matrix2<f64>> }
 
 pub struct FastSlam { h: *mut sys::pfgpu_fs, n: usize, m: usize, calls: u32 }
 unsafe impl Send for FastSlam {}
@@ -54,6 +58,24 @@ pub fn get_best_particle(particles: &FastSlam) -> Particle {
 }
 impl FastSlam {
     pub fn len(&self) -> usize { self.n }
+    /// the posterior estimate over all particles (what render_gif_slam.rs:183-191 reads from the best particle, with its
+    /// `cov[(0,0)] < 100` filter as `cov00_max = 100.0`); `landmarks = false`: pose only, empty landmark vectors
+    pub fn estimate(&self, cov00_max: f64, landmarks: bool) -> Estimate {
+        let mut pm = sys::pfgpu_fs_pose_moments::default();
+        let m = if landmarks { self.m } else { 0 };
+        let mut lm = vec![sys::pfgpu_fs_lm_moments::default(); m];
+        let rc = unsafe { sys::pfgpu_fs_moments(self.h, cov00_max, &mut pm, if landmarks { lm.as_mut_ptr() } else { std::ptr::null_mut() }) };
+        assert_eq!(rc, 0, "pfgpu_fs_moments failed");
+        let (mut mean3, mut cov9) = ([0.0f64; 3], [0.0f64; 9]);
+        let (mut mass, mut mean2, mut cov4) = (vec![0.0f64; m], vec![0.0f64; 2 * m], vec![0.0f64; 4 * m]);
+        let one = [lm.as_ptr()];
+        let rc = unsafe { sys::pfgpu_fs_estimate_merge(&pm, if landmarks { one.as_ptr() } else { std::ptr::null() }, 1, m, mean3.as_mut_ptr(),
+                                                        cov9.as_mut_ptr(), mass.as_mut_ptr(), mean2.as_mut_ptr(), cov4.as_mut_ptr()) };
+        assert_eq!(rc, 0, "pfgpu_fs_estimate_merge failed");
+        Estimate { pose: Vector3::from_column_slice(&mean3), pose_cov: Matrix3::from_column_slice(&cov9), mass,
+                   mean: mean2.chunks(2).map(|q| Vector2::new(q[0], q[1])).collect(),
+                   cov: cov4.chunks(4).map(|q| Matrix2::new(q[0], q[1], q[2], q[3])).collect() }
+    }
     pub(crate) fn raw(&self) -> *mut sys::pfgpu_fs { self.h }
     /// the reference's Vec<Particle>, materialised (checkpoint / API-compat)
     pub fn download(&self) -> Vec<Particle> {

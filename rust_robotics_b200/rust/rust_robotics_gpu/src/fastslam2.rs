@@ -5,7 +5,7 @@
 use nalgebra::Vector2;
 use pfgpu_sys as sys;
 
-pub use crate::fastslam1::{get_best_particle, get_observations, FastSlam, Landmark, Particle};
+pub use crate::fastslam1::{get_best_particle, get_observations, Estimate, FastSlam, Landmark, Particle};
 
 /// create_particles fs2.rs:418-422
 pub fn create_particles(n_particles: usize, n_landmarks: usize) -> FastSlam {
