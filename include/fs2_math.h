@@ -133,4 +133,33 @@ PFC_HD void fs2_propose_pose(double* px, double* py, double* pyaw, const FsLm* L
     *px = out[0]; *py = out[1]; *pyaw = fs_normalize_angle(out[2]);   /* set_pose fs2.rs:77-81 */
 }
 
+/* The association metric of the unknown-correspondence step (DESIGN §3.5): the squared Mahalanobis distance y^T S^-1 y of
+ * observation (z0, z1) from landmark L seen at pose (px, py, pyaw).  y and S are formed exactly as update_landmark_and_weight
+ * forms them (fs2.rs:258-262), S^-1 as try_inverse forms it and the quadratic form in fs2.rs:275's order (the rule itself is
+ * search_correspond_landmark_id of ekf_slam.rs:284-308).  Returns 0 when det S == 0 (try_inverse fails: the slot is skipped,
+ * ekf_slam.rs:293), else 1 with the distance in *d2 (NaN / inf pass through).  The caller tests `cov00 < 100` first. */
+PFC_HD int fs_assoc_d2(const FsLm* L, double px, double py, double pyaw, double z0, double z1, double r00, double r11, double* d2out) {
+    const double dx = L->x - px, dy = L->y - py;
+    const double d2 = dx * dx + dy * dy;
+    const double d = sqrt(d2);
+    const double zp1 = fs_normalize_angle(pfc_atan2(dy, dx) - pyaw);
+    const double y0 = z0 - d, y1 = fs_normalize_angle(z1 - zp1);
+    const pfc_rcp_t rd = pfc_rcp_make(d), rd2 = pfc_rcp_make(d2);
+    const double h00 = pfc_div_by(dx, rd), h01 = pfc_div_by(dy, rd), h10 = pfc_div_by(-dy, rd2), h11 = pfc_div_by(dx, rd2);
+    const double p00 = L->c00, p01 = L->c01, p10 = L->c10, p11 = L->c11;
+    const double a00 = h00 * p00 + h01 * p10, a01 = h00 * p01 + h01 * p11;
+    const double a10 = h10 * p00 + h11 * p10, a11 = h10 * p01 + h11 * p11;
+    const double s00 = (a00 * h00 + a01 * h01) + r00;
+    const double s01 = (a00 * h10 + a01 * h11) + 0.0;
+    const double s10 = (a10 * h00 + a11 * h01) + 0.0;
+    const double s11 = (a10 * h10 + a11 * h11) + r11;
+    const double det = s00 * s11 - s10 * s01;
+    if (det == 0.0) return 0;
+    const pfc_rcp_t rdet = pfc_rcp_make(det);
+    const double i00 = pfc_div_by(s11, rdet), i01 = pfc_div_by(-s01, rdet), i10 = pfc_div_by(-s10, rdet), i11 = pfc_div_by(s00, rdet);
+    const double t0 = y0 * i00 + y1 * i10, t1 = y0 * i01 + y1 * i11;
+    *d2out = t0 * y0 + t1 * y1;
+    return 1;
+}
+
 #endif

@@ -160,6 +160,18 @@ int  pfgpu_fs_last_gate(pfgpu_fs*, int* did_resample);     /* whether the last s
  * factor 1e-10 when det S <= 0).  A step without observations is the motion model with two draws (:347-356).  May be changed
  * between steps; every rank of a sharded engine must make the same call. */
 int  pfgpu_fs_set_variant(pfgpu_fs*, int variant);
+/* FastSLAM 2.0 with UNKNOWN data association (not in the reference's fastslam2; its rule is ekf_slam.rs:284-308's, applied per
+ * particle; DESIGN §3.5).  z2 = k (d, angle) pairs without landmark ids, k unbounded.  Per particle: the landmark of z2[0] for the
+ * proposal is the association at the noise-free motion prediction; then, observation by observation at the sampled pose against
+ * the map as the earlier observations left it, A = the initialised slot (cov00 < 100) with the smallest squared Mahalanobis
+ * distance y^T S^-1 y (first minimum in slot order; det S == 0 skips the slot), accepted when below gate_d2 (16 = ekf_slam.rs:19's
+ * M_DIST_TH^2).  Matched: update_landmark_and_weight on it; otherwise a birth in the lowest empty slot (!(cov00 < 100)); no
+ * empty slot: the observation is dropped.  Normalise, gate and resample as pfgpu_fs_step.  k = 0 is pfgpu_fs_step with k = 0.
+ * Variant 1: PFGPU_ERR_UNSUPPORTED.  Non-finite u / z2, or gate_d2 not > 0 (+inf allowed): PFGPU_ERR_INVALID.  May be interleaved
+ * with pfgpu_fs_step; every rank of a sharded engine makes the same calls. */
+int  pfgpu_fs_step_unknown(pfgpu_fs*, const double u[2], const double* z2, size_t k, double gate_d2, int* did_resample);
+/* (matched, born, dropped) observation counts of the last pfgpu_fs_step_unknown, summed over this handle's particles; synchronises */
+int  pfgpu_fs_assoc_counts(pfgpu_fs*, uint64_t counts[3]);
 int  pfgpu_fs_count(pfgpu_fs*, size_t* n_local, size_t* n_global, size_t* n_landmarks);
 /* Estimate (not in the reference, whose callers read the best particle's map, keeping landmarks with cov00 < 100).  With W the sum
  * of the stored weights (never assumed to be 1):

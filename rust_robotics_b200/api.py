@@ -73,7 +73,7 @@ EXPORTS = [
     "pfgpu_nccl_unique_id", "pfgpu_pf_stats", "pfgpu_fs_stats", "pfgpu_pf_time_main_kernel",
     "pfgpu_fs_time_main_kernel", "pfgpu_pf_mark", "pfgpu_pf_elapsed_ms", "pfgpu_fs_mark", "pfgpu_fs_elapsed_ms",
     "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
-    "pfgpu_fs_moments", "pfgpu_fs_estimate_merge",
+    "pfgpu_fs_moments", "pfgpu_fs_estimate_merge", "pfgpu_fs_step_unknown", "pfgpu_fs_assoc_counts",
 ]
 
 
@@ -148,6 +148,8 @@ def load_library():
     L.pfgpu_fs_shard_mode.argtypes = [vp, C.POINTER(C.c_int)]
     L.pfgpu_fs_moments.argtypes = [vp, C.c_double, C.POINTER(_FsPoseMoments), c_dp]
     L.pfgpu_fs_estimate_merge.argtypes = [C.POINTER(_FsPoseMoments), C.POINTER(c_dp), C.c_int, C.c_size_t, c_dp, c_dp, c_dp, c_dp, c_dp]
+    L.pfgpu_fs_step_unknown.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.POINTER(C.c_int)]
+    L.pfgpu_fs_assoc_counts.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
     _LIB = L
@@ -593,7 +595,8 @@ class FastSlam1:
     def estimate(self, cov00_max=100.0, landmarks=True):
         """Weighted posterior estimate (DESIGN §3.4): FsEstimate(pose (3,), pose_cov (3, 3), mass (m,), mean (m, 2), cov (m, 2, 2));
         the landmark fields are None with landmarks=False.  Only landmark copies with cov00 < cov00_max count (the examples'
-        filter; inf takes every copy).  Synchronises."""
+        filter; inf takes every copy).  After fastslam2_update_unknown steps slot l is not the same landmark in every particle, so
+        the landmark fields mix landmarks: read the best particle's map (get_best_particle + particle_landmarks).  Synchronises."""
         return self.merge_moments([self.moments(cov00_max, landmarks)])
 
     @staticmethod
@@ -627,3 +630,32 @@ class FastSlam2(FastSlam1):
 
     def fastslam2_update(self, u, z, **kw):
         return self.fastslam_update(u, z, **kw)
+
+    # -- unknown data association (not in fs2.rs; the rule of ekf_slam.rs:284-308 per particle, DESIGN §3.5) --
+    def fastslam2_update_unknown(self, u, z, gate_d2=16.0, want_flag=True):
+        """One step from observations WITHOUT landmark ids: z = k (d, angle) pairs.  Every particle associates each observation with
+        the landmark of its own map at the smallest Mahalanobis distance below gate_d2, or adds a landmark in its lowest empty slot
+        (an observation is dropped when the map is full).  Returns whether the step resampled (None when want_flag is False: no
+        host sync).  Slot l is then NOT the same landmark in every particle: read a map from one particle (get_best_particle and
+        particle_landmarks), not from estimate()."""
+        uu = _f64(u)
+        zz = _f64(z).reshape(-1, 2) if len(z) else np.zeros((0, 2))
+        did = C.c_int()
+        _check(self.L, self.L.pfgpu_fs_step_unknown(self.h, _dp(uu), _dp(zz) if zz.size else None, zz.shape[0], float(gate_d2),
+                                                    C.byref(did) if want_flag else None))
+        return bool(did.value) if want_flag else None
+
+    @staticmethod
+    def step_all_unknown(ranks, u, z, gate_d2=16.0):
+        """one fastslam2_update_unknown on every in-process rank (create_sharded_local): enqueue everywhere, then synchronise"""
+        for g in ranks:
+            g.fastslam2_update_unknown(u, z, gate_d2, want_flag=False)
+        for g in ranks:
+            g.sync()
+        return ranks[0].did_resample()
+
+    def assoc_counts(self):
+        """(matched, born, dropped) observations of the last unknown-association step over this handle's particles (synchronises)"""
+        c = (C.c_uint64 * 3)()
+        _check(self.L, self.L.pfgpu_fs_assoc_counts(self.h, c))
+        return tuple(int(v) for v in c)

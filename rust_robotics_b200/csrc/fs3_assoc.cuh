@@ -1,0 +1,157 @@
+// fs3_assoc.cuh — FastSLAM 2.0 step with UNKNOWN data association (DESIGN §3.5): observations arrive as (d, angle) pairs and
+// every particle decides against its own map which landmark each one came from (the rule of search_correspond_landmark_id,
+// ekf_slam.rs:284-308, per particle: fs_assoc_d2 of include/fs2_math.h).  One launch, fs3_assoc_kernel, replaces
+// fs2_propose_kernel and the EKF launch(es) of a known-id step; fs3_assoc_mark_kernel then settles the lazy-clone bookkeeping
+// and the unchanged post kernel (fs3.cuh) runs with no observation list of its own.
+//
+// Lazy clone.  The per-landmark generations of fs3.cuh assume that every particle updates the same landmarks in a step; here
+// they do not.  So the kernel's first scan (the proposal's, which visits every slot anyway) MATERIALISES every landmark that is
+// read through an ancestry row: slot i's copy, read through the row (maybe on a peer), is stored to column i of the OTHER buffer,
+// and fs3_assoc_mark_kernel makes every such landmark "identity" in that buffer afterwards.  From then on the kernel reads and
+// updates column i of the landmark's target buffer in place.  That is safe because rows only ever reference the buffer lmst
+// names: for a landmark read through a row, peers read buffer `buf` while everybody writes buffer `buf ^ 1`; an identity landmark
+// has no row, so nobody but slot i reads its column i.  (lmst is identical on every rank: every rank runs the same steps.)
+#pragma once
+#include "fs3.cuh"
+
+#define FS3_ASSOC_NT 128          // threads per CTA: two 64-particle groups (the partial sums of wraw_all)
+
+// out-of-line pieces with their own copies (a routine shared with the existing kernels would be register-allocated for all callers)
+__device__ __noinline__ int fs3a_d2(const FsLm* L, double px, double py, double pyaw, double z0, double z1, double r00, double r11, double* q) {
+    return fs_assoc_d2(L, px, py, pyaw, z0, z1, r00, r11, q);
+}
+__device__ __noinline__ double fs3a_update(FsLm* L, double px, double py, double pyaw, double z0, double z1, double r00, double r11) {
+    int wrote;
+    return fs_update_landmark_v(L, px, py, pyaw, z0, z1, r00, r11, &wrote, 2);    // update_landmark_and_weight fs2.rs:242-280
+}
+__device__ __noinline__ void fs3a_propose(double* x, double* y, double* a, const FsLm* L, double u0, double u1, double dt, double z0, double z1,
+                                          double r00, double r11, double n0, double n1, double n2) {
+    const double mc[9] = { 0.1, 0.0, 0.0, 0.0, 0.1, 0.0, 0.0, 0.0, 0.01 };           // MOTION_COV fs2.rs:31
+    fs2_propose_pose(x, y, a, L, u0, u1, dt, z0, z1, r00, r11, mc, n0, n1, n2);
+}
+__device__ __forceinline__ FsLm fs3a_load(const double* p, size_t ld) {
+    FsLm L;
+    L.x = p[0]; L.y = p[ld]; L.c00 = p[2 * ld]; L.c01 = p[3 * ld]; L.c10 = p[4 * ld]; L.c11 = p[5 * ld];
+    return L;
+}
+__device__ __forceinline__ void fs3a_store(double* p, size_t ld, const FsLm& L) {
+    p[0] = L.x; p[ld] = L.y; p[2 * ld] = L.c00; p[3 * ld] = L.c01; p[4 * ld] = L.c10; p[5 * ld] = L.c11;
+}
+// buffer that holds slot i's copy of a landmark in state s once this step's first scan has run
+__device__ __forceinline__ int fs3a_tbuf(int s) { return (s & 1) ^ ((s >> 1) ? 1 : 0); }
+
+// A(pose, z) over slot i's map (every landmark materialised): the matching slot or -1, and the lowest empty slot or -1
+__device__ __forceinline__ void fs3a_scan(const Fs3Dev& d, unsigned i, double px, double py, double pyaw, double z0, double z1, double r00,
+                                          double r11, double gate_d2, int* match, int* empty) {
+    const size_t ld = d.ld;
+    double best = 1.7976931348623157e308;                              // f64::MAX: strict `<`, the first minimum wins
+    int bl = -1, e = -1;
+#pragma unroll 1
+    for (unsigned l = 0; l < d.m; ++l) {
+        const double* p = d.lm[fs3a_tbuf(d.lmst[l])] + (size_t)l * 6 * ld + i;
+        const double c00 = p[2 * ld];
+        if (!(c00 < 100.0)) { if (e < 0) e = (int)l; continue; }       // is_initialized fs2.rs:49-51
+        FsLm L = fs3a_load(p, ld);
+        double q;
+        if (fs3a_d2(&L, px, py, pyaw, z0, z1, r00, r11, &q) && q < best) { best = q; bl = (int)l; }
+    }
+    *match = bl >= 0 && best < gate_d2 ? bl : -1;
+    *empty = e;
+}
+
+// One thread per local slot, a warp on 32 consecutive slots: every field read of landmark l is one coalesced 256-byte segment of
+// the field-major map.  z2 = k (d, angle) pairs in device memory.  counts[0..2] += (matched, born, dropped) of this launch.
+// Writes this step's unnormalised weights and 64-particle partial sums into every rank's wraw_all / part_all (the EKF epilogue's
+// duty); the post kernel signals "arrived" and waits for the peers as after an EKF launch.
+__global__ void __launch_bounds__(FS3_ASSOC_NT)
+fs3_assoc_kernel(const __grid_constant__ Fs3Dev d, const double* __restrict__ z2, int k, double gate_d2, double u0, double u1, double dt,
+                 double r00, double r11, uint64_t seed, uint32_t call, unsigned step, unsigned long long* counts) {
+    pf_grid_dep_sync();
+    __shared__ double s_part[FS3_ASSOC_NT / 32];
+    if (d.G > 1 && d.wait_inline) {             // peers' rows / poses / maps are stable once their previous post kernel is over
+        if (threadIdx.x == 0) fs3_wait_peers(d, 1, step);
+        __syncthreads();
+    }
+    const Fs3State* st = d.st;
+    const int cur = st->cur, rcur = st->rcur, par = (int)(step & 1u);
+    const size_t ld = d.ld;
+    const unsigned i = blockIdx.x * FS3_ASSOC_NT + threadIdx.x;
+    double w = 0.0;
+    unsigned cm = 0, cb = 0, cd = 0;
+    if (i < d.n) {
+        double x = d.px[cur][i], y = d.py[cur][i], a = d.pyaw[cur][i];
+        w = d.w[i];                                                    // Particle::weight
+        double n0, n1, n2, unused;
+        if (st->noise_call == call + 1u) { n0 = d.nz[0][i]; n1 = d.nz[1][i]; }      // drawn by the previous post kernel's idle warps
+        else pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_PREDICT, call, (uint64_t)d.off + i), &n0, &n1);
+        pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS2_POSE3, call, (uint64_t)d.off + i), &n2, &unused);
+        // ---- proposal scan at the noise-free prediction x_pred (compute_proposal fs2.rs:183), materialising every landmark read
+        //      through a row into column i of the other buffer ----
+        const double z0 = z2[0], z1 = z2[1];
+        double sn, cs;
+        pfc_sincos(a, &sn, &cs);
+        const double xp0 = x + u0 * dt * cs, xp1 = y + u0 * dt * sn, xp2 = fs_normalize_angle(a + u1 * dt);
+        double best = 1.7976931348623157e308;
+        int bl = -1;
+#pragma unroll 1
+        for (unsigned l = 0; l < d.m; ++l) {
+            const int s = d.lmst[l], buf = s & 1;
+            const size_t lbase = (size_t)l * 6 * ld;
+            FsLm L;
+            if (s >> 1) {
+                const unsigned ref = d.rows[rcur][(size_t)((s >> 1) - 1) * ld + i];
+                const double* base = d.G > 1 ? reinterpret_cast<const double*>(d.peer[ref >> 28] + d.o_lm[buf]) : d.lm[buf];
+                L = fs3a_load(base + lbase + (ref & 0x0FFFFFFFu), ld);
+                fs3a_store(d.lm[buf ^ 1] + lbase + i, ld, L);
+            } else L = fs3a_load(d.lm[buf] + lbase + i, ld);
+            double q;
+            if (L.c00 < 100.0 && fs3a_d2(&L, xp0, xp1, xp2, z0, z1, r00, r11, &q) && q < best) { best = q; bl = (int)l; }
+        }
+        FsLm P = { 0.0, 0.0, 1000.0, 0.0, 0.0, 1000.0 };               // no match: compute_proposal's uninitialised branch (fs2.rs:188-191)
+        if (bl >= 0 && best < gate_d2) P = fs3a_load(d.lm[fs3a_tbuf(d.lmst[bl])] + (size_t)bl * 6 * ld + i, ld);
+        fs3a_propose(&x, &y, &a, &P, u0, u1, dt, z0, z1, r00, r11, n0, n1, n2);
+        // ---- the observations in order: scan at the sampled pose, then update the match, or a birth, or drop ----
+#pragma unroll 1
+        for (int j = 0; j < k; ++j) {
+            const double zj0 = z2[2 * j], zj1 = z2[2 * j + 1];
+            int l, e;
+            fs3a_scan(d, i, x, y, a, zj0, zj1, r00, r11, gate_d2, &l, &e);
+            if (l >= 0) cm++;
+            else if (e >= 0) { l = e; cb++; }
+            else { cd++; continue; }                                   // the map is full: the observation is dropped
+            double* p = d.lm[fs3a_tbuf(d.lmst[l])] + (size_t)l * 6 * ld + i;
+            FsLm L = fs3a_load(p, ld);
+            w = w * fs3a_update(&L, x, y, a, zj0, zj1, r00, r11);
+            fs3a_store(p, ld, L);
+        }
+        d.px[cur][i] = x; d.py[cur][i] = y; d.pyaw[cur][i] = a;
+    }
+    // ---- weights and 64-particle partials to every rank; the counters ----
+    const unsigned lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    const double ws = warp_sum(w);                                     // honest (tree-order) sum: steers x3_classify only
+    if (lane == 0) s_part[wid] = ws;
+    const unsigned long long c3[3] = { __reduce_add_sync(0xffffffffu, cm), __reduce_add_sync(0xffffffffu, cb), __reduce_add_sync(0xffffffffu, cd) };
+    if (lane < 3 && c3[lane]) atomicAdd(counts + lane, c3[lane]);
+    __syncthreads();
+#pragma unroll 1
+    for (int gg = 0; gg < d.G; ++gg) {
+        double* wr = (d.G > 1 ? reinterpret_cast<double*>(d.peer[gg] + d.o_wraw[par]) : d.wraw[par]) + d.off;
+        if (i < d.n) wr[i] = w;
+        const unsigned ge = blockIdx.x * (FS3_ASSOC_NT / 64) + threadIdx.x;
+        if (threadIdx.x < FS3_ASSOC_NT / 64 && ge < d.npart) {
+            double* pp = d.G > 1 ? reinterpret_cast<double*>(d.peer[gg] + d.o_part[par]) : d.part[par];
+            pp[(size_t)d.rank * d.npart + ge] = s_part[2 * threadIdx.x] + s_part[2 * threadIdx.x + 1];
+        }
+    }
+}
+
+// After fs3_assoc_kernel: every landmark it materialised is identity in its target buffer; the launch's counters move to
+// counts[3..5] (what pfgpu_fs_assoc_counts reports) and counts[0..2] are cleared for the next step.
+__global__ void fs3_assoc_mark_kernel(const __grid_constant__ Fs3Dev d, unsigned long long* counts) {
+    pf_grid_dep_sync();
+    for (unsigned l = blockIdx.x * blockDim.x + threadIdx.x; l < d.m; l += gridDim.x * blockDim.x) {
+        const int s = d.lmst[l];
+        if (s >> 1) d.lmst[l] = fs3a_tbuf(s);
+    }
+    if (blockIdx.x == 0 && threadIdx.x < 3) { counts[3 + threadIdx.x] = counts[threadIdx.x]; counts[threadIdx.x] = 0ull; }
+}

@@ -3,6 +3,7 @@
 #pragma once
 #include "fs3.cuh"
 #include "fs3_est.cuh"
+#include "fs3_assoc.cuh"
 
 struct pfgpu_fs {
     Ctx ctx;
@@ -29,6 +30,8 @@ struct pfgpu_fs {
     bool post_global = false;         // the post kernel keeps its weight tiles in global memory (fs3_post_kernel<512, true>) ...
     double* vtile = nullptr;          // ... here: [post_tiles][post_K][512]
     char* est = nullptr; size_t est_bytes = 0;   // pfgpu_fs_moments scratch, allocated by the first call (fs3_est.cuh)
+    double* zbuf = nullptr; size_t zcap = 0;     // pfgpu_fs_step_unknown: the (d, angle) list of the step (grows, never shrinks)
+    unsigned long long* acnt = nullptr;         // [6] association counters: this launch's, then the last unknown step's (fs3_assoc.cuh)
 };
 
 extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.rs:13-23
@@ -260,6 +263,7 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(d.bar); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
     cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage); cudaFree(h->est);
+    cudaFree(h->zbuf); cudaFree(h->acnt);
     if (h->h_rec) cudaFreeHost(h->h_rec);
     if (h->comm) ncclCommDestroy(h->comm);
     marks_free(h->marks);
@@ -381,6 +385,19 @@ static int fs3_launch_ekf(pfgpu_fs* h, const Fs3ObsParam& po, const double u[2],
     return 0;
 }
 
+// normalise, N_eff gate and (when it opens) the whole resample of step h->n_step: one launch.  po / k_last: the last EKF launch's
+// observations, whose lazy-clone bookkeeping the post kernel applies (k_last = 0: none)
+static int fs3_launch_post(pfgpu_fs* h, const Fs3ObsParam& po, int k_last, bool host_waits) {
+    const Fs3Dev& d = h->d;
+    if (h->post_global)
+        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, true>), h->post_tiles, 512, 0, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    else if (h->post_nt == 512)
+        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, false>), h->post_tiles, 512, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    else
+        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<256, false>), h->post_tiles, 256, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    return 0;
+}
+
 extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs* z, size_t k, int* did) {
     if (!h || !u || (k && !z)) return PFGPU_ERR_INVALID;
     if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
@@ -436,12 +453,8 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
         PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
     }
     // normalise, N_eff gate and (when it opens) the whole resample: one launch
-    if (h->post_global)
-        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, true>), h->post_tiles, 512, 0, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
-    else if (h->post_nt == 512)
-        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, false>), h->post_tiles, 512, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
-    else
-        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<256, false>), h->post_tiles, 256, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    int rc = fs3_launch_post(h, po, k_last, host_waits);
+    if (rc) return rc;
     h->n_step++;
     h->steps++;
     if (did) {     // the gate lives on the device; only a caller who asks pays a sync
@@ -450,6 +463,69 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
         return fs_check_err(h);
     }
     return 0;
+}
+// FastSLAM 2.0 with unknown data association (DESIGN §3.5): fs3_assoc_kernel, the lazy-clone bookkeeping, then the post kernel
+extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const double* z2, size_t k, double gate_d2, int* did) {
+    if (!h || !u || (k && !z2)) return PFGPU_ERR_INVALID;
+    if (h->variant != 2) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "unknown data association needs FastSLAM 2.0 (pfgpu_fs_set_variant(h, 2)): FastSLAM 1.0 "
+                 "never initialises a fresh landmark's covariance, so a landmark it adds could never be matched");
+        return PFGPU_ERR_UNSUPPORTED;
+    }
+    if (!finite_d(u[0]) || !finite_d(u[1]) || !(gate_d2 > 0.0)) return PFGPU_ERR_INVALID;      // gate_d2 = +inf is allowed
+    for (size_t j = 0; j < 2 * k; ++j) if (!finite_d(z2[j])) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    Fs3Dev& d = h->d;
+    if (!h->acnt) {
+        PF_CUDA(cudaMalloc(&h->acnt, 6 * sizeof(unsigned long long)));
+        PF_CUDA(cudaMemsetAsync(h->acnt, 0, 6 * sizeof(unsigned long long), h->ctx.stream));
+    }
+    if (k == 0) {           // no observation: the known-id step with k = 0, bit for bit; nothing was associated
+        PF_CUDA(cudaMemsetAsync(h->acnt + 3, 0, 3 * sizeof(unsigned long long), h->ctx.stream));
+        return pfgpu_fs_step(h, u, nullptr, 0, did);
+    }
+    if (2 * k > h->zcap) {  // (the previous step may still read the old list: wait for it before the buffer goes)
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+        cudaFree(h->zbuf); h->zbuf = nullptr; h->zcap = 0;
+        const size_t cap = std::max<size_t>(64, 4 * k);
+        PF_CUDA(cudaMalloc(&h->zbuf, cap * sizeof(double)));
+        h->zcap = cap;
+    }
+    // stream-ordered behind every kernel of the previous step, so a list is never overwritten while a step reads it
+    PF_CUDA(cudaMemcpyAsync(h->zbuf, z2, 2 * k * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+    const bool host_waits = d.G > 1 && !d.wait_inline;
+    if (host_waits) PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 1, (unsigned)h->n_step);            // peers' previous post kernels are over
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
+    PF_LAUNCH(h->ctx, fs3_assoc_kernel, cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d, (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1],
+              h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step, h->acnt);
+    if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
+    PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_assoc_mark_kernel, std::max(1u, std::min(cdiv_u(d.m, 256), 64u)), 256, 0, d, h->acnt);
+    if (host_waits) {
+        PF_LAUNCH(h->ctx, fs3_signal_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
+        PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
+    }
+    Fs3ObsParam po;
+    memset(&po, 0, sizeof(po));
+    int rc = fs3_launch_post(h, po, 0, host_waits);
+    if (rc) return rc;
+    h->n_step++;
+    h->steps++;
+    if (did) {
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+        *did = h->h_rec->gate;
+        return fs_check_err(h);
+    }
+    return 0;
+}
+extern "C" int pfgpu_fs_assoc_counts(pfgpu_fs* h, uint64_t counts[3]) {
+    if (!h || !counts) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    unsigned long long c[3] = { 0ull, 0ull, 0ull };
+    if (h->acnt) PF_CUDA(cudaMemcpy(c, h->acnt + 3, sizeof(c), cudaMemcpyDeviceToHost));
+    for (int j = 0; j < 3; ++j) counts[j] = (uint64_t)c[j];
+    return fs_check_err(h);
 }
 extern "C" int pfgpu_fs_set_variant(pfgpu_fs* h, int variant) {
     if (!h || (variant != 1 && variant != 2)) return PFGPU_ERR_INVALID;

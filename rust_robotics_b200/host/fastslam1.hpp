@@ -4,6 +4,7 @@
 #pragma once
 #include <array>
 #include <tuple>
+#include <utility>
 #include <vector>
 #include "pfgpu.h"
 #include "particle_filter.hpp"
@@ -77,6 +78,8 @@ public:
     size_t len() const { return n_; }
     // 1 = fastslam1::fastslam_update, 2 = fastslam2::fastslam2_update (crates/rust_robotics_slam/src/fastslam2.rs:376-383)
     void set_variant(int variant) { check(pfgpu_fs_set_variant(h_, variant), "set_variant"); }
+protected:
+    pfgpu_fs* handle() const { return h_; }
 };
 
 // the reference's free-function names
@@ -92,7 +95,24 @@ using fastslam1::Landmark; using fastslam1::Particle; using fastslam1::Observati
 struct FastSlam : fastslam1::FastSlam {
     FastSlam(size_t n_particles, size_t n_landmarks, uint64_t seed = 42, int device = 0, const pfgpu_fs_config* cfg = nullptr)
         : fastslam1::FastSlam(n_particles, n_landmarks, seed, device, cfg) { set_variant(2); }
+    // observations WITHOUT landmark ids, (distance, angle): every particle associates them with its own map (pfgpu_fs_step_unknown)
+    bool update_unknown(const std::array<double, 2>& u, const std::vector<std::pair<double, double>>& z, double gate_d2 = 16.0) {
+        std::vector<double> z2(2 * z.size());
+        for (size_t i = 0; i < z.size(); ++i) { z2[2 * i] = z[i].first; z2[2 * i + 1] = z[i].second; }
+        int did = 0;
+        check(pfgpu_fs_step_unknown(handle(), u.data(), z2.data(), z.size(), gate_d2, &did), "fastslam2_update_unknown");
+        return did != 0;
+    }
+    // (matched, born, dropped) observations of the last update_unknown over all particles
+    std::array<uint64_t, 3> assoc_counts() const {
+        std::array<uint64_t, 3> c{};
+        check(pfgpu_fs_assoc_counts(handle(), c.data()), "assoc_counts");
+        return c;
+    }
 };
 inline bool fastslam2_update(FastSlam& particles, const std::array<double, 2>& u, const std::vector<Observation>& z) { return particles.step(u, z); }
+inline bool fastslam2_update_unknown(FastSlam& particles, const std::array<double, 2>& u, const std::vector<std::pair<double, double>>& z) {
+    return particles.update_unknown(u, z);
+}
 }  // namespace fastslam2
 }  // namespace rust_robotics_b200

@@ -84,6 +84,9 @@ extern "C" {
                                      out: *mut pfgpu_fs_obs, k: *mut usize) -> c_int;
     pub fn pfgpu_fs_last_gate(h: *mut pfgpu_fs, did_resample: *mut c_int) -> c_int;
     pub fn pfgpu_fs_set_variant(h: *mut pfgpu_fs, variant: c_int) -> c_int;
+    // FastSLAM 2.0 with unknown data association (no reference counterpart in fastslam2; ekf_slam.rs:284-308's rule per particle)
+    pub fn pfgpu_fs_step_unknown(h: *mut pfgpu_fs, u: *const f64, z2: *const f64, k: usize, gate_d2: f64, did_resample: *mut c_int) -> c_int;
+    pub fn pfgpu_fs_assoc_counts(h: *mut pfgpu_fs, counts: *mut u64) -> c_int;
     pub fn pfgpu_fs_last_neff(h: *mut pfgpu_fs, neff: *mut f64) -> c_int;
     pub fn pfgpu_fs_particle_landmarks(h: *mut pfgpu_fs, index_local: usize, lm6: *mut f64) -> c_int;
     pub fn pfgpu_fs_count(h: *mut pfgpu_fs, n_local: *mut usize, n_global: *mut usize, n_landmarks: *mut usize) -> c_int;

@@ -18,3 +18,20 @@ pub fn create_particles(n_particles: usize, n_landmarks: usize) -> FastSlam {
 pub fn fastslam2_update(particles: &mut FastSlam, u: Vector2<f64>, z: &[(f64, f64, usize)]) {
     crate::fastslam1::fastslam_update(particles, u, z)      // the handle carries the variant
 }
+/// FastSLAM 2.0 with UNKNOWN data association (not in fs2.rs): `z` holds (distance, angle) pairs without landmark ids, and every
+/// particle associates each one with the landmark of its own map at the smallest Mahalanobis distance below the gate
+/// M_DIST_TH^2 = 16 of ekf_slam.rs:19, or adds it in its lowest empty slot (DESIGN §3.5).  Slot l is then not the same landmark
+/// in every particle: read a map from one particle (`get_best_particle`).
+pub fn fastslam2_update_unknown(particles: &mut FastSlam, u: Vector2<f64>, z: &[(f64, f64)]) {
+    let uu = [u[0], u[1]];
+    let z2: Vec<f64> = z.iter().flat_map(|&(d, a)| [d, a]).collect();
+    let rc = unsafe { sys::pfgpu_fs_step_unknown(particles.raw(), uu.as_ptr(), z2.as_ptr(), z.len(), 16.0, std::ptr::null_mut()) };
+    assert_eq!(rc, 0, "pfgpu_fs_step_unknown failed");
+}
+/// (matched, born, dropped) observations of the last `fastslam2_update_unknown`, summed over the particles
+pub fn assoc_counts(particles: &FastSlam) -> [u64; 3] {
+    let mut c = [0u64; 3];
+    let rc = unsafe { sys::pfgpu_fs_assoc_counts(particles.raw(), c.as_mut_ptr()) };
+    assert_eq!(rc, 0, "pfgpu_fs_assoc_counts failed");
+    c
+}
