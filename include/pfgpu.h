@@ -196,6 +196,32 @@ int  pfgpu_fs_moments(pfgpu_fs*, double cov00_max, pfgpu_fs_pose_moments* pose, 
  * are invalid. */
 int  pfgpu_fs_estimate_merge(const pfgpu_fs_pose_moments* pose, const pfgpu_fs_lm_moments* const* lm, int world, size_t n_landmarks,
                              double pose_mean3[3], double pose_cov9_colmajor[9], double* lm_mass, double* lm_mean2, double* lm_cov4);
+/* Path history (not in the reference, whose particles keep no past poses; DESIGN §3.6).  A FastSLAM particle is a path hypothesis;
+ * the engine can keep the last `capacity` steps of every particle's path on the device:
+ *   window   entry s is written after step s (s counts every pfgpu_fs_step / pfgpu_fs_step_unknown since create, k = 0 included).
+ *            It holds, per slot i, the pose (x, y, yaw) after the step (after the resample's clone) and a parent a_s(i): the global
+ *            ancestor of slot i when step s resampled, i itself otherwise.  Enabling writes a root entry (the current poses, every
+ *            parent the slot itself) at the current step count; so do pfgpu_fs_upload and pfgpu_fs_seed_map while history is enabled,
+ *            which restart the window.  A full ring drops its oldest entry; the oldest entry held is always a root.
+ *   path     of global slot g: slot_S = g at the newest entry S, slot_{s-1} = a_s(slot_s); pose_s[slot_s] at every entry.  Equal to
+ *            the list of past poses each particle would carry if it were cloned with the particle at every resample.
+ *   moments  genealogy smoother: at every entry s, pfgpu_fs_moments' definition (DESIGN §3.4) over the lineage poses of the current
+ *            particles with their CURRENT weights, about the centre c_s = the step-s pose on the lineage of global slot n - 1.
+ *            Sharded: each rank returns its own particles' moments; merge entry by entry with pfgpu_fs_estimate_merge (lm = NULL).
+ * pfgpu_fs_history_enable: capacity entries (capacity * ld * 28 bytes per rank, ld = local particles rounded up to 64); 0
+ *   disables and frees.  Re-enabling starts a new window.  Collective on a sharded engine, with the same capacity on every rank.  A
+ *   ring that does not fit in device memory: PFGPU_ERR_CUDA, and history stays as it was.  While enabled every step adds one
+ *   kernel launch and no host synchronisation.
+ * pfgpu_fs_history_window: the steps of the oldest and the newest entry held.
+ * pfgpu_fs_path: the newest min(max_steps, window length) entries of slot index_global's path, oldest first: step numbers, slot ids
+ *   and poses (pose3: 3 per entry); *n = entries written.  step / slot / pose3 are nullable, each holds max_steps entries.
+ * pfgpu_fs_path_moments: the same entries' moments, oldest first, into out (max_steps entries).
+ * Both queries synchronise and are valid where pfgpu_fs_download is (on a sharded engine no rank may step until every rank's call
+ * has returned).  History disabled, an index out of range or max_steps == 0: PFGPU_ERR_INVALID. */
+int  pfgpu_fs_history_enable(pfgpu_fs*, size_t capacity);
+int  pfgpu_fs_history_window(pfgpu_fs*, uint64_t* first_step, uint64_t* last_step);
+int  pfgpu_fs_path(pfgpu_fs*, size_t index_global, size_t max_steps, uint64_t* step, uint32_t* slot, double* pose3, size_t* n);
+int  pfgpu_fs_path_moments(pfgpu_fs*, size_t max_steps, uint64_t* step, pfgpu_fs_pose_moments* out, size_t* n);
 int  pfgpu_fs_sync(pfgpu_fs*);
 
 /* ============================================ plumbing ============================================== */

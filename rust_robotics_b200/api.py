@@ -59,6 +59,10 @@ class _FsPoseMoments(C.Structure):
 # FastSlam1.estimate(): pose (3,) mean of (x, y, yaw), pose_cov (3, 3); per landmark (None when not asked for) mass (m,),
 # mean (m, 2), cov (m, 2, 2)
 FsEstimate = collections.namedtuple("FsEstimate", ["pose", "pose_cov", "mass", "mean", "cov"])
+# FastSlam1.path(): steps (L,) u64, slots (L,) u32 (global slot at each step), poses (L, 3); oldest first
+FsPath = collections.namedtuple("FsPath", ["steps", "slots", "poses"])
+# FastSlam1.path_estimate(): steps (L,), pose (L, 3) weighted mean of the lineage poses, pose_cov (L, 3, 3); oldest first
+FsPathEstimate = collections.namedtuple("FsPathEstimate", ["steps", "pose", "pose_cov"])
 
 
 EXPORTS = [
@@ -74,6 +78,7 @@ EXPORTS = [
     "pfgpu_fs_time_main_kernel", "pfgpu_pf_mark", "pfgpu_pf_elapsed_ms", "pfgpu_fs_mark", "pfgpu_fs_elapsed_ms",
     "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
     "pfgpu_fs_moments", "pfgpu_fs_estimate_merge", "pfgpu_fs_step_unknown", "pfgpu_fs_assoc_counts",
+    "pfgpu_fs_history_enable", "pfgpu_fs_history_window", "pfgpu_fs_path", "pfgpu_fs_path_moments",
 ]
 
 
@@ -150,6 +155,10 @@ def load_library():
     L.pfgpu_fs_estimate_merge.argtypes = [C.POINTER(_FsPoseMoments), C.POINTER(c_dp), C.c_int, C.c_size_t, c_dp, c_dp, c_dp, c_dp, c_dp]
     L.pfgpu_fs_step_unknown.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.POINTER(C.c_int)]
     L.pfgpu_fs_assoc_counts.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.pfgpu_fs_history_enable.argtypes = [vp, C.c_size_t]
+    L.pfgpu_fs_history_window.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    L.pfgpu_fs_path.argtypes = [vp, C.c_size_t, C.c_size_t, C.POINTER(C.c_uint64), c_u32p, c_dp, C.POINTER(C.c_size_t)]
+    L.pfgpu_fs_path_moments.argtypes = [vp, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(_FsPoseMoments), C.POINTER(C.c_size_t)]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
     _LIB = L
@@ -606,6 +615,72 @@ class FastSlam1:
         for g in ranks:
             g.sync()
         return FastSlam1.merge_moments([g.moments(cov00_max, landmarks) for g in ranks])
+
+    # -- path history (no reference counterpart: fs1.rs's particles keep no past poses; DESIGN §3.6) --
+    def enable_history(self, capacity):
+        """Keep the last `capacity` steps of every particle's path on the device (28 bytes per particle and step); 0 disables.
+        Starts a new window at the current poses.  On a sharded engine every rank makes the same call."""
+        _check(self.L, self.L.pfgpu_fs_history_enable(self.h, int(capacity)))
+
+    def history_window(self):
+        """(first, last): the steps of the oldest and the newest entry held"""
+        a, b = C.c_uint64(), C.c_uint64()
+        _check(self.L, self.L.pfgpu_fs_history_window(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def _max_steps(self, max_steps):
+        if max_steps is not None:
+            return int(max_steps)
+        first, last = self.history_window()
+        return last - first + 1
+
+    def path(self, index=None, max_steps=None):
+        """FsPath of global slot `index` (default: the best particle), oldest first: the poses of its lineage, which are the poses
+        that produced its map.  At most max_steps entries (default: the whole window).  Synchronises."""
+        if index is None:
+            index = self.get_best_particle()[0]
+        cap = self._max_steps(max_steps)
+        steps, slots, poses = np.empty(max(cap, 1), dtype=np.uint64), np.empty(max(cap, 1), dtype=np.uint32), np.empty((max(cap, 1), 3))
+        n = C.c_size_t()
+        _check(self.L, self.L.pfgpu_fs_path(self.h, int(index), cap, steps.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            slots.ctypes.data_as(c_u32p), _dp(poses), C.byref(n)))
+        return FsPath(steps[:n.value], slots[:n.value], poses[:n.value])
+
+    def path_moments(self, max_steps=None):
+        """pfgpu_fs_path_moments: (steps, [pose moments per step]) of the particles this handle owns, oldest first"""
+        cap = self._max_steps(max_steps)
+        steps = np.empty(max(cap, 1), dtype=np.uint64)
+        out = (_FsPoseMoments * max(cap, 1))()
+        n = C.c_size_t()
+        _check(self.L, self.L.pfgpu_fs_path_moments(self.h, cap, steps.ctypes.data_as(C.POINTER(C.c_uint64)), out, C.byref(n)))
+        return steps[:n.value], [out[j] for j in range(n.value)]
+
+    @staticmethod
+    def merge_path_moments(per_rank):
+        """[(steps, moments)] in rank order -> FsPathEstimate: every step merged with pfgpu_fs_estimate_merge (pose only)"""
+        steps = per_rank[0][0]
+        assert all(np.array_equal(s, steps) for s, _ in per_rank), "ranks hold different history windows"
+        L = load_library()
+        world = len(per_rank)
+        pose, cov = np.empty((len(steps), 3)), np.empty((len(steps), 3, 3))
+        for j in range(len(steps)):
+            poses = (_FsPoseMoments * world)(*[m[j] for _, m in per_rank])
+            mean, c9 = np.empty(3), np.empty(9)
+            _check(L, L.pfgpu_fs_estimate_merge(poses, None, world, 0, _dp(mean), _dp(c9), None, None, None))
+            pose[j], cov[j] = mean, c9.reshape(3, 3).T
+        return FsPathEstimate(steps, pose, cov)
+
+    def path_estimate(self, max_steps=None):
+        """Genealogy smoother (DESIGN §3.6): at every step of the window, the weighted mean and covariance of the current particles'
+        lineage poses under their current weights; FsPathEstimate, oldest first.  Synchronises."""
+        return self.merge_path_moments([self.path_moments(max_steps)])
+
+    @staticmethod
+    def path_estimate_all(ranks, max_steps=None):
+        """path_estimate() of an in-process sharded engine: synchronises every rank, then merges their moments step by step"""
+        for g in ranks:
+            g.sync()
+        return FastSlam1.merge_path_moments([g.path_moments(max_steps) for g in ranks])
 
     def time_main_kernel(self, on=True):
         _check(self.L, self.L.pfgpu_fs_time_main_kernel(self.h, int(on)))

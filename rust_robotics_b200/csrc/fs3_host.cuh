@@ -4,6 +4,7 @@
 #include "fs3.cuh"
 #include "fs3_est.cuh"
 #include "fs3_assoc.cuh"
+#include "fs3_hist.cuh"
 
 struct pfgpu_fs {
     Ctx ctx;
@@ -32,7 +33,13 @@ struct pfgpu_fs {
     char* est = nullptr; size_t est_bytes = 0;   // pfgpu_fs_moments scratch, allocated by the first call (fs3_est.cuh)
     double* zbuf = nullptr; size_t zcap = 0;     // pfgpu_fs_step_unknown: the (d, angle) list of the step (grows, never shrinks)
     unsigned long long* acnt = nullptr;         // [6] association counters: this launch's, then the last unknown step's (fs3_assoc.cuh)
+    pfgpu_fs* sib[FS3_MAXG] = {};               // in-process sharded engine: every rank's handle (pfgpu_fs_create_sharded_local)
+    char* hist = nullptr; size_t hist_cap = 0;  // path history ring (fs3_hist.cuh), pfgpu_fs_history_enable
+    uint64_t hist_first = 0;                    // oldest entry held (a root); the newest is `steps`
+    void* hist_peer[FS3_MAXG] = {};             // peers' rings mapped through cudaIpc (one process per GPU)
+    char* hs = nullptr; size_t hs_bytes = 0;    // path / path-moments scratch, grows on demand
 };
+static int fs_hist_record(pfgpu_fs* h, int root);
 
 extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.rs:13-23
     c->dt = 0.1; c->max_range = 20.0; c->nth = 100.0 / 1.5; c->q00 = 0.3; c->q11 = 0.0305; c->r00 = 0.5; c->r11 = 0.0305;
@@ -247,6 +254,7 @@ extern "C" int pfgpu_fs_create_sharded_local(const pfgpu_fs_config* cfg, size_t 
                 cudaGetLastError();
             }
             out[a]->d.peer[b] = out[b]->arena;
+            out[a]->sib[b] = out[b];
             if (a != b && devices[a] == devices[b]) out[a]->d.wait_inline = 0;     // ranks sharing a GPU must not hold SMs while they wait
         }
     return PFGPU_OK;
@@ -264,6 +272,8 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
     cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage); cudaFree(h->est);
     cudaFree(h->zbuf); cudaFree(h->acnt);
+    for (int g = 0; g < FS3_MAXG; ++g) if (h->hist_peer[g]) cudaIpcCloseMemHandle(h->hist_peer[g]);
+    cudaFree(h->hist); cudaFree(h->hs);
     if (h->h_rec) cudaFreeHost(h->h_rec);
     if (h->comm) ncclCommDestroy(h->comm);
     marks_free(h->marks);
@@ -315,7 +325,7 @@ extern "C" int pfgpu_fs_upload(pfgpu_fs* h, const double* pose_w, const double* 
         }
         PF_LAUNCH(h->ctx, fs3_lmst_reset_kernel, 1, 256, 0, d);
     }
-    return 0;
+    return h->hist ? fs_hist_record(h, 1) : 0;       // the uploaded state restarts the path history window
 }
 extern "C" int pfgpu_fs_download(pfgpu_fs* h, double* pose_w, double* lm, size_t n) {
     if (!h || n != h->d.n) return PFGPU_ERR_INVALID;
@@ -349,6 +359,7 @@ extern "C" int pfgpu_fs_seed_map(pfgpu_fs* h, const double pose3[3], const doubl
     PF_CUDA(cudaSetDevice(h->ctx.device));
     Fs3Dev& d = h->d;
     PF_LAUNCH(h->ctx, fs3_seed_pose_kernel, cdiv_u(d.n, 256), 256, 0, d, pose3[0], pose3[1], pose3[2]);
+    if (h->hist) { int rc = fs_hist_record(h, 1); if (rc) return rc; }      // the seeded state restarts the path history window
     if (m) {
         int rc = fs_stage(h, m * 2 * sizeof(double));
         if (rc) return rc;
@@ -457,6 +468,7 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
     if (rc) return rc;
     h->n_step++;
     h->steps++;
+    if (h->hist) { rc = fs_hist_record(h, 0); if (rc) return rc; }      // entry `steps` of the path history (one launch)
     if (did) {     // the gate lives on the device; only a caller who asks pays a sync
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
         *did = h->h_rec->gate;
@@ -511,6 +523,7 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
     if (rc) return rc;
     h->n_step++;
     h->steps++;
+    if (h->hist) { rc = fs_hist_record(h, 0); if (rc) return rc; }      // entry `steps` of the path history (one launch)
     if (did) {
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
         *did = h->h_rec->gate;
@@ -761,4 +774,186 @@ extern "C" int pfgpu_fs_estimate_merge(const pfgpu_fs_pose_moments* pose, const 
         }
     }
     return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// path history (DESIGN §3.6): pfgpu_fs_history_enable / _window, pfgpu_fs_path, pfgpu_fs_path_moments
+// ---------------------------------------------------------------------------------------------------------------------
+static_assert(sizeof(pfgpu_fs_pose_moments) == 13 * sizeof(double), "fs3_hist_merge_kernel writes 13 doubles per entry");
+
+// entry `steps` <- the live poses (root: every parent is the slot itself, and the window restarts there)
+static int fs_hist_record(pfgpu_fs* h, int root) {
+    const unsigned e = (unsigned)(h->steps % h->hist_cap);
+    PF_LAUNCH(h->ctx, fs3_hist_record_kernel, cdiv_u(h->d.n, FS3_HIST_NT), FS3_HIST_NT, 0, h->d, h->hist, (unsigned)h->hist_cap, e, root);
+    if (root) h->hist_first = h->steps;
+    else if (h->steps - h->hist_first >= h->hist_cap) h->hist_first = h->steps - h->hist_cap + 1;     // the ring is full: drop the oldest
+    return 0;
+}
+static void fs_hist_release(pfgpu_fs* h) {
+    for (int g = 0; g < FS3_MAXG; ++g) if (h->hist_peer[g]) { cudaIpcCloseMemHandle(h->hist_peer[g]); h->hist_peer[g] = nullptr; }
+    cudaFree(h->hist); h->hist = nullptr; h->hist_cap = 0; h->hist_first = 0;
+}
+// every rank's `bytes` from `mine` into all[world] over the handle's communicator (one process per GPU)
+static int fs_allgather(pfgpu_fs* h, const void* mine, size_t bytes, void* all) {
+    char* buf = nullptr;
+    PF_CUDA(cudaMalloc(&buf, (size_t)(h->world + 1) * bytes));
+    int rc = 0;
+    if (cudaMemcpy(buf + (size_t)h->world * bytes, mine, bytes, cudaMemcpyHostToDevice) != cudaSuccess) rc = PFGPU_ERR_CUDA;
+    else if (ncclAllGather(buf + (size_t)h->world * bytes, buf, bytes, ncclChar, h->comm, h->ctx.stream) != ncclSuccess) rc = PFGPU_ERR_NCCL;
+    else if (cudaStreamSynchronize(h->ctx.stream) != cudaSuccess || cudaMemcpy(all, buf, (size_t)h->world * bytes, cudaMemcpyDeviceToHost) != cudaSuccess)
+        rc = PFGPU_ERR_CUDA;
+    if (rc) { cudaGetLastError(); snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: exchanging ring handles failed"); }
+    cudaFree(buf);
+    return rc;
+}
+
+extern "C" int pfgpu_fs_history_enable(pfgpu_fs* h, size_t capacity) {
+    if (!h) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));               // nothing in flight still writes the old ring
+    if (capacity == 0) { fs_hist_release(h); return 0; }
+    const size_t per = fs3_hist_bytes(1, h->d.ld);
+    char* ring = nullptr;
+    int ok = capacity <= 0xFFFFFFFFull && capacity <= SIZE_MAX / per;
+    if (ok && cudaMalloc(&ring, capacity * per) != cudaSuccess) { ok = 0; ring = nullptr; cudaGetLastError(); }
+    void* opened[FS3_MAXG] = {};
+    if (h->comm) {          // one process per GPU: every rank maps every peer's ring once; all ranks agree on the outcome
+        struct Rec { cudaIpcMemHandle_t hd; uint64_t cap; int ok, pad; } mine, all[FS3_MAXG];
+        memset(&mine, 0, sizeof(mine));
+        if (ok && cudaIpcGetMemHandle(&mine.hd, ring) != cudaSuccess) { ok = 0; cudaGetLastError(); }
+        mine.cap = capacity; mine.ok = ok;
+        int rc = fs_allgather(h, &mine, sizeof(mine), all);
+        if (rc) { cudaFree(ring); return rc; }
+        bool same = true;
+        for (int g = 0; g < h->world; ++g) { ok = ok && all[g].ok; same = same && all[g].cap == capacity; }
+        if (!ok || !same) {
+            cudaFree(ring);
+            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), !ok ? "path history: a ring of %zu entries does not fit on every rank"
+                                                            : "path history: every rank must enable the same capacity (%zu here)", capacity);
+            return !ok ? PFGPU_ERR_CUDA : PFGPU_ERR_INVALID;
+        }
+        int mapped = 1, maps[FS3_MAXG];
+        for (int g = 0; g < h->world; ++g)
+            if (g != h->rank && cudaIpcOpenMemHandle(&opened[g], all[g].hd, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
+                mapped = 0; opened[g] = nullptr; cudaGetLastError();
+            }
+        rc = fs_allgather(h, &mapped, sizeof(int), maps);
+        for (int g = 0; g < h->world && !rc; ++g) mapped = mapped && maps[g];
+        if (rc || !mapped) {
+            for (int g = 0; g < FS3_MAXG; ++g) if (opened[g]) cudaIpcCloseMemHandle(opened[g]);
+            cudaFree(ring);
+            if (!rc) snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: mapping a peer's ring failed");
+            return rc ? rc : PFGPU_ERR_UNSUPPORTED;
+        }
+    } else if (!ok) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: a ring of %zu entries x %u slots does not fit in device memory", capacity, h->d.ld);
+        return PFGPU_ERR_CUDA;
+    }
+    fs_hist_release(h);
+    h->hist = ring; h->hist_cap = capacity;
+    memcpy(h->hist_peer, opened, sizeof(opened));
+    int rc = fs_hist_record(h, 1);
+    if (rc) return rc;
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_fs_history_window(pfgpu_fs* h, uint64_t* first_step, uint64_t* last_step) {
+    if (!h || !h->hist) return PFGPU_ERR_INVALID;
+    if (first_step) *first_step = h->hist_first;
+    if (last_step) *last_step = h->steps;
+    return 0;
+}
+
+static int fs_hist_scratch(pfgpu_fs* h, size_t bytes) {
+    if (bytes <= h->hs_bytes) return 0;
+    if (h->hs) { cudaFree(h->hs); h->hs = nullptr; h->hs_bytes = 0; }
+    PF_CUDA(cudaMalloc(&h->hs, bytes));
+    h->hs_bytes = bytes;
+    return 0;
+}
+// common prologue of the queries: synchronise, the rings of every rank, the number of entries L to return
+static int fs_hist_begin(pfgpu_fs* h, size_t max_steps, Fs3Hist* H, unsigned* L) {
+    if (!h->hist || max_steps == 0) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    int rc = fs_check_err(h);
+    if (rc) return rc;
+    memset(H, 0, sizeof(*H));
+    H->cap = (unsigned)h->hist_cap; H->ld = h->d.ld; H->n = h->d.n;
+    for (int g = 0; g < h->world; ++g) {
+        const pfgpu_fs* o = h->sib[g];
+        const char* b = g == h->rank ? h->hist : o ? o->hist : (const char*)h->hist_peer[g];
+        if (!b || (o && (o->hist_cap != h->hist_cap || o->hist_first != h->hist_first || o->steps != h->steps))) {
+            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: rank %d holds no ring with this window (pfgpu_fs_history_enable, upload and "
+                     "seed_map are made on every rank)", g);
+            return PFGPU_ERR_INVALID;
+        }
+        H->base[g] = b;
+    }
+    *L = (unsigned)std::min<uint64_t>(h->steps - h->hist_first + 1, (uint64_t)std::min<size_t>(max_steps, 0xFFFFFFFFu));
+    return 0;
+}
+
+extern "C" int pfgpu_fs_path(pfgpu_fs* h, size_t index_global, size_t max_steps, uint64_t* step, uint32_t* slot, double* pose3, size_t* n) {
+    if (!h || !n || index_global >= h->d.n_glob) return PFGPU_ERR_INVALID;
+    Fs3Hist H; unsigned L = 0;
+    int rc = fs_hist_begin(h, max_steps, &H, &L);
+    if (rc) return rc;
+    const size_t o_pose = ((size_t)L * sizeof(unsigned) + 255) & ~(size_t)255;
+    rc = fs_hist_scratch(h, o_pose + (size_t)L * 3 * sizeof(double));
+    if (rc) return rc;
+    unsigned* dslot = reinterpret_cast<unsigned*>(h->hs);
+    double* dpose = reinterpret_cast<double*>(h->hs + o_pose);
+    PF_LAUNCH(h->ctx, fs3_hist_path_kernel, 1, 32, 0, H, (unsigned)(h->steps % h->hist_cap), L, (unsigned)index_global, dslot, dpose);
+    std::vector<unsigned> s(L);
+    std::vector<double> p(3 * (size_t)L);
+    PF_CUDA(cudaMemcpyAsync(s.data(), dslot, (size_t)L * sizeof(unsigned), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaMemcpyAsync(p.data(), dpose, (size_t)L * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    for (size_t j = 0; j < L; ++j) {                              // oldest first
+        const size_t k = L - 1 - j;
+        if (step) step[j] = h->steps - k;
+        if (slot) slot[j] = s[k];
+        if (pose3) for (int c = 0; c < 3; ++c) pose3[3 * j + c] = p[3 * k + c];
+    }
+    *n = L;
+    return fs_check_err(h);
+}
+
+extern "C" int pfgpu_fs_path_moments(pfgpu_fs* h, size_t max_steps, uint64_t* step, pfgpu_fs_pose_moments* out, size_t* n) {
+    if (!h || !out || !n) return PFGPU_ERR_INVALID;
+    Fs3Hist H; unsigned L = 0;
+    int rc = fs_hist_begin(h, max_steps, &H, &L);
+    if (rc) return rc;
+    const Fs3Dev& d = h->d;
+    const unsigned nb = cdiv_u(d.n, FS3_HIST_NT);
+    const unsigned Lc = (unsigned)std::max<size_t>(1, std::min<size_t>(L, FS3_HIST_SCRATCH_CAP / ((size_t)nb * sizeof(Fs3PoseMom))));
+    // scratch: centre slots [L] | centres [L][3] | lineage slots [n] | block partials [Lc][nb] | moments [L][13]
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t o_ctr = up((size_t)L * sizeof(unsigned)), o_lin = o_ctr + up((size_t)L * 3 * sizeof(double));
+    const size_t o_part = o_lin + up((size_t)d.n * sizeof(unsigned)), o_out = o_part + up((size_t)Lc * nb * sizeof(Fs3PoseMom));
+    rc = fs_hist_scratch(h, o_out + (size_t)L * sizeof(pfgpu_fs_pose_moments));
+    if (rc) return rc;
+    char* S = h->hs;
+    const double* ctr = reinterpret_cast<const double*>(S + o_ctr);
+    // the centres: the lineage of global slot n - 1, read the same on every rank
+    PF_LAUNCH(h->ctx, fs3_hist_path_kernel, 1, 32, 0, H, (unsigned)(h->steps % h->hist_cap), L, d.n_glob - 1u, reinterpret_cast<unsigned*>(S),
+              reinterpret_cast<double*>(S + o_ctr));
+    for (unsigned k0 = 0; k0 < L; k0 += Lc) {
+        const unsigned k1 = std::min(L, k0 + Lc), e0 = (unsigned)((h->steps - k0) % h->hist_cap);
+        PF_LAUNCH(h->ctx, fs3_hist_moments_kernel, nb, FS3_HIST_NT, 0, d, H, e0, k0, k1, reinterpret_cast<unsigned*>(S + o_lin), ctr,
+                  reinterpret_cast<Fs3PoseMom*>(S + o_part));
+        PF_LAUNCH(h->ctx, fs3_hist_merge_kernel, cdiv_u(k1 - k0, 128), 128, 0, reinterpret_cast<const Fs3PoseMom*>(S + o_part), nb, k0, k1, ctr,
+                  reinterpret_cast<double*>(S + o_out));
+    }
+    std::vector<pfgpu_fs_pose_moments> tmp(L);
+    PF_CUDA(cudaMemcpyAsync(tmp.data(), S + o_out, (size_t)L * sizeof(pfgpu_fs_pose_moments), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    for (size_t j = 0; j < L; ++j) {                              // oldest first
+        const size_t k = L - 1 - j;
+        if (step) step[j] = h->steps - k;
+        out[j] = tmp[k];
+    }
+    *n = L;
+    return fs_check_err(h);
 }

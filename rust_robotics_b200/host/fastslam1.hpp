@@ -20,6 +20,8 @@ struct Estimate {
     std::array<double, 3> pose; std::array<double, 9> pose_cov;
     std::vector<double> mass; std::vector<std::array<double, 2>> mean; std::vector<std::array<double, 4>> cov;
 };
+// one step of a particle's path (include/pfgpu.h pfgpu_fs_path): step number, the lineage's global slot then, its pose
+struct PathEntry { uint64_t step; uint32_t slot; double x, y, yaw; };
 
 class FastSlam {
     pfgpu_fs* h_ = nullptr;
@@ -74,6 +76,24 @@ public:
         check(pfgpu_fs_estimate_merge(&pm, landmarks ? &one : nullptr, 1, m, e.pose.data(), e.pose_cov.data(), e.mass.data(),
                                       m ? e.mean[0].data() : nullptr, m ? e.cov[0].data() : nullptr), "estimate");
         return e;
+    }
+    // path history (no reference counterpart; include/pfgpu.h pfgpu_fs_history_enable): keep the last `capacity` steps of every
+    // particle's path on the device; 0 disables
+    void enable_history(size_t capacity) { check(pfgpu_fs_history_enable(h_, capacity), "enable_history"); }
+    // the path of global slot `index` (the poses of its lineage), oldest first, at most max_steps entries
+    std::vector<PathEntry> path(size_t index, size_t max_steps) const {
+        std::vector<uint64_t> step(max_steps); std::vector<uint32_t> slot(max_steps); std::vector<double> pose(3 * max_steps);
+        size_t n = 0;
+        check(pfgpu_fs_path(h_, index, max_steps, step.data(), slot.data(), pose.data(), &n), "path");
+        std::vector<PathEntry> out(n);
+        for (size_t j = 0; j < n; ++j) out[j] = {step[j], slot[j], pose[3 * j], pose[3 * j + 1], pose[3 * j + 2]};
+        return out;
+    }
+    // the path of the best particle (get_best_particle's index)
+    std::vector<PathEntry> best_path(size_t max_steps) const {
+        size_t idx = 0;
+        check(pfgpu_fs_best(h_, &idx, nullptr), "get_best_particle");
+        return path(idx, max_steps);
     }
     size_t len() const { return n_; }
     // 1 = fastslam1::fastslam_update, 2 = fastslam2::fastslam2_update (crates/rust_robotics_slam/src/fastslam2.rs:376-383)

@@ -96,6 +96,12 @@ extern "C" {
     pub fn pfgpu_fs_estimate_merge(pose: *const pfgpu_fs_pose_moments, lm: *const *const pfgpu_fs_lm_moments, world: c_int, n_landmarks: usize,
                                    pose_mean3: *mut f64, pose_cov9_colmajor: *mut f64, lm_mass: *mut f64, lm_mean2: *mut f64,
                                    lm_cov4: *mut f64) -> c_int;
+    // path history (no reference counterpart): a ring of per-step poses and resample parents, DESIGN §3.6
+    pub fn pfgpu_fs_history_enable(h: *mut pfgpu_fs, capacity: usize) -> c_int;
+    pub fn pfgpu_fs_history_window(h: *mut pfgpu_fs, first_step: *mut u64, last_step: *mut u64) -> c_int;
+    pub fn pfgpu_fs_path(h: *mut pfgpu_fs, index_global: usize, max_steps: usize, step: *mut u64, slot: *mut u32, pose3: *mut f64,
+                         n: *mut usize) -> c_int;
+    pub fn pfgpu_fs_path_moments(h: *mut pfgpu_fs, max_steps: usize, step: *mut u64, out: *mut pfgpu_fs_pose_moments, n: *mut usize) -> c_int;
     pub fn pfgpu_pf_sync(h: *mut pfgpu_pf) -> c_int;
     // multi-GPU: one process per GPU; rank 0 makes the id, the host program broadcasts its 128 bytes, every rank creates
     // its shard with the GLOBAL particle count (INTEGRATION.md "Multi-GPU")

@@ -76,6 +76,20 @@ impl FastSlam {
                    mean: mean2.chunks(2).map(|q| Vector2::new(q[0], q[1])).collect(),
                    cov: cov4.chunks(4).map(|q| Matrix2::new(q[0], q[1], q[2], q[3])).collect() }
     }
+    /// keep the last `capacity` steps of every particle's path on the device (no reference counterpart, DESIGN §3.6); 0 disables
+    pub fn enable_history(&mut self, capacity: usize) {
+        let rc = unsafe { sys::pfgpu_fs_history_enable(self.h, capacity) };
+        assert_eq!(rc, 0, "pfgpu_fs_history_enable failed");
+    }
+    /// the path of global slot `index`, oldest first: (step, slot at that step, pose x y yaw) — the poses that produced the
+    /// particle's map; at most `max_steps` entries
+    pub fn path(&self, index: usize, max_steps: usize) -> Vec<(u64, u32, Vector3<f64>)> {
+        let (mut step, mut slot, mut pose) = (vec![0u64; max_steps], vec![0u32; max_steps], vec![0.0f64; 3 * max_steps]);
+        let mut n = 0usize;
+        let rc = unsafe { sys::pfgpu_fs_path(self.h, index, max_steps, step.as_mut_ptr(), slot.as_mut_ptr(), pose.as_mut_ptr(), &mut n) };
+        assert_eq!(rc, 0, "pfgpu_fs_path failed");
+        (0..n).map(|j| (step[j], slot[j], Vector3::new(pose[3 * j], pose[3 * j + 1], pose[3 * j + 2]))).collect()
+    }
     pub(crate) fn raw(&self) -> *mut sys::pfgpu_fs { self.h }
     /// the reference's Vec<Particle>, materialised (checkpoint / API-compat)
     pub fn download(&self) -> Vec<Particle> {
