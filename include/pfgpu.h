@@ -222,6 +222,24 @@ int  pfgpu_fs_history_enable(pfgpu_fs*, size_t capacity);
 int  pfgpu_fs_history_window(pfgpu_fs*, uint64_t* first_step, uint64_t* last_step);
 int  pfgpu_fs_path(pfgpu_fs*, size_t index_global, size_t max_steps, uint64_t* step, uint32_t* slot, double* pose3, size_t* n);
 int  pfgpu_fs_path_moments(pfgpu_fs*, size_t max_steps, uint64_t* step, pfgpu_fs_pose_moments* out, size_t* n);
+/* Landmark existence counters for unknown data association (not in the reference, which takes ids and never removes a landmark;
+ * the counter of FastSLAM with unknown correspondences, Probabilistic Robotics Table 13.3; DESIGN §3.7).  While enabled every slot
+ * of every particle carries an integer tau, cloned with the particle on resample.  In each pfgpu_fs_step_unknown, per particle:
+ * a match sets tau += 1, a birth tau = 1, a drop changes nothing; then every initialised slot (cov00 < 100) that no observation of
+ * the step matched or bore and that lies within `range` of the sampled pose (sqrt(dx^2 + dy^2) <= range) gets tau -= 1, and a
+ * slot whose tau falls below 0 is removed: reset to the fresh landmark (0, 0, 1000 I), i.e. empty.  k = 0 steps run the same
+ * pass after the motion step.  Weights never depend on tau.
+ * pfgpu_fs_existence_enable: range > 0 (+inf allowed) enables and sets every tau to 1 (so do re-enabling, pfgpu_fs_upload and
+ *   pfgpu_fs_seed_map while enabled); 0 disables and frees; NaN or negative: PFGPU_ERR_INVALID.  8 * m * ld bytes per rank.
+ *   Collective on a sharded engine.  While enabled pfgpu_fs_step (known ids) returns PFGPU_ERR_UNSUPPORTED.  Disabled (the default)
+ *   nothing changes.
+ * pfgpu_fs_existence_counts: tau of local slots first_local .. first_local + count - 1, count x m particle-major; 0 for an empty
+ *   slot.  Synchronises; valid where pfgpu_fs_download is.  Counters disabled: PFGPU_ERR_INVALID.
+ * pfgpu_fs_existence_removed: copies removed by the last pfgpu_fs_step_unknown over this handle's particles (0 when disabled);
+ *   synchronises. */
+int  pfgpu_fs_existence_enable(pfgpu_fs*, double range);
+int  pfgpu_fs_existence_counts(pfgpu_fs*, size_t first_local, size_t count, int32_t* out);
+int  pfgpu_fs_existence_removed(pfgpu_fs*, uint64_t* removed);
 int  pfgpu_fs_sync(pfgpu_fs*);
 
 /* ============================================ plumbing ============================================== */

@@ -79,6 +79,7 @@ EXPORTS = [
     "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
     "pfgpu_fs_moments", "pfgpu_fs_estimate_merge", "pfgpu_fs_step_unknown", "pfgpu_fs_assoc_counts",
     "pfgpu_fs_history_enable", "pfgpu_fs_history_window", "pfgpu_fs_path", "pfgpu_fs_path_moments",
+    "pfgpu_fs_existence_enable", "pfgpu_fs_existence_counts", "pfgpu_fs_existence_removed",
 ]
 
 
@@ -159,6 +160,9 @@ def load_library():
     L.pfgpu_fs_history_window.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.pfgpu_fs_path.argtypes = [vp, C.c_size_t, C.c_size_t, C.POINTER(C.c_uint64), c_u32p, c_dp, C.POINTER(C.c_size_t)]
     L.pfgpu_fs_path_moments.argtypes = [vp, C.c_size_t, C.POINTER(C.c_uint64), C.POINTER(_FsPoseMoments), C.POINTER(C.c_size_t)]
+    L.pfgpu_fs_existence_enable.argtypes = [vp, C.c_double]
+    L.pfgpu_fs_existence_counts.argtypes = [vp, C.c_size_t, C.c_size_t, C.POINTER(C.c_int32)]
+    L.pfgpu_fs_existence_removed.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
     _LIB = L
@@ -734,3 +738,26 @@ class FastSlam2(FastSlam1):
         c = (C.c_uint64 * 3)()
         _check(self.L, self.L.pfgpu_fs_assoc_counts(self.h, c))
         return tuple(int(v) for v in c)
+
+    # -- landmark existence counters (not in fs2.rs, which takes ids and never removes a landmark; DESIGN §3.7) --
+    def enable_existence(self, range=None):
+        """Track an existence counter per landmark copy in fastslam2_update_unknown: +1 per match, 1 at a birth, -1 when the copy
+        lies within `range` of the sampled pose and no observation went to it; below 0 the copy is removed and its slot is empty
+        again.  range=None: config.max_range; inf allowed; 0 disables.  Every counter starts at 1 (also after set_state and
+        seed_map).  While enabled known-id steps are refused.  On a sharded engine every rank makes the same call."""
+        r = self.config.max_range if range is None else float(range)
+        _check(self.L, self.L.pfgpu_fs_existence_enable(self.h, r))
+
+    def existence_counts(self, first=0, count=None):
+        """(count, m) int32: the counters of local slots first .. first + count - 1 (default: all), 0 for an empty slot.  Synchronises."""
+        if count is None:
+            count = self.n_local - first
+        out = np.zeros((count, self.m), dtype=np.int32)
+        _check(self.L, self.L.pfgpu_fs_existence_counts(self.h, int(first), int(count), out.ctypes.data_as(C.POINTER(C.c_int32))))
+        return out
+
+    def removed_count(self):
+        """landmark copies removed by the last fastslam2_update_unknown over this handle's particles (0 when disabled); synchronises"""
+        v = C.c_uint64()
+        _check(self.L, self.L.pfgpu_fs_existence_removed(self.h, C.byref(v)))
+        return int(v.value)

@@ -5,6 +5,7 @@
 #include "fs3_est.cuh"
 #include "fs3_assoc.cuh"
 #include "fs3_hist.cuh"
+#include "fs3_exist.cuh"
 
 struct pfgpu_fs {
     Ctx ctx;
@@ -32,14 +33,20 @@ struct pfgpu_fs {
     double* vtile = nullptr;          // ... here: [post_tiles][post_K][512]
     char* est = nullptr; size_t est_bytes = 0;   // pfgpu_fs_moments scratch, allocated by the first call (fs3_est.cuh)
     double* zbuf = nullptr; size_t zcap = 0;     // pfgpu_fs_step_unknown: the (d, angle) list of the step (grows, never shrinks)
-    unsigned long long* acnt = nullptr;         // [6] association counters: this launch's, then the last unknown step's (fs3_assoc.cuh)
+    unsigned long long* acnt = nullptr;         // [8] association counters: this launch's, then the last unknown step's (fs3_assoc.cuh);
+                                                // [6]: copies removed by the last tracked unknown step (fs3_exist.cuh)
     pfgpu_fs* sib[FS3_MAXG] = {};               // in-process sharded engine: every rank's handle (pfgpu_fs_create_sharded_local)
     char* hist = nullptr; size_t hist_cap = 0;  // path history ring (fs3_hist.cuh), pfgpu_fs_history_enable
     uint64_t hist_first = 0;                    // oldest entry held (a root); the newest is `steps`
     void* hist_peer[FS3_MAXG] = {};             // peers' rings mapped through cudaIpc (one process per GPU)
     char* hs = nullptr; size_t hs_bytes = 0;    // path / path-moments scratch, grows on demand
+    int* ex = nullptr; double ex_range = 0.0;   // landmark existence counters [2][m][ld] and their range (fs3_exist.cuh), pfgpu_fs_existence_enable
+    void* ex_peer[FS3_MAXG] = {};               // peers' counters mapped through cudaIpc (one process per GPU)
 };
 static int fs_hist_record(pfgpu_fs* h, int root);
+static int fs_ex_fill(pfgpu_fs* h);
+static int fs_ex_param(pfgpu_fs* h, Fs3Ex* X);
+static int fs_allgather(pfgpu_fs* h, const void* mine, size_t bytes, void* all);
 
 extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.rs:13-23
     c->dt = 0.1; c->max_range = 20.0; c->nth = 100.0 / 1.5; c->q00 = 0.3; c->q11 = 0.0305; c->r00 = 0.5; c->r11 = 0.0305;
@@ -274,6 +281,8 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(h->zbuf); cudaFree(h->acnt);
     for (int g = 0; g < FS3_MAXG; ++g) if (h->hist_peer[g]) cudaIpcCloseMemHandle(h->hist_peer[g]);
     cudaFree(h->hist); cudaFree(h->hs);
+    for (int g = 0; g < FS3_MAXG; ++g) if (h->ex_peer[g]) cudaIpcCloseMemHandle(h->ex_peer[g]);
+    cudaFree(h->ex);
     if (h->h_rec) cudaFreeHost(h->h_rec);
     if (h->comm) ncclCommDestroy(h->comm);
     marks_free(h->marks);
@@ -325,6 +334,7 @@ extern "C" int pfgpu_fs_upload(pfgpu_fs* h, const double* pose_w, const double* 
         }
         PF_LAUNCH(h->ctx, fs3_lmst_reset_kernel, 1, 256, 0, d);
     }
+    if (h->ex) { rc = fs_ex_fill(h); if (rc) return rc; }       // every existence counter restarts at 1
     return h->hist ? fs_hist_record(h, 1) : 0;       // the uploaded state restarts the path history window
 }
 extern "C" int pfgpu_fs_download(pfgpu_fs* h, double* pose_w, double* lm, size_t n) {
@@ -367,6 +377,7 @@ extern "C" int pfgpu_fs_seed_map(pfgpu_fs* h, const double pose3[3], const doubl
         dim3 grid(cdiv_u(d.n, 256), (unsigned)std::min<size_t>(m, 65535));
         PF_LAUNCH(h->ctx, fs3_seed_lm_kernel, grid, 256, 0, d, h->stage, sigma, cov0, h->seed);
         PF_LAUNCH(h->ctx, fs3_lmst_reset_kernel, 1, 256, 0, d);
+        if (h->ex) { rc = fs_ex_fill(h); if (rc) return rc; }   // every existence counter restarts at 1
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     }
     return 0;
@@ -412,6 +423,11 @@ static int fs3_launch_post(pfgpu_fs* h, const Fs3ObsParam& po, int k_last, bool 
 extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs* z, size_t k, int* did) {
     if (!h || !u || (k && !z)) return PFGPU_ERR_INVALID;
     if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    if (h->ex) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters are enabled: known-id steps are not supported (the EKF launch "
+                 "moves landmarks without their counters); disable them with pfgpu_fs_existence_enable(h, 0) first");
+        return PFGPU_ERR_UNSUPPORTED;
+    }
     Fs3Dev& d = h->d;
     for (size_t j = 0; j < k; ++j) {
         if (!finite_d(z[j].d) || !finite_d(z[j].angle)) return PFGPU_ERR_INVALID;
@@ -489,14 +505,16 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
     PF_CUDA(cudaSetDevice(h->ctx.device));
     Fs3Dev& d = h->d;
     if (!h->acnt) {
-        PF_CUDA(cudaMalloc(&h->acnt, 6 * sizeof(unsigned long long)));
-        PF_CUDA(cudaMemsetAsync(h->acnt, 0, 6 * sizeof(unsigned long long), h->ctx.stream));
+        PF_CUDA(cudaMalloc(&h->acnt, 8 * sizeof(unsigned long long)));
+        PF_CUDA(cudaMemsetAsync(h->acnt, 0, 8 * sizeof(unsigned long long), h->ctx.stream));
     }
-    if (k == 0) {           // no observation: the known-id step with k = 0, bit for bit; nothing was associated
+    Fs3Ex X;
+    if (h->ex) { int rc = fs_ex_param(h, &X); if (rc) return rc; }
+    if (k == 0 && !h->ex) {  // no observation: the known-id step with k = 0, bit for bit; nothing was associated
         PF_CUDA(cudaMemsetAsync(h->acnt + 3, 0, 3 * sizeof(unsigned long long), h->ctx.stream));
         return pfgpu_fs_step(h, u, nullptr, 0, did);
     }
-    if (2 * k > h->zcap) {  // (the previous step may still read the old list: wait for it before the buffer goes)
+    if (k && 2 * k > h->zcap) {  // (the previous step may still read the old list: wait for it before the buffer goes)
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
         cudaFree(h->zbuf); h->zbuf = nullptr; h->zcap = 0;
         const size_t cap = std::max<size_t>(64, 4 * k);
@@ -504,13 +522,19 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
         h->zcap = cap;
     }
     // stream-ordered behind every kernel of the previous step, so a list is never overwritten while a step reads it
-    PF_CUDA(cudaMemcpyAsync(h->zbuf, z2, 2 * k * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+    if (k) PF_CUDA(cudaMemcpyAsync(h->zbuf, z2, 2 * k * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     const bool host_waits = d.G > 1 && !d.wait_inline;
     if (host_waits) PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 1, (unsigned)h->n_step);            // peers' previous post kernels are over
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
-    PF_LAUNCH(h->ctx, fs3_assoc_kernel, cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d, (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1],
-              h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step, h->acnt);
+    if (h->ex) {            // with existence counters (DESIGN §3.7); acnt[6] collects this step's removals
+        PF_CUDA(cudaMemsetAsync(h->acnt + 6, 0, sizeof(unsigned long long), h->ctx.stream));
+        PF_LAUNCH(h->ctx, fs3_assoc_ex_kernel, cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d, X, (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1],
+                  h->cfg.dt, sqrt(h->cfg.q00), sqrt(h->cfg.q11), h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step, h->acnt,
+                  h->acnt + 6);
+    } else
+        PF_LAUNCH(h->ctx, fs3_assoc_kernel, cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d, (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1],
+                  h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step, h->acnt);
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_assoc_mark_kernel, std::max(1u, std::min(cdiv_u(d.m, 256), 64u)), 256, 0, d, h->acnt);
     if (host_waits) {
@@ -538,6 +562,136 @@ extern "C" int pfgpu_fs_assoc_counts(pfgpu_fs* h, uint64_t counts[3]) {
     unsigned long long c[3] = { 0ull, 0ull, 0ull };
     if (h->acnt) PF_CUDA(cudaMemcpy(c, h->acnt + 3, sizeof(c), cudaMemcpyDeviceToHost));
     for (int j = 0; j < 3; ++j) counts[j] = (uint64_t)c[j];
+    return fs_check_err(h);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// landmark existence counters (DESIGN §3.7): pfgpu_fs_existence_enable / _counts / _removed
+// ---------------------------------------------------------------------------------------------------------------------
+static size_t fs_ex_words(const pfgpu_fs* h) { return (size_t)2 * (h->d.m ? h->d.m : 1) * h->d.ld; }
+static int fs_ex_fill(pfgpu_fs* h) {
+    const size_t words = fs_ex_words(h);
+    PF_LAUNCH(h->ctx, fs3_ex_fill_kernel, (unsigned)std::min<size_t>(cdiv_u(words, 256), 4096), 256, 0, h->ex, words);
+    return 0;
+}
+// every rank's counters: own, the siblings' (in-process ranks) or the IPC mappings (one process per GPU)
+static int fs_ex_param(pfgpu_fs* h, Fs3Ex* X) {
+    memset(X, 0, sizeof(*X));
+    X->range = h->ex_range;
+    for (int g = 0; g < h->world; ++g) {
+        const pfgpu_fs* o = h->sib[g];
+        int* b = g == h->rank ? h->ex : o ? o->ex : (int*)h->ex_peer[g];
+        if (!b) {
+            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: rank %d has not enabled them (pfgpu_fs_existence_enable is "
+                     "made on every rank)", g);
+            return PFGPU_ERR_INVALID;
+        }
+        X->base[g] = b;
+    }
+    return 0;
+}
+static void fs_ex_release(pfgpu_fs* h) {
+    for (int g = 0; g < FS3_MAXG; ++g) if (h->ex_peer[g]) { cudaIpcCloseMemHandle(h->ex_peer[g]); h->ex_peer[g] = nullptr; }
+    cudaFree(h->ex); h->ex = nullptr; h->ex_range = 0.0;
+}
+
+extern "C" int pfgpu_fs_existence_enable(pfgpu_fs* h, double range) {
+    if (!h || std::isnan(range) || range < 0.0) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));               // nothing in flight still reads the old counters
+    if (range == 0.0) { fs_ex_release(h); return 0; }
+    if (!h->acnt) {
+        PF_CUDA(cudaMalloc(&h->acnt, 8 * sizeof(unsigned long long)));
+        PF_CUDA(cudaMemset(h->acnt, 0, 8 * sizeof(unsigned long long)));
+    }
+    PF_CUDA(cudaMemset(h->acnt + 6, 0, sizeof(unsigned long long)));
+    if (h->ex) {            // re-enabling: the same storage (and mappings), every counter back to 1
+        h->ex_range = range;
+        int rc = fs_ex_fill(h);
+        if (rc) return rc;
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+        return 0;
+    }
+    int* ex = nullptr;
+    int ok = cudaMalloc(&ex, fs_ex_words(h) * sizeof(int)) == cudaSuccess;
+    if (!ok) { ex = nullptr; cudaGetLastError(); }
+    void* opened[FS3_MAXG] = {};
+    if (h->comm) {          // one process per GPU: every rank maps every peer's counters once; all ranks agree on the outcome
+        struct Rec { cudaIpcMemHandle_t hd; int ok, pad; } mine, all[FS3_MAXG];
+        memset(&mine, 0, sizeof(mine));
+        if (ok && cudaIpcGetMemHandle(&mine.hd, ex) != cudaSuccess) { ok = 0; cudaGetLastError(); }
+        mine.ok = ok;
+        int rc = fs_allgather(h, &mine, sizeof(mine), all);
+        if (rc) { cudaFree(ex); return rc; }
+        for (int g = 0; g < h->world; ++g) ok = ok && all[g].ok;
+        if (!ok) {
+            cudaFree(ex);
+            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: %zu bytes do not fit on every rank", fs_ex_words(h) * sizeof(int));
+            return PFGPU_ERR_CUDA;
+        }
+        int mapped = 1, maps[FS3_MAXG];
+        for (int g = 0; g < h->world; ++g)
+            if (g != h->rank && cudaIpcOpenMemHandle(&opened[g], all[g].hd, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
+                mapped = 0; opened[g] = nullptr; cudaGetLastError();
+            }
+        if (mapped) {       // filled before the second exchange: no rank steps before every rank's counters are 1
+            h->ex = ex; h->ex_range = range;
+            rc = fs_ex_fill(h);
+            h->ex = nullptr;
+            if (!rc && cudaStreamSynchronize(h->ctx.stream) != cudaSuccess) rc = PFGPU_ERR_CUDA;
+            if (rc) mapped = 0;
+        }
+        rc = fs_allgather(h, &mapped, sizeof(int), maps);
+        for (int g = 0; g < h->world && !rc; ++g) mapped = mapped && maps[g];
+        if (rc || !mapped) {
+            for (int g = 0; g < FS3_MAXG; ++g) if (opened[g]) cudaIpcCloseMemHandle(opened[g]);
+            cudaFree(ex);
+            h->ex_range = 0.0;
+            if (!rc) snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: mapping a peer's counters failed");
+            return rc ? rc : PFGPU_ERR_UNSUPPORTED;
+        }
+        h->ex = ex; h->ex_range = range;
+        memcpy(h->ex_peer, opened, sizeof(opened));
+        return 0;
+    }
+    if (!ok) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: %zu bytes do not fit in device memory", fs_ex_words(h) * sizeof(int));
+        return PFGPU_ERR_CUDA;
+    }
+    h->ex = ex; h->ex_range = range;
+    int rc = fs_ex_fill(h);
+    if (rc) return rc;
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_fs_existence_counts(pfgpu_fs* h, size_t first_local, size_t count, int32_t* out) {
+    if (!h || !h->ex || (count && !out) || first_local > h->d.n || count > h->d.n - first_local) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    Fs3Dev& d = h->d;
+    if (!count || !d.m) return 0;
+    Fs3Ex X;
+    int rc = fs_ex_param(h, &X);
+    if (rc) return rc;
+    const size_t per = (size_t)d.m * sizeof(int);
+    size_t chunk = std::max<size_t>(1, FS_XFER_CHUNK_BYTES / per);
+    if (chunk > count) chunk = count;
+    rc = fs_stage(h, chunk * per);
+    if (rc) return rc;
+    for (size_t i0 = 0; i0 < count; i0 += chunk) {
+        const size_t cnt = std::min(chunk, count - i0);
+        PF_LAUNCH(h->ctx, fs3_ex_pack_kernel, cdiv_u(cnt * d.m, 256), 256, 0, d, X, reinterpret_cast<int*>(h->stage), first_local + i0, cnt);
+        PF_CUDA(cudaMemcpyAsync(out + i0 * d.m, h->stage, cnt * per, cudaMemcpyDeviceToHost, h->ctx.stream));
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    }
+    return fs_check_err(h);
+}
+extern "C" int pfgpu_fs_existence_removed(pfgpu_fs* h, uint64_t* removed) {
+    if (!h || !removed) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    unsigned long long c = 0ull;
+    if (h->ex && h->acnt) PF_CUDA(cudaMemcpy(&c, h->acnt + 6, sizeof(c), cudaMemcpyDeviceToHost));
+    *removed = (uint64_t)c;
     return fs_check_err(h);
 }
 extern "C" int pfgpu_fs_set_variant(pfgpu_fs* h, int variant) {

@@ -129,6 +129,27 @@ struct FastSlam : fastslam1::FastSlam {
         check(pfgpu_fs_assoc_counts(handle(), c.data()), "assoc_counts");
         return c;
     }
+    // landmark existence counters (DESIGN §3.7): range > 0 (inf allowed) enables, 0 disables; every counter starts at 1
+    void enable_existence(double range) { check(pfgpu_fs_existence_enable(handle(), range), "enable_existence"); }
+    // the counters of particles first .. first + count - 1, count x m particle-major; 0 for an empty slot
+    std::vector<int32_t> existence_counts(size_t first, size_t count) const {
+        size_t nl = 0, ng = 0, m = 0;
+        check(pfgpu_fs_count(handle(), &nl, &ng, &m), "count");
+        std::vector<int32_t> out(count * m);
+        check(pfgpu_fs_existence_counts(handle(), first, count, out.data()), "existence_counts");
+        return out;
+    }
+    // landmark copies removed by the last update_unknown
+    uint64_t removed_count() const {
+        uint64_t r = 0;
+        check(pfgpu_fs_existence_removed(handle(), &r), "removed_count");
+        return r;
+    }
+    size_t best_index() const {
+        size_t idx = 0;
+        check(pfgpu_fs_best(handle(), &idx, nullptr), "get_best_particle");
+        return idx;
+    }
 };
 inline bool fastslam2_update(FastSlam& particles, const std::array<double, 2>& u, const std::vector<Observation>& z) { return particles.step(u, z); }
 inline bool fastslam2_update_unknown(FastSlam& particles, const std::array<double, 2>& u, const std::vector<std::pair<double, double>>& z) {

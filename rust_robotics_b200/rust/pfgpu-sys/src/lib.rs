@@ -102,6 +102,10 @@ extern "C" {
     pub fn pfgpu_fs_path(h: *mut pfgpu_fs, index_global: usize, max_steps: usize, step: *mut u64, slot: *mut u32, pose3: *mut f64,
                          n: *mut usize) -> c_int;
     pub fn pfgpu_fs_path_moments(h: *mut pfgpu_fs, max_steps: usize, step: *mut u64, out: *mut pfgpu_fs_pose_moments, n: *mut usize) -> c_int;
+    // landmark existence counters for unknown data association (no reference counterpart), DESIGN §3.7
+    pub fn pfgpu_fs_existence_enable(h: *mut pfgpu_fs, range: f64) -> c_int;
+    pub fn pfgpu_fs_existence_counts(h: *mut pfgpu_fs, first_local: usize, count: usize, out: *mut i32) -> c_int;
+    pub fn pfgpu_fs_existence_removed(h: *mut pfgpu_fs, removed: *mut u64) -> c_int;
     pub fn pfgpu_pf_sync(h: *mut pfgpu_pf) -> c_int;
     // multi-GPU: one process per GPU; rank 0 makes the id, the host program broadcasts its 128 bytes, every rank creates
     // its shard with the GLOBAL particle count (INTEGRATION.md "Multi-GPU")

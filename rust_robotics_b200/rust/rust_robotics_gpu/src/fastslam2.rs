@@ -35,3 +35,27 @@ pub fn assoc_counts(particles: &FastSlam) -> [u64; 3] {
     assert_eq!(rc, 0, "pfgpu_fs_assoc_counts failed");
     c
 }
+/// Landmark existence counters (not in fs2.rs, DESIGN §3.7): from now on every `fastslam2_update_unknown` removes landmark copies
+/// that lie within `range` of their particle's pose but keep going unobserved.  `range` > 0 (inf allowed) enables, 0 disables;
+/// every counter starts at 1.  While enabled `fastslam2_update` (known ids) is refused.
+pub fn enable_existence(particles: &mut FastSlam, range: f64) {
+    let rc = unsafe { sys::pfgpu_fs_existence_enable(particles.raw(), range) };
+    assert_eq!(rc, 0, "pfgpu_fs_existence_enable failed");
+}
+/// the counters of particles `first .. first + count`, `count` x m particle-major; 0 for an empty slot
+pub fn existence_counts(particles: &FastSlam, first: usize, count: usize) -> Vec<i32> {
+    let (mut nl, mut ng, mut m) = (0usize, 0usize, 0usize);
+    let rc = unsafe { sys::pfgpu_fs_count(particles.raw(), &mut nl, &mut ng, &mut m) };
+    assert_eq!(rc, 0, "pfgpu_fs_count failed");
+    let mut out = vec![0i32; count * m];
+    let rc = unsafe { sys::pfgpu_fs_existence_counts(particles.raw(), first, count, out.as_mut_ptr()) };
+    assert_eq!(rc, 0, "pfgpu_fs_existence_counts failed");
+    out
+}
+/// landmark copies removed by the last `fastslam2_update_unknown`
+pub fn removed_count(particles: &FastSlam) -> u64 {
+    let mut r = 0u64;
+    let rc = unsafe { sys::pfgpu_fs_existence_removed(particles.raw(), &mut r) };
+    assert_eq!(rc, 0, "pfgpu_fs_existence_removed failed");
+    r
+}
