@@ -46,7 +46,6 @@ struct pfgpu_fs {
 static int fs_hist_record(pfgpu_fs* h, int root);
 static int fs_ex_fill(pfgpu_fs* h);
 static int fs_ex_param(pfgpu_fs* h, Fs3Ex* X);
-static int fs_allgather(pfgpu_fs* h, const void* mine, size_t bytes, void* all);
 
 extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.rs:13-23
     c->dt = 0.1; c->max_range = 20.0; c->nth = 100.0 / 1.5; c->q00 = 0.3; c->q11 = 0.0305; c->r00 = 0.5; c->r11 = 0.0305;
@@ -67,6 +66,65 @@ static int fs_stage(pfgpu_fs* h, size_t bytes) {
     PF_CUDA(cudaMalloc(&h->stage, bytes));
     h->stage_bytes = bytes;
     return 0;
+}
+
+// every rank's `bytes` from `mine` into all[world] over the handle's communicator (one process per GPU)
+static int fs_allgather(pfgpu_fs* h, const void* mine, size_t bytes, void* all, const char* what) {
+    char* buf = nullptr;
+    PF_CUDA(cudaMalloc(&buf, (size_t)(h->world + 1) * bytes));
+    int rc = 0;
+    if (cudaMemcpy(buf + (size_t)h->world * bytes, mine, bytes, cudaMemcpyHostToDevice) != cudaSuccess) rc = PFGPU_ERR_CUDA;
+    else if (ncclAllGather(buf + (size_t)h->world * bytes, buf, bytes, ncclChar, h->comm, h->ctx.stream) != ncclSuccess) rc = PFGPU_ERR_NCCL;
+    else if (cudaStreamSynchronize(h->ctx.stream) != cudaSuccess || cudaMemcpy(all, buf, (size_t)h->world * bytes, cudaMemcpyDeviceToHost) != cudaSuccess)
+        rc = PFGPU_ERR_CUDA;
+    if (rc) { cudaGetLastError(); snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "%s: the exchange between ranks failed", what); }
+    cudaFree(buf);
+    return rc;
+}
+// closes the cudaIpc mappings of peers' buffers (this rank's own entry is never a mapping)
+static void fs_unmap(const pfgpu_fs* h, void* opened[FS3_MAXG]) {
+    for (int g = 0; g < FS3_MAXG; ++g) if (g != h->rank && opened[g]) { cudaIpcCloseMemHandle(opened[g]); opened[g] = nullptr; }
+}
+// One process per GPU: maps this rank's allocation `mine` on every peer rank through cudaIpc, and opened[g] <- rank g's for every
+// peer g.  Collective; every rank returns the same outcome, and on failure nothing stays mapped: PFGPU_ERR_CUDA if some rank's
+// allocation failed (ok = 0), PFGPU_ERR_INVALID if the ranks' tags differ, PFGPU_ERR_UNSUPPORTED if an allocation cannot be
+// exported or mapped, the exchange's own code if that failed.  The second exchange is also a fence: what every rank wrote to its
+// allocation before the call is there before any rank returns.
+static int fs_share(pfgpu_fs* h, void* mine, int ok, uint64_t tag, void* opened[FS3_MAXG], const char* what) {
+    struct Rec { cudaIpcMemHandle_t hd; uint64_t tag; int ok, pad; } me, all[FS3_MAXG];
+    memset(&me, 0, sizeof(me));
+    if (ok && cudaIpcGetMemHandle(&me.hd, mine) == cudaSuccess) ok = 2;       // 2: shared, 1: no cudaIpc export, 0: no allocation
+    else cudaGetLastError();
+    me.tag = tag; me.ok = ok;
+    int rc = fs_allgather(h, &me, sizeof(me), all, what);
+    if (rc) return rc;
+    bool same = true;
+    for (int g = 0; g < h->world; ++g) { ok = std::min(ok, all[g].ok); same = same && all[g].tag == tag; }
+    if (!ok || !same) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), !ok ? "%s: the allocation failed on some rank" : "%s: every rank must pass the same size (%llu here)",
+                 what, (unsigned long long)tag);
+        return !ok ? PFGPU_ERR_CUDA : PFGPU_ERR_INVALID;
+    }
+    int mapped = ok == 2, maps[FS3_MAXG];
+    for (int g = 0; g < h->world && mapped; ++g)
+        if (g != h->rank && cudaIpcOpenMemHandle(&opened[g], all[g].hd, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
+            mapped = 0; opened[g] = nullptr; cudaGetLastError();
+        }
+    rc = fs_allgather(h, &mapped, sizeof(int), maps, what);
+    for (int g = 0; g < h->world && !rc; ++g) mapped = mapped && maps[g];
+    if (rc || !mapped) {
+        fs_unmap(h, opened);
+        if (!rc) snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "%s: mapping a peer's copy through cudaIpc failed (sharded FastSLAM needs peer "
+                          "access between all GPUs)", what);
+        return rc ? rc : PFGPU_ERR_UNSUPPORTED;
+    }
+    return 0;
+}
+// rank g's copy of a per-rank buffer: this rank's own, an in-process sibling's (sib), or the cudaIpc mapping (one process per GPU)
+template <class T>
+static T* fs_rank_buf(const pfgpu_fs* h, int g, T* pfgpu_fs::*own, void* const* mapped) {
+    const pfgpu_fs* o = g == h->rank ? h : h->sib[g];
+    return o ? o->*own : static_cast<T*>(mapped[g]);
 }
 
 static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global, size_t offset, size_t m, uint64_t seed, int device,
@@ -193,29 +251,9 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         memcpy(&id, uid, sizeof(id));
         ncclResult_t nr = ncclCommInitRank(&h->comm, world, id, rank);
         if (nr != ncclSuccess) { snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "ncclCommInitRank: %s", ncclGetErrorString(nr)); return fail(PFGPU_ERR_NCCL); }
-        // map every peer's arena (the 64-byte IPC handles travel over the communicator); all ranks must agree on the outcome
-        int ok = 1;
-        cudaIpcMemHandle_t mine, all[FS3_MAXG];
-        char* d_hand = nullptr;
-        FS_TRY(cudaMalloc(&d_hand, (size_t)(world + 1) * sizeof(cudaIpcMemHandle_t)));
-        if (cudaIpcGetMemHandle(&mine, h->arena) != cudaSuccess) { ok = 0; memset(&mine, 0, sizeof(mine)); cudaGetLastError(); }
-        FS_TRY(cudaMemcpy(d_hand + (size_t)world * sizeof(mine), &mine, sizeof(mine), cudaMemcpyHostToDevice));
-        PF_NCCL(ncclAllGather(d_hand + (size_t)world * sizeof(mine), d_hand, sizeof(mine), ncclChar, h->comm, h->ctx.stream));
-        FS_TRY(cudaStreamSynchronize(h->ctx.stream));
-        FS_TRY(cudaMemcpy(all, d_hand, (size_t)world * sizeof(mine), cudaMemcpyDeviceToHost));
-        for (int g = 0; g < world && ok; ++g) {
-            if (g == rank) continue;
-            if (cudaIpcOpenMemHandle(&h->peer_ptr[g], all[g], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { ok = 0; h->peer_ptr[g] = nullptr; cudaGetLastError(); }
-        }
-        int* d_ok = reinterpret_cast<int*>(d_hand);
-        FS_TRY(cudaMemcpy(d_ok + world, &ok, sizeof(int), cudaMemcpyHostToDevice));
-        PF_NCCL(ncclAllGather(d_ok + world, d_ok, 1, ncclInt, h->comm, h->ctx.stream));     // also the "everybody has zeroed and mapped" fence
-        FS_TRY(cudaStreamSynchronize(h->ctx.stream));
-        int oks[FS3_MAXG];
-        FS_TRY(cudaMemcpy(oks, d_ok, (size_t)world * sizeof(int), cudaMemcpyDeviceToHost));
-        cudaFree(d_hand);
-        for (int g = 0; g < world; ++g) ok = ok && oks[g];
-        if (!ok) { snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "sharded FastSLAM needs peer access between all GPUs (cudaIpc mapping failed)"); return fail(PFGPU_ERR_UNSUPPORTED); }
+        // map every peer's arena; the second exchange is also the "everybody has zeroed and mapped" fence
+        rc = fs_share(h, h->arena, 1, 0, h->peer_ptr, "FastSLAM arena");
+        if (rc) return fail(rc);
         for (int g = 0; g < world; ++g) d.peer[g] = (char*)h->peer_ptr[g];
     }
 #undef FS_TRY
@@ -271,7 +309,9 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaSetDevice(h->ctx.device);
     if (h->ctx.stream) cudaStreamSynchronize(h->ctx.stream);
     Fs3Dev& d = h->d;
-    for (int g = 0; g < h->world; ++g) if (g != h->rank && h->peer_ptr[g]) cudaIpcCloseMemHandle(h->peer_ptr[g]);   // (local mode: none were opened)
+    fs_unmap(h, h->peer_ptr);                      // (local mode: none were opened)
+    fs_unmap(h, h->hist_peer);
+    fs_unmap(h, h->ex_peer);
     cudaFree(h->arena);
     cudaFree(d.st); cudaFree(d.lmst); cudaFree(d.w); cudaFree(d.nz[0]); cudaFree(d.nz[1]); cudaFree(d.wn_all); cudaFree(d.cum_all); cudaFree(d.rcomb_all); cudaFree(d.idx);
     cudaFree(d.tileP); cudaFree(d.tileQ); cudaFree(d.entCnt); cudaFree(d.entKey); cudaFree(d.entTile); cudaFree(d.entP); cudaFree(d.entV); cudaFree(d.entL);
@@ -279,10 +319,7 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
     cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage); cudaFree(h->est);
     cudaFree(h->zbuf); cudaFree(h->acnt);
-    for (int g = 0; g < FS3_MAXG; ++g) if (h->hist_peer[g]) cudaIpcCloseMemHandle(h->hist_peer[g]);
-    cudaFree(h->hist); cudaFree(h->hs);
-    for (int g = 0; g < FS3_MAXG; ++g) if (h->ex_peer[g]) cudaIpcCloseMemHandle(h->ex_peer[g]);
-    cudaFree(h->ex);
+    cudaFree(h->hist); cudaFree(h->hs); cudaFree(h->ex);
     if (h->h_rec) cudaFreeHost(h->h_rec);
     if (h->comm) ncclCommDestroy(h->comm);
     marks_free(h->marks);
@@ -407,16 +444,26 @@ static int fs3_launch_ekf(pfgpu_fs* h, const Fs3ObsParam& po, const double u[2],
     return 0;
 }
 
-// normalise, N_eff gate and (when it opens) the whole resample of step h->n_step: one launch.  po / k_last: the last EKF launch's
-// observations, whose lazy-clone bookkeeping the post kernel applies (k_last = 0: none)
-static int fs3_launch_post(pfgpu_fs* h, const Fs3ObsParam& po, int k_last, bool host_waits) {
+// The end of step h->n_step, from the host-side signal / wait pair on.  The post kernel normalises, evaluates the N_eff gate and
+// (when it opens) runs the whole resample in one launch; po / k_last: the last EKF launch's observations, whose lazy-clone
+// bookkeeping the post kernel applies (k_last = 0: none).
+static int fs_step_end(pfgpu_fs* h, const Fs3ObsParam& po, int k_last, bool host_waits, int* did) {
     const Fs3Dev& d = h->d;
-    if (h->post_global)
-        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, true>), h->post_tiles, 512, 0, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
-    else if (h->post_nt == 512)
-        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<512, false>), h->post_tiles, 512, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
-    else
-        PF_LAUNCH_PDL(h->ctx, h->pdl, (fs3_post_kernel<256, false>), h->post_tiles, 256, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K, h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    if (host_waits) {      // the post kernel signals "my weights are pushed" itself; the wait for the others' is its own launch here
+        PF_LAUNCH(h->ctx, fs3_signal_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
+        PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
+    }
+    auto post = h->post_global ? fs3_post_kernel<512, true> : h->post_nt == 512 ? fs3_post_kernel<512, false> : fs3_post_kernel<256, false>;
+    PF_LAUNCH_PDL(h->ctx, h->pdl, post, h->post_tiles, h->post_nt, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K,
+                  h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
+    h->n_step++;
+    h->steps++;
+    if (h->hist) { int rc = fs_hist_record(h, 0); if (rc) return rc; }      // entry `steps` of the path history (one launch)
+    if (did) {     // the gate lives on the device; only a caller who asks pays a sync
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+        *did = h->h_rec->gate;
+        return fs_check_err(h);
+    }
     return 0;
 }
 
@@ -475,21 +522,13 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
         k_last = (int)kk;
     }
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
-    if (host_waits) {      // the post kernel signals "my weights are pushed" itself; the wait for the others' is its own launch here
-        PF_LAUNCH(h->ctx, fs3_signal_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
-        PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
-    }
-    // normalise, N_eff gate and (when it opens) the whole resample: one launch
-    int rc = fs3_launch_post(h, po, k_last, host_waits);
-    if (rc) return rc;
-    h->n_step++;
-    h->steps++;
-    if (h->hist) { rc = fs_hist_record(h, 0); if (rc) return rc; }      // entry `steps` of the path history (one launch)
-    if (did) {     // the gate lives on the device; only a caller who asks pays a sync
-        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-        *did = h->h_rec->gate;
-        return fs_check_err(h);
-    }
+    return fs_step_end(h, po, k_last, host_waits, did);
+}
+// the association counters [8] (fs3_assoc.cuh), allocated and cleared on the handle's stream by the first call that needs them
+static int fs_acnt(pfgpu_fs* h) {
+    if (h->acnt) return 0;
+    PF_CUDA(cudaMalloc(&h->acnt, 8 * sizeof(unsigned long long)));
+    PF_CUDA(cudaMemsetAsync(h->acnt, 0, 8 * sizeof(unsigned long long), h->ctx.stream));
     return 0;
 }
 // FastSLAM 2.0 with unknown data association (DESIGN §3.5): fs3_assoc_kernel, the lazy-clone bookkeeping, then the post kernel
@@ -504,12 +543,10 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
     for (size_t j = 0; j < 2 * k; ++j) if (!finite_d(z2[j])) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
     Fs3Dev& d = h->d;
-    if (!h->acnt) {
-        PF_CUDA(cudaMalloc(&h->acnt, 8 * sizeof(unsigned long long)));
-        PF_CUDA(cudaMemsetAsync(h->acnt, 0, 8 * sizeof(unsigned long long), h->ctx.stream));
-    }
-    Fs3Ex X;
-    if (h->ex) { int rc = fs_ex_param(h, &X); if (rc) return rc; }
+    int rc = fs_acnt(h);
+    if (rc) return rc;
+    Fs3Ex X = {};            // zero without existence counters
+    if (h->ex) { rc = fs_ex_param(h, &X); if (rc) return rc; }
     if (k == 0 && !h->ex) {  // no observation: the known-id step with k = 0, bit for bit; nothing was associated
         PF_CUDA(cudaMemsetAsync(h->acnt + 3, 0, 3 * sizeof(unsigned long long), h->ctx.stream));
         return pfgpu_fs_step(h, u, nullptr, 0, did);
@@ -527,33 +564,16 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
     if (host_waits) PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 1, (unsigned)h->n_step);            // peers' previous post kernels are over
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
-    if (h->ex) {            // with existence counters (DESIGN §3.7); acnt[6] collects this step's removals
-        PF_CUDA(cudaMemsetAsync(h->acnt + 6, 0, sizeof(unsigned long long), h->ctx.stream));
-        PF_LAUNCH(h->ctx, fs3_assoc_ex_kernel, cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d, X, (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1],
-                  h->cfg.dt, sqrt(h->cfg.q00), sqrt(h->cfg.q11), h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step, h->acnt,
-                  h->acnt + 6);
-    } else
-        PF_LAUNCH(h->ctx, fs3_assoc_kernel, cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d, (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1],
-                  h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step, h->acnt);
+    // with existence counters (DESIGN §3.7), acnt[6] collects this step's removals
+    if (h->ex) PF_CUDA(cudaMemsetAsync(h->acnt + 6, 0, sizeof(unsigned long long), h->ctx.stream));
+    PF_LAUNCH(h->ctx, (h->ex ? fs3_assoc_kernel<true> : fs3_assoc_kernel<false>), cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d,
+              (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1], h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step,
+              h->acnt, X, sqrt(h->cfg.q00), sqrt(h->cfg.q11), h->ex ? h->acnt + 6 : nullptr);
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_assoc_mark_kernel, std::max(1u, std::min(cdiv_u(d.m, 256), 64u)), 256, 0, d, h->acnt);
-    if (host_waits) {
-        PF_LAUNCH(h->ctx, fs3_signal_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
-        PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
-    }
     Fs3ObsParam po;
     memset(&po, 0, sizeof(po));
-    int rc = fs3_launch_post(h, po, 0, host_waits);
-    if (rc) return rc;
-    h->n_step++;
-    h->steps++;
-    if (h->hist) { rc = fs_hist_record(h, 0); if (rc) return rc; }      // entry `steps` of the path history (one launch)
-    if (did) {
-        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-        *did = h->h_rec->gate;
-        return fs_check_err(h);
-    }
-    return 0;
+    return fs_step_end(h, po, 0, host_waits, did);
 }
 extern "C" int pfgpu_fs_assoc_counts(pfgpu_fs* h, uint64_t counts[3]) {
     if (!h || !counts) return PFGPU_ERR_INVALID;
@@ -579,8 +599,7 @@ static int fs_ex_param(pfgpu_fs* h, Fs3Ex* X) {
     memset(X, 0, sizeof(*X));
     X->range = h->ex_range;
     for (int g = 0; g < h->world; ++g) {
-        const pfgpu_fs* o = h->sib[g];
-        int* b = g == h->rank ? h->ex : o ? o->ex : (int*)h->ex_peer[g];
+        int* b = fs_rank_buf(h, g, &pfgpu_fs::ex, h->ex_peer);
         if (!b) {
             snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: rank %d has not enabled them (pfgpu_fs_existence_enable is "
                      "made on every rank)", g);
@@ -591,7 +610,7 @@ static int fs_ex_param(pfgpu_fs* h, Fs3Ex* X) {
     return 0;
 }
 static void fs_ex_release(pfgpu_fs* h) {
-    for (int g = 0; g < FS3_MAXG; ++g) if (h->ex_peer[g]) { cudaIpcCloseMemHandle(h->ex_peer[g]); h->ex_peer[g] = nullptr; }
+    fs_unmap(h, h->ex_peer);
     cudaFree(h->ex); h->ex = nullptr; h->ex_range = 0.0;
 }
 
@@ -600,68 +619,26 @@ extern "C" int pfgpu_fs_existence_enable(pfgpu_fs* h, double range) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));               // nothing in flight still reads the old counters
     if (range == 0.0) { fs_ex_release(h); return 0; }
-    if (!h->acnt) {
-        PF_CUDA(cudaMalloc(&h->acnt, 8 * sizeof(unsigned long long)));
-        PF_CUDA(cudaMemset(h->acnt, 0, 8 * sizeof(unsigned long long)));
-    }
-    PF_CUDA(cudaMemset(h->acnt + 6, 0, sizeof(unsigned long long)));
+    int rc = fs_acnt(h);
+    if (rc) return rc;
+    PF_CUDA(cudaMemsetAsync(h->acnt + 6, 0, sizeof(unsigned long long), h->ctx.stream));
     if (h->ex) {            // re-enabling: the same storage (and mappings), every counter back to 1
         h->ex_range = range;
-        int rc = fs_ex_fill(h);
+        rc = fs_ex_fill(h);
         if (rc) return rc;
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
         return 0;
     }
-    int* ex = nullptr;
-    int ok = cudaMalloc(&ex, fs_ex_words(h) * sizeof(int)) == cudaSuccess;
-    if (!ok) { ex = nullptr; cudaGetLastError(); }
-    void* opened[FS3_MAXG] = {};
-    if (h->comm) {          // one process per GPU: every rank maps every peer's counters once; all ranks agree on the outcome
-        struct Rec { cudaIpcMemHandle_t hd; int ok, pad; } mine, all[FS3_MAXG];
-        memset(&mine, 0, sizeof(mine));
-        if (ok && cudaIpcGetMemHandle(&mine.hd, ex) != cudaSuccess) { ok = 0; cudaGetLastError(); }
-        mine.ok = ok;
-        int rc = fs_allgather(h, &mine, sizeof(mine), all);
-        if (rc) { cudaFree(ex); return rc; }
-        for (int g = 0; g < h->world; ++g) ok = ok && all[g].ok;
-        if (!ok) {
-            cudaFree(ex);
-            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: %zu bytes do not fit on every rank", fs_ex_words(h) * sizeof(int));
-            return PFGPU_ERR_CUDA;
-        }
-        int mapped = 1, maps[FS3_MAXG];
-        for (int g = 0; g < h->world; ++g)
-            if (g != h->rank && cudaIpcOpenMemHandle(&opened[g], all[g].hd, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
-                mapped = 0; opened[g] = nullptr; cudaGetLastError();
-            }
-        if (mapped) {       // filled before the second exchange: no rank steps before every rank's counters are 1
-            h->ex = ex; h->ex_range = range;
-            rc = fs_ex_fill(h);
-            h->ex = nullptr;
-            if (!rc && cudaStreamSynchronize(h->ctx.stream) != cudaSuccess) rc = PFGPU_ERR_CUDA;
-            if (rc) mapped = 0;
-        }
-        rc = fs_allgather(h, &mapped, sizeof(int), maps);
-        for (int g = 0; g < h->world && !rc; ++g) mapped = mapped && maps[g];
-        if (rc || !mapped) {
-            for (int g = 0; g < FS3_MAXG; ++g) if (opened[g]) cudaIpcCloseMemHandle(opened[g]);
-            cudaFree(ex);
-            h->ex_range = 0.0;
-            if (!rc) snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: mapping a peer's counters failed");
-            return rc ? rc : PFGPU_ERR_UNSUPPORTED;
-        }
-        h->ex = ex; h->ex_range = range;
-        memcpy(h->ex_peer, opened, sizeof(opened));
-        return 0;
-    }
+    // every counter is 1 before the exchange below, so before any rank can step
+    int ok = cudaMalloc(&h->ex, fs_ex_words(h) * sizeof(int)) == cudaSuccess;
     if (!ok) {
+        h->ex = nullptr; cudaGetLastError();
         snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters: %zu bytes do not fit in device memory", fs_ex_words(h) * sizeof(int));
-        return PFGPU_ERR_CUDA;
-    }
-    h->ex = ex; h->ex_range = range;
-    int rc = fs_ex_fill(h);
-    if (rc) return rc;
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    } else ok = fs_ex_fill(h) == 0 && cudaStreamSynchronize(h->ctx.stream) == cudaSuccess;
+    // one process per GPU: every rank maps every peer's counters once
+    rc = h->comm ? fs_share(h, h->ex, ok, 0, h->ex_peer, "landmark existence counters") : ok ? 0 : PFGPU_ERR_CUDA;
+    if (rc) { fs_ex_release(h); return rc; }
+    h->ex_range = range;
     return 0;
 }
 extern "C" int pfgpu_fs_existence_counts(pfgpu_fs* h, size_t first_local, size_t count, int32_t* out) {
@@ -944,23 +921,9 @@ static int fs_hist_record(pfgpu_fs* h, int root) {
     return 0;
 }
 static void fs_hist_release(pfgpu_fs* h) {
-    for (int g = 0; g < FS3_MAXG; ++g) if (h->hist_peer[g]) { cudaIpcCloseMemHandle(h->hist_peer[g]); h->hist_peer[g] = nullptr; }
+    fs_unmap(h, h->hist_peer);
     cudaFree(h->hist); h->hist = nullptr; h->hist_cap = 0; h->hist_first = 0;
 }
-// every rank's `bytes` from `mine` into all[world] over the handle's communicator (one process per GPU)
-static int fs_allgather(pfgpu_fs* h, const void* mine, size_t bytes, void* all) {
-    char* buf = nullptr;
-    PF_CUDA(cudaMalloc(&buf, (size_t)(h->world + 1) * bytes));
-    int rc = 0;
-    if (cudaMemcpy(buf + (size_t)h->world * bytes, mine, bytes, cudaMemcpyHostToDevice) != cudaSuccess) rc = PFGPU_ERR_CUDA;
-    else if (ncclAllGather(buf + (size_t)h->world * bytes, buf, bytes, ncclChar, h->comm, h->ctx.stream) != ncclSuccess) rc = PFGPU_ERR_NCCL;
-    else if (cudaStreamSynchronize(h->ctx.stream) != cudaSuccess || cudaMemcpy(all, buf, (size_t)h->world * bytes, cudaMemcpyDeviceToHost) != cudaSuccess)
-        rc = PFGPU_ERR_CUDA;
-    if (rc) { cudaGetLastError(); snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: exchanging ring handles failed"); }
-    cudaFree(buf);
-    return rc;
-}
-
 extern "C" int pfgpu_fs_history_enable(pfgpu_fs* h, size_t capacity) {
     if (!h) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
@@ -971,34 +934,9 @@ extern "C" int pfgpu_fs_history_enable(pfgpu_fs* h, size_t capacity) {
     int ok = capacity <= 0xFFFFFFFFull && capacity <= SIZE_MAX / per;
     if (ok && cudaMalloc(&ring, capacity * per) != cudaSuccess) { ok = 0; ring = nullptr; cudaGetLastError(); }
     void* opened[FS3_MAXG] = {};
-    if (h->comm) {          // one process per GPU: every rank maps every peer's ring once; all ranks agree on the outcome
-        struct Rec { cudaIpcMemHandle_t hd; uint64_t cap; int ok, pad; } mine, all[FS3_MAXG];
-        memset(&mine, 0, sizeof(mine));
-        if (ok && cudaIpcGetMemHandle(&mine.hd, ring) != cudaSuccess) { ok = 0; cudaGetLastError(); }
-        mine.cap = capacity; mine.ok = ok;
-        int rc = fs_allgather(h, &mine, sizeof(mine), all);
+    if (h->comm) {          // one process per GPU: every rank maps every peer's ring once, with the same capacity everywhere
+        const int rc = fs_share(h, ring, ok, capacity, opened, "path history");
         if (rc) { cudaFree(ring); return rc; }
-        bool same = true;
-        for (int g = 0; g < h->world; ++g) { ok = ok && all[g].ok; same = same && all[g].cap == capacity; }
-        if (!ok || !same) {
-            cudaFree(ring);
-            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), !ok ? "path history: a ring of %zu entries does not fit on every rank"
-                                                            : "path history: every rank must enable the same capacity (%zu here)", capacity);
-            return !ok ? PFGPU_ERR_CUDA : PFGPU_ERR_INVALID;
-        }
-        int mapped = 1, maps[FS3_MAXG];
-        for (int g = 0; g < h->world; ++g)
-            if (g != h->rank && cudaIpcOpenMemHandle(&opened[g], all[g].hd, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
-                mapped = 0; opened[g] = nullptr; cudaGetLastError();
-            }
-        rc = fs_allgather(h, &mapped, sizeof(int), maps);
-        for (int g = 0; g < h->world && !rc; ++g) mapped = mapped && maps[g];
-        if (rc || !mapped) {
-            for (int g = 0; g < FS3_MAXG; ++g) if (opened[g]) cudaIpcCloseMemHandle(opened[g]);
-            cudaFree(ring);
-            if (!rc) snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: mapping a peer's ring failed");
-            return rc ? rc : PFGPU_ERR_UNSUPPORTED;
-        }
     } else if (!ok) {
         snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: a ring of %zu entries x %u slots does not fit in device memory", capacity, h->d.ld);
         return PFGPU_ERR_CUDA;
@@ -1036,7 +974,7 @@ static int fs_hist_begin(pfgpu_fs* h, size_t max_steps, Fs3Hist* H, unsigned* L)
     H->cap = (unsigned)h->hist_cap; H->ld = h->d.ld; H->n = h->d.n;
     for (int g = 0; g < h->world; ++g) {
         const pfgpu_fs* o = h->sib[g];
-        const char* b = g == h->rank ? h->hist : o ? o->hist : (const char*)h->hist_peer[g];
+        const char* b = fs_rank_buf(h, g, &pfgpu_fs::hist, h->hist_peer);
         if (!b || (o && (o->hist_cap != h->hist_cap || o->hist_first != h->hist_first || o->steps != h->steps))) {
             snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "path history: rank %d holds no ring with this window (pfgpu_fs_history_enable, upload and "
                      "seed_map are made on every rank)", g);
