@@ -573,23 +573,34 @@ __device__ __forceinline__ double fs3_value(const Fs3Dev& d, int slot, size_t i,
     if (slot == 3) return S2 > 0.0 ? fs3_div(w, S2) : w;
     return i == 0 ? r0 : inv;
 }
-// exact by construction: one thread walks all values in order (bad values, too many dirty ones, failed certificate)
+// exact by construction: one thread walks all values in order (bad values, too many dirty ones, failed certificate).
+// The CDF (slot 3) is stored as its running maximum, NaN sticky: on a CDF that goes down (negative weights) or turns NaN the
+// lower bound of r in it is the reference's index, the first j with !(c_j < r) (fs1.rs:224-226 carries j over slots with
+// non-decreasing r); on a non-decreasing CDF it is the CDF itself.
+__device__ __forceinline__ double fs3_runmax(double m, double c) { return (m != m || c <= m) ? m : c; }
 template <int NT, bool GT = false>
 __device__ __noinline__ void fs3_serial_walk(const Fs3Dev& d, Fs3Sh<NT>& sh, unsigned K, int slot, double* out, int par, double S2, double r0, double inv) {
     if (threadIdx.x == 0) {
         const size_t T = (size_t)NT * K, lo = (size_t)blockIdx.x * T;
-        double s = 0.0;
+        double s = 0.0, mx = -INFINITY, mbase = -INFINITY;
         sh.tbase = 0.0;
 #pragma unroll 1
-        for (size_t i = 0; i < d.n_glob; ++i) { if (i == lo) sh.tbase = s; s = s + fs3_value(d, slot, i, par, S2, r0, inv); }
+        for (size_t i = 0; i < d.n_glob; ++i) {
+            if (i == lo) { sh.tbase = s; mbase = mx; }
+            s = s + fs3_value(d, slot, i, par, S2, r0, inv);
+            if (slot == 3) mx = fs3_runmax(mx, s);
+        }
         if (lo >= d.n_glob) sh.tbase = s;
         sh.total = s;
         if (blockIdx.x == 0) d.st->serial_walks += 1;
         if (out) {
-            double c = sh.tbase;
+            double c = sh.tbase, m = mbase;
 #pragma unroll 1
-            for (size_t i = lo; i < lo + T && i < d.n_glob; ++i) { c = c + fs3_value(d, slot, i, par, S2, r0, inv); out[i] = c; }
-            if (slot == 3) d.tileEnd[blockIdx.x] = c;
+            for (size_t i = lo; i < lo + T && i < d.n_glob; ++i) {
+                c = c + fs3_value(d, slot, i, par, S2, r0, inv);
+                if (slot == 3) { m = fs3_runmax(m, c); out[i] = m; } else out[i] = c;
+            }
+            if (slot == 3) d.tileEnd[blockIdx.x] = m;
         }
     }
     __syncthreads();
@@ -1011,13 +1022,6 @@ __device__ __noinline__ int fs3_xsum_emit(const Fs3Dev& d, Fs3Sh<NT>& sh, const 
     return near;
 }
 
-// lower bound of r in the exact CDF, clamped: "while r > cum_sum[j+1] && j < n-1 { j += 1 }" (fs1.rs:224-226) with r and j both
-// non-decreasing over the slots, i.e. the first j with c_j >= r.  Searched inside [lo, hi) (c_{lo-1} < r guaranteed by the caller).
-__device__ __forceinline__ unsigned fs3_lower_bound(const double* c, unsigned lo, unsigned hi, double r) {
-#pragma unroll 1
-    while (lo < hi) { const unsigned mid = lo + ((hi - lo) >> 1); if (__ldcg(c + mid) < r) lo = mid + 1; else hi = mid; }
-    return lo;
-}
 // warp-cooperative 32-way search of one r over c[0 .. n): returns the lower bound (all lanes)
 __device__ __forceinline__ unsigned fs3_warp_search(const double* c, unsigned n, double r) {
     const int lane = threadIdx.x & 31;
@@ -1137,8 +1141,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         if (__syncthreads_or(near) && tid == 0) d.flagsg[FS3_CERT_FLAG] = 1;
         FS3_TRACE(4);
     }
-    // w = w_raw / S; best particle of the tile (LAST maximum, fs1.rs:269-274)
-    double bw = -1.0; unsigned bi = 0;
+    // w = w_raw / S; best particle of the tile (LAST maximum, fs1.rs:269-274; from -inf, so weights below -1 take part too)
+    double bw = -INFINITY; unsigned bi = 0;
 #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) {
         double v = vals[k * NT + tid];
@@ -1374,7 +1378,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     if (tid < 8) { d.bar[tid] = 0u; d.resflag[tid] = 0u; }
     if (tid < 32) {
         // best particle: the last maximum over the tiles (no resample) / the last slot (after a resample every weight is 1/n)
-        double bw2 = -1.0; unsigned bi2 = 0;
+        double bw2 = -INFINITY; unsigned bi2 = 0;
 #pragma unroll 1
         for (unsigned x = tid; x < nt; x += 32) { const double ow = __ldcg(d.tileBw + x); const unsigned oi = __ldcg(d.tileBi + x); if (ow > bw2 || (ow == bw2 && oi > bi2)) { bw2 = ow; bi2 = oi; } }
 #pragma unroll 1

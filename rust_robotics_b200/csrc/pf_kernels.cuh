@@ -122,8 +122,10 @@ __global__ void pf_force_last_kernel(PfDev d) {
 }
 
 // index search: first i with r <= c_i (pf.rs:459-465, fallback 0; mcl.rs:387-392, fallback len-1).
-// The cumulative weights are non-decreasing, so the linear scan equals a lower_bound.
-__global__ void __launch_bounds__(PF_NT) pf_search_kernel(PfDev d, uint64_t seed, int mode) {
+// Non-negative finite weights give non-decreasing cumulative weights, so the linear scan equals a lower_bound.  `bad`: the scan
+// of the cumulative weights saw a negative, infinite or NaN weight (xs flags[3]); then the CDF may go down or hold NaN, which
+// the linear scan skips, and each slot scans as the reference does.
+__global__ void __launch_bounds__(PF_NT) pf_search_kernel(PfDev d, uint64_t seed, int mode, const int* bad) {
     if (!*d.gate) return;
     const size_t t = (size_t)blockIdx.x * PF_NT + threadIdx.x;
     if (t >= d.n) return;
@@ -131,6 +133,10 @@ __global__ void __launch_bounds__(PF_NT) pf_search_kernel(PfDev d, uint64_t seed
     double r = pfc_u01_53(pfc_blk_u64(pfc_rng_block(seed, PFC_STREAM_PF_RESAMPLE, call, d.offset + t), 0));
     const double* __restrict__ c = d.cum;
     size_t lo = 0, hi = d.n;
+    if (*bad) {
+        while (lo < d.n && !(r <= c[lo])) ++lo;
+        hi = lo;
+    }
     while (lo < hi) {
         size_t mid = lo + ((hi - lo) >> 1);
         if (c[mid] < r) lo = mid + 1; else hi = mid;

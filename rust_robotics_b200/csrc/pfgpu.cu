@@ -573,7 +573,7 @@ static int pf_resample_impl(pfgpu_pf* h) {
     h->xs.gate = nullptr;
     if (rc) return rc;
     if (h->cfg.mode == 1) PF_LAUNCH(h->ctx, pf_force_last_kernel, 1, 1, 0, d);
-    PF_LAUNCH(h->ctx, pf_search_kernel, cdiv_u(d.n, PF_NT), PF_NT, 0, d, h->seed, h->cfg.mode);
+    PF_LAUNCH(h->ctx, pf_search_kernel, cdiv_u(d.n, PF_NT), PF_NT, 0, d, h->seed, h->cfg.mode, h->xs.flags + 3);
     PF_LAUNCH(h->ctx, pf_gather_kernel, cdiv_u(d.n, PF_NT), PF_NT, 0, d);
     PF_LAUNCH(h->ctx, pf_flip_kernel, 1, 1, 0, d);
     return 0;
