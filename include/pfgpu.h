@@ -246,7 +246,9 @@ int  pfgpu_fs_sync(pfgpu_fs*);
 int  pfgpu_nccl_unique_id(void* out128);     /* ncclGetUniqueId; 128 bytes */
 
 /* Counters for benches / tests.  kernel_launches = kernels of this library launched by the handle;
- * serial_fallbacks = times an exact-sum pipeline fell back to its single-thread path (should be 0). */
+ * serial_fallbacks = times an exact-sum pipeline fell back to its single-thread path (should be 0).  PF / MCL with the fused
+ * step (one launch after predict + likelihood): the separate kernels' count + the fused launch's serial walks + its refused
+ * certificates, and xsum_dirty_last comes from whichever of the two ran the most recent exact sum. */
 typedef struct {
     uint64_t kernel_launches;
     uint64_t steps;

@@ -34,6 +34,7 @@
 // kernel of step s waits for all arrive == s+1.  done[g] = step+1 after rank g's post kernel; the EKF kernel of step s+1
 // waits for all done == s+1 (rows / poses / maps of a peer are only read between those two points, when nobody writes them).
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "x3_core.h"
 #include "../../include/fs_ekf_math.h"
@@ -43,13 +44,20 @@
 #define FS3_MAX_OBS 31            // observations per EKF launch (one warp each, plus the helper warp)
 #define FS3_MAX_TILES 160
 #define FS3_ENT_CAP 512           // dirty values itemised per sum (more: that sum takes the serial walk)
-#define FS3_SLOTS 5               // S, Q (border only), S2, cdf, comb (n not a power of two)
+#define FS3_ROUNDS 8              // grid-barrier rounds per launch (each one arrival counter, each exact sum one round)
 #define FS3_SPIN_LIMIT (1u << 27)
 #define FS3_MAX_LM 65536          // landmarks per particle: row ids (< m) fit the u16 row list
 #define FS3_ROW_CHUNK 1024        // live rows a post-kernel CTA lists in shared memory at a time (more: several passes)
-#define FS3_CERT_FLAG FS3_SLOTS   // flagsg[FS3_CERT_FLAG]: some CTA could not certify its piece of the CDF
 #define FS3_CERT_MAX_LOG2N 16     // certified CDF up to 2^16 particles: about 4 n^3 2^-53 comb values fall within its bound of a
                                   // CDF value, 1/8 at 2^16, 1 at 2^17, 64 at 2^19 (where it would almost always be refused)
+
+// Sum slots (what fs3_value adds): raw weights, squares of the normalised ones (PF / MCL N_eff near its threshold), the normalised
+// ones, the normalised ones / S2 (the CDF), the comb (n not a power of two).  flagsg[FS3_CERT_FLAG]: a CTA refused the certificate.
+enum Fs3Slot { FS3_S, FS3_Q, FS3_S2, FS3_CDF, FS3_COMB, FS3_SLOTS, FS3_CERT_FLAG = FS3_SLOTS };
+// Grid-barrier rounds (< FS3_ROUNDS), one meaning each.  An exact sum's round also indexes where it publishes its results, and
+// its parity picks the half of the block scratch (Fs3Sh::wd / wu / wi): two sums of one parity need a block barrier between them.
+enum Fs3Round { FS3_R_S, FS3_R_S2, FS3_R_CDF, FS3_R_COMB, FS3_R_CERT, FS3_R_CDF_DONE, FS3_R_BORDER };   // fs3_post_kernel
+enum Pf3Round { PF3_R_S, PF3_R_Q, PF3_R_CDF, PF3_R_CDF_DONE, PF3_R_TILES };                           // pf3_post_kernel (pf3.cuh)
 
 __host__ __device__ __forceinline__ unsigned fs3_bm_words(unsigned m) { return (m + 31u) / 32u; }
 __host__ __device__ __forceinline__ unsigned fs3_bm_ld(unsigned m) { return fs3_bm_words(m) + FS3_MAX_TILES; }
@@ -77,6 +85,42 @@ struct Fs3Rec {                   // mapped pinned host memory: what a caller re
 };
 
 struct Fs3Res { double total; unsigned long long Ptot; int D; int fail; };
+// Workspace of the exact sums (fs3_xsum, fs3_xsum_emit, fs3_serial_walk) and grid barriers of one post kernel (fs3_sum_alloc)
+struct Fs3Sum {
+    unsigned long long* tileP; double* tileQ;                  // [FS3_SLOTS][FS3_MAX_TILES] clean-increment sum per tile; [tiles] sum w_raw^2
+    unsigned* entCnt;                                          // [FS3_SLOTS] dirty values appended so far (any order)
+    unsigned* entKey; unsigned* entTile; unsigned long long* entP; double* entV; int* entL;   // [FS3_SLOTS][FS3_ENT_CAP]
+    unsigned* bar;                                             // [FS3_ROUNDS] grid-barrier arrival counters of the running launch
+    unsigned* resflag;                                         // [FS3_ROUNDS] "the chain of this round is evaluated" flags
+    Fs3Res* res;                                               // [FS3_ROUNDS] its results: total, entry count, failure
+    unsigned long long* resTP; unsigned* resKey; unsigned long long* resP; double* resAft;   // [FS3_ROUNDS][tiles] / [FS3_ROUNDS][FS3_ENT_CAP] for the scans
+    double* tileEnd;                                           // [FS3_MAX_TILES] last CDF value of every tile (coarse level of the index search)
+    int* flagsg;                                               // [FS3_SLOTS + 1] "bad value seen" per sum, then the certificate flag
+    unsigned long long* trace;                                 // optional [48] phase timestamps (PFGPU_POST_TRACE)
+    Fs3State* st;                                              // the launch's state (FastSLAM: Fs3Dev::st): serial_walks, cert_fail, dirty_last, err, post_done
+    // what a serial walk re-reads (fs3_value): raw[par] for FS3_S, wn for FS3_Q, FS3_S2 and FS3_CDF
+    const double* raw[2];                                      // [n] raw weights, by step parity
+    const double* wn;                                          // [n] normalised weights
+    unsigned n;                                                // values per sum
+};
+// x's arrays and Fs3State in ONE zeroed allocation (x.tileP is its base), and x.n; the caller sets raw, wn.  No peer touches it.
+inline cudaError_t fs3_sum_alloc(Fs3Sum& x, unsigned n, bool trace) {
+    const size_t nsl = (size_t)FS3_SLOTS * FS3_MAX_TILES, nen = (size_t)FS3_SLOTS * FS3_ENT_CAP, nre = (size_t)FS3_ROUNDS * FS3_ENT_CAP;
+    char* base = nullptr; size_t off = 0;
+    auto take = [&](auto*& p, size_t cnt) { p = base ? reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + off) : nullptr; off += (cnt * sizeof(*p) + 255) & ~(size_t)255; };
+    for (int pass = 0; pass < 2; ++pass) {                     // pass 0 sizes the allocation, pass 1 carves it
+        if (pass) { const cudaError_t e = cudaMalloc(&base, off); if (e != cudaSuccess) return e; off = 0; }
+        take(x.tileP, nsl); take(x.tileQ, FS3_MAX_TILES); take(x.entCnt, FS3_SLOTS);
+        take(x.entKey, nen); take(x.entTile, nen); take(x.entP, nen); take(x.entV, nen); take(x.entL, nen);
+        take(x.bar, FS3_ROUNDS); take(x.resflag, FS3_ROUNDS); take(x.res, FS3_ROUNDS); take(x.resTP, (size_t)FS3_ROUNDS * FS3_MAX_TILES);
+        take(x.resKey, nre); take(x.resP, nre); take(x.resAft, nre); take(x.tileEnd, FS3_MAX_TILES); take(x.flagsg, FS3_SLOTS + 1);
+        take(x.st, 1); x.trace = nullptr;
+        if (trace) take(x.trace, 48);
+    }
+    x.n = n;
+    return cudaMemset(base, 0, off);
+}
+inline void fs3_sum_free(Fs3Sum& x) { cudaFree(x.tileP); x.tileP = nullptr; }
 struct Fs3Dev {
     unsigned n, n_glob, off, m, ld;           // local / global particles, first global slot, landmarks, column stride
     int G, rank;
@@ -98,20 +142,11 @@ struct Fs3Dev {
     double* cum_all;                          // [n_glob] CDF of the resample: certified fl(P_j / S), or the exact one
     double* rcomb_all;                        // [n_glob] exact comb (only when n_glob is not a power of two)
     unsigned* idx;                            // [ld] global ancestor of local slot t at the last resample
-    unsigned long long* tileP; double* tileQ;                  // [FS3_SLOTS][FS3_MAX_TILES] clean-increment sum per tile; [tiles] sum w_raw^2
-    unsigned* entCnt;                                          // [FS3_SLOTS] dirty values appended so far (any order)
-    unsigned* entKey; unsigned* entTile; unsigned long long* entP; double* entV; int* entL;   // [FS3_SLOTS][FS3_ENT_CAP]
-    unsigned* bar;                                             // [8] grid-barrier arrival counters of the running post kernel
-    unsigned* resflag;                                         // [8] "the chain of this round is evaluated" flags
-    Fs3Res* res;                                               // [8] its results: total, entry count, failure
-    unsigned long long* resTP; unsigned* resKey; unsigned long long* resP; double* resAft;   // [8][tiles] / [8][FS3_ENT_CAP] for the scans
-    double* tileEnd;                                           // [FS3_MAX_TILES] last CDF value of every tile (coarse level of the index search)
-    unsigned* rowbm;                                           // [2][fs3_bm_ld(m)] by step parity: live-row bitmap ([ceil(m/32)] words),
-                                                               // then one "has an identity landmark" flag per post-kernel CTA
+    Fs3Sum x;                                 // the post kernel's exact sums (n_glob values; x.trace also times the EKF launch)
+    unsigned* rowbm;                          // [2][fs3_bm_ld(m)] by step parity: live-row bitmap ([ceil(m/32)] words),
+                                              // then one "has an identity landmark" flag per post-kernel CTA
     double* tileBw; unsigned* tileBi;         // [FS3_MAX_TILES] best (weight, global slot) per tile
-    int* flagsg;                              // [FS3_SLOTS + 1] "bad value seen" per sum, then the certificate flag (reset by the post kernel's last CTA)
     Fs3Rec* rec;
-    unsigned long long* trace;                // optional [32] phase timestamps (PFGPU_POST_TRACE)
 };
 
 __device__ __forceinline__ unsigned fs3_ref(int rank, unsigned col) { return ((unsigned)rank << 28) | col; }
@@ -217,10 +252,10 @@ fs3_ekf_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3ObsP
     const int cur = st->cur, rcur = st->rcur, par = (int)(step & 1u);
     const size_t ld = d.ld;
     const unsigned ngroups = d.ld / 64;
-    if (d.trace && blockIdx.x == 0 && threadIdx.x == 0 && (flags & 1)) {     // step timeline (PFGPU_POST_TRACE): [32] idle before this launch
+    if (d.x.trace && blockIdx.x == 0 && threadIdx.x == 0 && (flags & 1)) {     // step timeline (PFGPU_POST_TRACE): [32] idle before this launch
         unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        if (d.trace[36]) d.trace[32] += t - d.trace[36];
-        d.trace[38] = t; d.trace[37] = 0ull;
+        if (d.x.trace[36]) d.x.trace[32] += t - d.x.trace[36];
+        d.x.trace[38] = t; d.x.trace[37] = 0ull;
     }
     if (wj >= k_obs) {
         // ========== helper warp h: predict for trips h, h + nh, ... (ahead), weight products of the same trips (behind) ==========
@@ -306,7 +341,7 @@ fs3_ekf_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3ObsP
             if (!have) break;
             Wp = Wn; gprev = g; first = false; use++;
         }
-        if (d.trace && h == 0 && lane == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(d.trace + 37, t); }
+        if (d.x.trace && h == 0 && lane == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(d.x.trace + 37, t); }
         return;
     }
     // =============================== EKF warps: one observation each ===============================
@@ -405,7 +440,7 @@ fs3_ekf_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3ObsP
         if (g >= ngroups) break;
         stage = stage + 1 == nh ? 0 : stage + 1;
     }
-    if (d.trace && wj == 0 && lane == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(d.trace + 37, t); }
+    if (d.x.trace && wj == 0 && lane == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); atomicMax(d.x.trace + 37, t); }
 }
 
 // FastSLAM 2.0 (fs2.rs = crates/rust_robotics_slam/src/fastslam2.rs): the pose of every particle is sampled from the proposal that
@@ -493,21 +528,18 @@ struct Fs3Sh {
     x3_comb_table comb;
 };
 
-#define FS3_TRACE(k) do { if (d.trace && blockIdx.x == 0 && threadIdx.x == 0) { unsigned long long t__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t__)); d.trace[k] += t__ - t_prev; t_prev = t__; } } while (0)
+#define FS3_TRACE(k) do { if (x.trace && blockIdx.x == 0 && threadIdx.x == 0) { unsigned long long t__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t__)); x.trace[k] += t__ - t_prev; t_prev = t__; } } while (0)
 
 // grid barrier `round` of this launch: every CTA arrives once per round; the counters are zeroed by the launch's last CTA
-__device__ __forceinline__ void fs3_bar_arrive(const Fs3Dev& d, int round) {        // thread 0, after a block barrier
-    (void)atom_add_acq_rel_gpu(d.bar + round, 1u);
-}
-__device__ __forceinline__ void fs3_bar_wait(const Fs3Dev& d, int round, unsigned nblocks) {   // one thread
-    unsigned spins = 0;
-#pragma unroll 1
-    while (ld_acquire_gpu(d.bar + round) < nblocks) { if (++spins > FS3_SPIN_LIMIT) { d.st->err = 1; break; } __nanosleep(20); }
-}
 template <int NT>
-__device__ __forceinline__ void fs3_grid_sync(const Fs3Dev& d, int round, unsigned nblocks) {
+__device__ __forceinline__ void fs3_grid_sync(const Fs3Sum& x, int round, unsigned nblocks) {
     __syncthreads();
-    if (threadIdx.x == 0) { fs3_bar_arrive(d, round); fs3_bar_wait(d, round, nblocks); }
+    if (threadIdx.x == 0) {
+        (void)atom_add_acq_rel_gpu(x.bar + round, 1u);
+        unsigned spins = 0;
+#pragma unroll 1
+        while (ld_acquire_gpu(x.bar + round) < nblocks) { if (++spins > FS3_SPIN_LIMIT) { x.st->err = 1; break; } __nanosleep(20); }
+    }
     __syncthreads();
 }
 
@@ -565,12 +597,12 @@ __device__ __forceinline__ void fs3_block_sum2(double& x, double& y, double* smx
 
 __device__ __noinline__ double fs3_div(double a, double b) { return a / b; }      // one copy of the IEEE division sequence
 // value i of the sum `slot`, recomputed from global memory (serial walks only)
-__device__ __forceinline__ double fs3_value(const Fs3Dev& d, int slot, size_t i, int par, double S2, double r0, double inv) {
-    if (slot == 0) return __ldcg(d.wraw[par] + i);
-    const double w = slot == 4 ? 0.0 : __ldcg(d.wn_all + i);
-    if (slot == 1) return w * w;
-    if (slot == 2) return w;
-    if (slot == 3) return S2 > 0.0 ? fs3_div(w, S2) : w;
+__device__ __forceinline__ double fs3_value(const Fs3Sum& x, int slot, size_t i, int par, double S2, double r0, double inv) {
+    if (slot == FS3_S) return __ldcg(x.raw[par] + i);
+    const double w = slot == FS3_COMB ? 0.0 : __ldcg(x.wn + i);
+    if (slot == FS3_Q) return w * w;
+    if (slot == FS3_S2) return w;
+    if (slot == FS3_CDF) return S2 > 0.0 ? fs3_div(w, S2) : w;
     return i == 0 ? r0 : inv;
 }
 // exact by construction: one thread walks all values in order (bad values, too many dirty ones, failed certificate).
@@ -579,28 +611,28 @@ __device__ __forceinline__ double fs3_value(const Fs3Dev& d, int slot, size_t i,
 // non-decreasing r); on a non-decreasing CDF it is the CDF itself.
 __device__ __forceinline__ double fs3_runmax(double m, double c) { return (m != m || c <= m) ? m : c; }
 template <int NT, bool GT = false>
-__device__ __noinline__ void fs3_serial_walk(const Fs3Dev& d, Fs3Sh<NT>& sh, unsigned K, int slot, double* out, int par, double S2, double r0, double inv) {
+__device__ __noinline__ void fs3_serial_walk(const Fs3Sum& x, Fs3Sh<NT>& sh, unsigned K, int slot, double* out, int par, double S2, double r0, double inv) {
     if (threadIdx.x == 0) {
         const size_t T = (size_t)NT * K, lo = (size_t)blockIdx.x * T;
         double s = 0.0, mx = -INFINITY, mbase = -INFINITY;
         sh.tbase = 0.0;
 #pragma unroll 1
-        for (size_t i = 0; i < d.n_glob; ++i) {
+        for (size_t i = 0; i < x.n; ++i) {
             if (i == lo) { sh.tbase = s; mbase = mx; }
-            s = s + fs3_value(d, slot, i, par, S2, r0, inv);
-            if (slot == 3) mx = fs3_runmax(mx, s);
+            s = s + fs3_value(x, slot, i, par, S2, r0, inv);
+            if (slot == FS3_CDF) mx = fs3_runmax(mx, s);
         }
-        if (lo >= d.n_glob) sh.tbase = s;
+        if (lo >= x.n) sh.tbase = s;
         sh.total = s;
-        if (blockIdx.x == 0) d.st->serial_walks += 1;
+        if (blockIdx.x == 0) x.st->serial_walks += 1;
         if (out) {
             double c = sh.tbase, m = mbase;
 #pragma unroll 1
-            for (size_t i = lo; i < lo + T && i < d.n_glob; ++i) {
-                c = c + fs3_value(d, slot, i, par, S2, r0, inv);
-                if (slot == 3) { m = fs3_runmax(m, c); out[i] = m; } else out[i] = c;
+            for (size_t i = lo; i < lo + T && i < x.n; ++i) {
+                c = c + fs3_value(x, slot, i, par, S2, r0, inv);
+                if (slot == FS3_CDF) { m = fs3_runmax(m, c); out[i] = m; } else out[i] = c;
             }
-            if (slot == 3) d.tileEnd[blockIdx.x] = m;
+            if (slot == FS3_CDF) x.tileEnd[blockIdx.x] = m;
         }
     }
     __syncthreads();
@@ -610,9 +642,11 @@ __device__ __noinline__ int fs3_classify(double v, double a0, double a1, unsigne
     return x3_classify(v, a0, a1, m32, inc, lvl);            // one copy of the code for the three passes of fs3_xsum
 }
 // Work that hides inside an exact sum, on warps that would otherwise sleep at a block barrier while warp 0 waits for the grid
-// and evaluates the chain.  First sum of a launch: the lazy-clone bookkeeping of every CTA's landmark slice, the comb table and
-// the N(0,1) pairs of the next predict.
-struct Fs3Hook { unsigned long long comb_n; uint64_t seed; uint32_t noise_call; int k_last; const Fs3ObsParam* po; int par; };
+// and evaluates the chain.  First sum of fs3_post_kernel: the lazy-clone bookkeeping of every CTA's landmark slice, the comb table
+// and the N(0,1) pairs of the next predict (EKF call step + 1), on the Fs3Dev whose d.x the sum runs in, found by its address (a
+// pointer to it in the hook costs fs3_post_kernel<512, true> 32 bytes of spills and pf3_post_kernel four registers).
+struct Fs3Hook { unsigned long long comb_n; uint64_t seed; unsigned step; int k_last; const Fs3ObsParam* po; };
+static_assert(std::is_standard_layout<Fs3Dev>::value, "fs3_xsum's hook finds the Fs3Dev around d.x with offsetof");
 // what fs3_xsum_emit needs of a thread's pass through fs3_xsum: approximate prefix in front of its first value, clean-increment
 // sum in front of it inside the tile, and the binade of its run (-1: classified value by value)
 struct Fs3Run { double a_first; unsigned long long Pex; int e_run; };
@@ -731,22 +765,22 @@ __device__ __forceinline__ void fs3_row_fill(const Fs3Dev& d, Fs3Sh<NT>& sh, int
 // keeps this thread's state, so that fs3_xsum_emit can store the exact inclusive prefixes afterwards (sh.fail = 0; with
 // sh.fail = 1 the serial walk has already stored them to `out`).  Contains ONE grid barrier (`round`).
 template <int NT, bool GT = false>
-__device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
+__device__ __noinline__ double fs3_xsum(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
                                         unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run,
                                         const Fs3Hook* hook = nullptr) {
     const int tid = threadIdx.x, lane = tid & 31, pp = round & 1;
     const unsigned b = blockIdx.x;
     const size_t T = (size_t)NT * K;
     unsigned long long t_prev = 0;
-    const int tb0 = slot == 0 ? 8 : (slot == 3 ? 12 : 24);   // trace slots (PFGPU_POST_TRACE): S -> 8..11, CDF -> 12..15
-    if (d.trace && b == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_prev));
+    const int tb0 = slot == FS3_S ? 8 : (slot == FS3_CDF ? 12 : 24);   // trace slots (PFGPU_POST_TRACE): S -> 8..11, CDF -> 12..15
+    if (x.trace && b == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_prev));
     // ---- approximate prefixes, classification, tile aggregate ----
     double ts = 0.0; bool bad = false;
 #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) { const double v = vals[k * NT + tid]; ts += v; if (!(v >= 0.0) || !(v <= 1.7976931348623157e308)) bad = true; }
-    if (slot == 0) FS3_TRACE(28);
+    if (slot == FS3_S) FS3_TRACE(28);
     const double a_first = toff + fs3_scan_d<NT>(ts, sh.wd[pp]);
-    if (slot == 0) FS3_TRACE(29);
+    if (slot == FS3_S) FS3_TRACE(29);
     unsigned long long P = 0; int nd = 0;
     // Almost every thread's K prefixes stay inside one binade, clear of its edges: then each value is classified at that binade
     // without a running prefix (no loop-carried FP chain, a dozen integer instructions per value).  The same predicate, from the
@@ -768,11 +802,11 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             a = a1;
         }
     }
-    if (slot == 0) FS3_TRACE(30);
+    if (slot == FS3_S) FS3_TRACE(30);
     unsigned long long Pex, Ptile; int dex, ndtile;
     fs3_scan_ui<NT>(P, nd, &Pex, &dex, &Ptile, &ndtile, sh.wu[pp], sh.wi[pp]);
     if (nd > 0) {                                              // rare: itemise this thread's dirty values (any order; sorted by the chain)
-        const unsigned e0 = atomicAdd(d.entCnt + slot, (unsigned)nd);
+        const unsigned e0 = atomicAdd(x.entCnt + slot, (unsigned)nd);
         double a = a_first; unsigned long long Pr = Pex; unsigned e = e0;
     #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) {
@@ -781,22 +815,23 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             if (e_run >= 0 ? x3_classify_at(v, e_run, &inc) : fs3_classify(v, a, a1, m32, &inc, &lvl)) {
                 if (e < FS3_ENT_CAP) {
                     const size_t o = (size_t)slot * FS3_ENT_CAP + e;
-                    d.entKey[o] = (unsigned)((size_t)b * T + (size_t)tid * K + k); d.entTile[o] = b; d.entP[o] = Pr; d.entV[o] = v; d.entL[o] = lvl;
+                    x.entKey[o] = (unsigned)((size_t)b * T + (size_t)tid * K + k); x.entTile[o] = b; x.entP[o] = Pr; x.entV[o] = v; x.entL[o] = lvl;
                 }
                 e++;
             } else Pr += inc;
             a = a1;
         }
     }
-    if (bad) d.flagsg[slot] = 1;
-    if (tid == 0) { d.tileP[(size_t)slot * FS3_MAX_TILES + b] = Ptile; if (slot == 0) d.tileQ[b] = extraQ; }
+    if (bad) x.flagsg[slot] = 1;
+    if (tid == 0) { x.tileP[(size_t)slot * FS3_MAX_TILES + b] = Ptile; if (slot == FS3_S) x.tileQ[b] = extraQ; }
     FS3_TRACE(tb0);
     __syncthreads();
     // ---- grid barrier + chain.  The LAST CTA to arrive evaluates the chain (every aggregate is published by then and it reads
     // them uncontended: 128 CTAs fetching the same few sectors at once serialise in L2) and publishes the results; the others
     // wait for its flag.  Warp 0 only; the other warps wait at the block barrier below. ----
     if (hook && tid >= 32) {
-        fs3_row_scan<NT>(d, *hook->po, hook->k_last, hook->par, b, nt);
+        const Fs3Dev& d = *reinterpret_cast<const Fs3Dev*>(reinterpret_cast<const char*>(&x) - offsetof(Fs3Dev, x));
+        fs3_row_scan<NT>(d, *hook->po, hook->k_last, (int)(hook->step & 1u), b, nt);
         if (tid < 64) {                            // warp 1
             if (hook->comb_n && lane == 0) x3_comb_build(&sh.comb, r0, inv, (double)hook->comb_n, hook->comb_n);
         } else {                                   // warps 2..: the N(0,1) pairs of the next predict for this CTA's share of the local slots
@@ -804,16 +839,16 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
 #pragma unroll 1
             for (unsigned t = t_lo + (unsigned)(tid - 64); t < t_hi; t += (unsigned)(NT - 64)) {
                 double z0, z1;
-                fs3_normal_pair(hook->seed, hook->noise_call, (uint64_t)d.off + t, &z0, &z1);
+                fs3_normal_pair(hook->seed, hook->step + 1u, (uint64_t)d.off + t, &z0, &z1);
                 d.nz[0][t] = z0; d.nz[1][t] = z1;
             }
         }
     }
     if (tid < 32) {
         int leader = 0;
-        if (tid == 0) leader = (atom_add_acq_rel_gpu(d.bar + round, 1u) + 1u == nt) ? 1 : 0;
+        if (tid == 0) leader = (atom_add_acq_rel_gpu(x.bar + round, 1u) + 1u == nt) ? 1 : 0;
         leader = __shfl_sync(0xffffffffu, leader, 0);
-        Fs3Res* res = d.res + round;
+        Fs3Res* res = x.res + round;
         const size_t rb = (size_t)round * FS3_ENT_CAP, rt = (size_t)round * FS3_MAX_TILES;
         if (leader) {
             FS3_TRACE(tb0 + 1);
@@ -822,18 +857,18 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             const size_t eb = (size_t)slot * FS3_ENT_CAP;
             unsigned long long tp[(FS3_MAX_TILES + 31) / 32];
 #pragma unroll
-            for (unsigned i = 0; i < (FS3_MAX_TILES + 31) / 32; ++i) tp[i] = (i * 32u + lane) < nt ? __ldcg(d.tileP + (size_t)slot * FS3_MAX_TILES + i * 32u + lane) : 0ull;
-            const unsigned cnt = __ldcg(d.entCnt + slot);
-            int fail = __ldcg(d.flagsg + slot);
-            unsigned ekey = __ldcg(d.entKey + eb + lane), etile = __ldcg(d.entTile + eb + lane);
-            unsigned long long eP = __ldcg(d.entP + eb + lane);
-            double eV = __ldcg(d.entV + eb + lane);
-            int eL = __ldcg(d.entL + eb + lane);
+            for (unsigned i = 0; i < (FS3_MAX_TILES + 31) / 32; ++i) tp[i] = (i * 32u + lane) < nt ? __ldcg(x.tileP + (size_t)slot * FS3_MAX_TILES + i * 32u + lane) : 0ull;
+            const unsigned cnt = __ldcg(x.entCnt + slot);
+            int fail = __ldcg(x.flagsg + slot);
+            unsigned ekey = __ldcg(x.entKey + eb + lane), etile = __ldcg(x.entTile + eb + lane);
+            unsigned long long eP = __ldcg(x.entP + eb + lane);
+            double eV = __ldcg(x.entV + eb + lane);
+            int eL = __ldcg(x.entL + eb + lane);
             fail |= cnt > FS3_ENT_CAP ? 1 : 0;
 #pragma unroll
             for (unsigned i = 0; i < (FS3_MAX_TILES + 31) / 32; ++i) if (i * 32u + lane < nt) sh.tPoff[i * 32u + lane] = tp[i];
             __syncwarp();
-            if (slot == 0) FS3_TRACE(16);
+            if (slot == FS3_S) FS3_TRACE(16);
             // clean-increment sum in front of every tile: lane owns `per` consecutive tiles
             const unsigned per = (nt + 31u) / 32u, t0 = (unsigned)lane * per;
             unsigned long long lsum = 0;
@@ -845,9 +880,9 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             const unsigned long long Ptot = __shfl_sync(0xffffffffu, inc, 31);
             unsigned long long run = inc - lsum;
 #pragma unroll 1
-            for (unsigned i = 0; i < per; ++i) if (t0 + i < nt) { const unsigned long long x = sh.tPoff[t0 + i]; sh.tPoff[t0 + i] = run; run += x; }
+            for (unsigned i = 0; i < per; ++i) if (t0 + i < nt) { const unsigned long long tp = sh.tPoff[t0 + i]; sh.tPoff[t0 + i] = run; run += tp; }
             __syncwarp();
-            if (slot == 0) FS3_TRACE(17);
+            if (slot == FS3_S) FS3_TRACE(17);
             const int D = fail ? 0 : (int)cnt;
             double total = 0.0;
             if (D <= 32) {
@@ -862,7 +897,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
                 // move every entry to the lane of its rank (through shared memory: one conflict-free round)
                 if (have) { sh.skey[rank] = ekey; sh.sP[rank] = Pg; sh.sV[rank] = eV; sh.sL[rank] = eL; }
                 __syncwarp();
-                if (slot == 0) FS3_TRACE(18);
+                if (slot == FS3_S) FS3_TRACE(18);
                 // the serial part, lane 0 over the sorted entries in shared memory: one integer add on the bit pattern + one FP add
                 // per dirty value; the loads do not depend on the chain, so the compiler hoists them ahead (unroll 4)
                 int ok = 1;
@@ -885,7 +920,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
                 if (!ok) fail = 1;
             } else {
 #pragma unroll 1
-                for (int e = lane; e < D; e += 32) sh.ukey[e] = __ldcg(d.entKey + eb + e);
+                for (int e = lane; e < D; e += 32) sh.ukey[e] = __ldcg(x.entKey + eb + e);
                 __syncwarp();
 #pragma unroll 1
                 for (int e = lane; e < D; e += 32) {               // rank = position in index order (keys are distinct)
@@ -893,8 +928,8 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
                     int rank = 0;
 #pragma unroll 1
                     for (int j = 0; j < D; ++j) rank += sh.ukey[j] < key ? 1 : 0;
-                    sh.skey[rank] = key; sh.sP[rank] = sh.tPoff[__ldcg(d.entTile + eb + e)] + __ldcg(d.entP + eb + e);
-                    sh.sV[rank] = __ldcg(d.entV + eb + e); sh.sL[rank] = __ldcg(d.entL + eb + e);
+                    sh.skey[rank] = key; sh.sP[rank] = sh.tPoff[__ldcg(x.entTile + eb + e)] + __ldcg(x.entP + eb + e);
+                    sh.sV[rank] = __ldcg(x.entV + eb + e); sh.sL[rank] = __ldcg(x.entL + eb + e);
                 }
                 __syncwarp();
                 if (lane == 0) {                                   // the serial part: one integer add + one FP add per dirty value
@@ -922,26 +957,26 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
             __syncwarp();
             fail = __any_sync(0xffffffffu, fail);
             total = __shfl_sync(0xffffffffu, total, 0);
-            if (slot == 0) FS3_TRACE(19);
+            if (slot == FS3_S) FS3_TRACE(19);
             // publish: what the other CTAs need to finish on their own
             if (pub && !fail) {
 #pragma unroll 1
-                for (unsigned t = lane; t < nt; t += 32) d.resTP[rt + t] = sh.tPoff[t];
+                for (unsigned t = lane; t < nt; t += 32) x.resTP[rt + t] = sh.tPoff[t];
 #pragma unroll 1
-                for (int o = lane; o < D; o += 32) { d.resKey[rb + o] = sh.skey[o]; d.resP[rb + o] = sh.sP[o]; d.resAft[rb + o] = sh.aft[o]; }
+                for (int o = lane; o < D; o += 32) { x.resKey[rb + o] = sh.skey[o]; x.resP[rb + o] = sh.sP[o]; x.resAft[rb + o] = sh.aft[o]; }
             }
             if (lane == 0) {
                 res->total = total; res->Ptot = Ptot; res->D = D; res->fail = fail;
                 sh.total = total; sh.Ptot = Ptot; sh.D = D; sh.fail = fail; sh.lead = 1;
-                d.st->dirty_last = (int)cnt;
+                x.st->dirty_last = (int)cnt;
             }
             __syncwarp();                                          // the other lanes' stores above are ordered before lane 0's release
-            if (lane == 0) st_release_gpu(d.resflag + round, 1u);
-            if (slot == 0) { FS3_TRACE(20); if (d.trace && b == 0 && tid == 0) d.trace[21] += 1; }
+            if (lane == 0) st_release_gpu(x.resflag + round, 1u);
+            if (slot == FS3_S) { FS3_TRACE(20); if (x.trace && b == 0 && tid == 0) x.trace[21] += 1; }
         } else {
             if (lane == 0) {
                 unsigned spins = 0;
-                while (ld_acquire_gpu(d.resflag + round) == 0u) { if (++spins > FS3_SPIN_LIMIT) { d.st->err = 1; break; } __nanosleep(20); }
+                while (ld_acquire_gpu(x.resflag + round) == 0u) { if (++spins > FS3_SPIN_LIMIT) { x.st->err = 1; break; } __nanosleep(20); }
             }
             __syncwarp();
             FS3_TRACE(tb0 + 1);
@@ -952,7 +987,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
     }
     __syncthreads();
     FS3_TRACE(tb0 + 2);
-    if (sh.fail) { fs3_serial_walk<NT, GT>(d, sh, K, slot, out, par, S2, r0, inv); return sh.total; }
+    if (sh.fail) { fs3_serial_walk<NT, GT>(x, sh, K, slot, out, par, S2, r0, inv); return sh.total; }
     if (run) { run->a_first = a_first; run->Pex = Pex; run->e_run = e_run; }
     return sh.total;
 }
@@ -963,19 +998,19 @@ __device__ __noinline__ double fs3_xsum(const Fs3Dev& d, Fs3Sh<NT>& sh, const do
 // (x3_cdf_near_comb), or a clean run failed its certificate.  tend: the tile's last stored value goes to tileEnd[tile].
 // vals must still hold the values the sum saw.  Contains one block barrier.
 template <int NT, bool GT = false>
-__device__ __noinline__ int fs3_xsum_emit(const Fs3Dev& d, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
+__device__ __noinline__ int fs3_xsum_emit(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
                                           double* out, int tend, const Fs3Cert* cert, int tslot) {
     const int tid = threadIdx.x, lane = tid & 31;
     const unsigned b = blockIdx.x;
     const size_t T = (size_t)NT * K;
     unsigned long long t_prev = 0;
-    if (d.trace && b == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_prev));
+    if (x.trace && b == 0 && tid == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_prev));
     if (sh.fail) return 0;
     if (tid < 32 && !sh.lead) {                               // the sorted dirty entries + my tile's increment prefix, as the leader published them
         const size_t rb = (size_t)round * FS3_ENT_CAP, rt = (size_t)round * FS3_MAX_TILES;
-        if (lane == 0) sh.tPoff[b] = __ldcg(d.resTP + rt + b);
+        if (lane == 0) sh.tPoff[b] = __ldcg(x.resTP + rt + b);
 #pragma unroll 1
-        for (int o = lane; o < sh.D; o += 32) { sh.skey[o] = __ldcg(d.resKey + rb + o); sh.sP[o] = __ldcg(d.resP + rb + o); sh.aft[o] = __ldcg(d.resAft + rb + o); }
+        for (int o = lane; o < sh.D; o += 32) { sh.skey[o] = __ldcg(x.resKey + rb + o); sh.sP[o] = __ldcg(x.resP + rb + o); sh.aft[o] = __ldcg(x.resAft + rb + o); }
     }
     __syncthreads();
     const int D = sh.D, e_run = run->e_run;
@@ -997,7 +1032,7 @@ __device__ __noinline__ int fs3_xsum_emit(const Fs3Dev& d, Fs3Sh<NT>& sh, const 
             unsigned long long inc;
             if (x3_classify_at(vals[k * NT + tid], e_run, &inc)) { base = sh.aft[ko]; Pb = sh.sP[ko]; ko++; c = base; }
             else { Pc += inc; c = x3_apply(base, Pc - Pb, inc ? e_run : -1, &ok); }
-            if (g0 + k < d.n_glob) out[g0 + k] = c;
+            if (g0 + k < x.n) out[g0 + k] = c;
         }
         o = c;
     } else {
@@ -1010,14 +1045,14 @@ __device__ __noinline__ int fs3_xsum_emit(const Fs3Dev& d, Fs3Sh<NT>& sh, const 
             o = c;
             if (cert) {
                 o = fs3_div(c, cert->S);
-                if (g0 + k < d.n_glob) near |= x3_cdf_near_comb(o, cert->r0, cert->inv, cert->ninv, cert->n, cert->dl, cert->ab);
+                if (g0 + k < x.n) near |= x3_cdf_near_comb(o, cert->r0, cert->inv, cert->ninv, cert->n, cert->dl, cert->ab);
             }
-            if (g0 + k < d.n_glob) out[g0 + k] = o;
+            if (g0 + k < x.n) out[g0 + k] = o;
             a = a1;
         }
     }
-    if (tend && tid == NT - 1) d.tileEnd[b] = o;              // coarse level of the index search
-    if (!ok) { atomicAdd(&d.st->cert_fail, 1); near = 1; }
+    if (tend && tid == NT - 1) x.tileEnd[b] = o;              // coarse level of the index search
+    if (!ok) { atomicAdd(&x.st->cert_fail, 1); near = 1; }
     if (tslot >= 0) FS3_TRACE(tslot);
     return near;
 }
@@ -1064,17 +1099,18 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     { extern __shared__ __align__(16) double vals[]; vt = GTILE ? vtile + (size_t)blockIdx.x * NT * K : vals; }
     double* const vals = vt;                                  // [K][NT]
     __shared__ Fs3Sh<NT> sh;
+    const Fs3Sum& x = d.x;
     Fs3State* st = d.st;
     const int tid = threadIdx.x;
     const unsigned b = blockIdx.x, nt = gridDim.x;
     const size_t T = (size_t)NT * K, ng = d.n_glob;
     const int par = (int)(step & 1u);
     unsigned long long t_prev = 0;
-    if (d.trace && b == 0 && tid == 0) {
+    if (x.trace && b == 0 && tid == 0) {
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_prev));
-        const unsigned long long e1 = d.trace[37], e0 = d.trace[38];           // step timeline: [33] EKF launch (first CTA in .. last warp out),
-        if (e1 && e0) { d.trace[33] += e1 - e0; d.trace[34] += t_prev - e1; }   // [34] idle between the EKF launch and this one
-        d.trace[39] = t_prev;
+        const unsigned long long e1 = x.trace[37], e0 = x.trace[38];           // step timeline: [33] EKF launch (first CTA in .. last warp out),
+        if (e1 && e0) { x.trace[33] += e1 - e0; x.trace[34] += t_prev - e1; }   // [34] idle between the EKF launch and this one
+        x.trace[39] = t_prev;
     }
     if (d.G > 1) {      // my EKF launch is complete: its pushes are in every peer's copy.  Say so, then wait for the others'.
         if (b == 0) fs3_signal_peers(d, 0, step + 1u);
@@ -1105,17 +1141,16 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     // a resample may then use the certified CDF fl(P_j / S) instead of the S2 and CDF sums (see below)
     const int cert_pub = log2n >= 0 && log2n <= FS3_CERT_MAX_LOG2N && !d.exact_cdf;
     Fs3Hook hook;
-    hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.noise_call = step + 1u; hook.k_last = k_last; hook.po = &po;
-    hook.par = par;
+    hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.step = step; hook.k_last = k_last; hook.po = &po;
     Fs3Run run;
-    const double S = fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff, 0, 0, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
+    const double S = fs3_xsum<NT, GTILE>(x, sh, vals, K, nt, toff, FS3_S, FS3_R_S, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
     const int S_walked = sh.fail;
     FS3_TRACE(1);
     // ---------------- gate: neff = 1 / sum w^2 < NTH (compute_neff fs1.rs:186-193, fs1.rs:262-263) ----------------
     // Only the DECISION feeds back into the state.  Q is first taken from the tree-order sums of w_raw^2 published with the
     // aggregates of S: sum (w_raw_i / S)^2 differs from the reference's sequential sum of fl(w_raw_i / S)^2 by at most
     // (n + 64) 2^-51 relatively; only when neff lands that close to NTH is the exact sequential sum walked (below, once wn_all is written).
-    double Q = (unsigned)tid < nt ? __ldcg(d.tileQ + tid) : 0.0, dummy = 0.0;
+    double Q = (unsigned)tid < nt ? __ldcg(x.tileQ + tid) : 0.0, dummy = 0.0;
     fs3_block_sum2<NT>(Q, dummy, sh.red[1], sh.wd[1]);
     if (S > 0.0) Q = fs3_div(fs3_div(Q, S), S);
     double neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
@@ -1137,8 +1172,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         cp.S = S; cp.r0 = r0; cp.inv = inv; cp.ninv = (double)ng; cp.n = ng;
         cp.dl = g / (1.0 - g) * (1.0 + 9.5367431640625e-07);             // gamma_4n (1 + 2^-20)
         cp.ab = (4.0 * (double)ng + 4.0) * 4.9406564584124654e-324 + (double)(log2n + 4) * 1.1102230246251565e-16;
-        const int near = fs3_xsum_emit<NT, GTILE>(d, sh, vals, K, m32, &run, 0, d.cum_all, 1, &cp, -1);
-        if (__syncthreads_or(near) && tid == 0) d.flagsg[FS3_CERT_FLAG] = 1;
+        const int near = fs3_xsum_emit<NT, GTILE>(x, sh, vals, K, m32, &run, FS3_R_S, d.cum_all, 1, &cp, -1);
+        if (__syncthreads_or(near) && tid == 0) x.flagsg[FS3_CERT_FLAG] = 1;
         FS3_TRACE(4);
     }
     // w = w_raw / S; best particle of the tile (LAST maximum, fs1.rs:269-274; from -inf, so weights below -1 take part too)
@@ -1168,7 +1203,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         d.tileBw[b] = bw; d.tileBi[b] = bi;
     }
     if (border) {                                              // rare
-        fs3_grid_sync<NT>(d, 6, nt);                           // wn_all is complete
+        fs3_grid_sync<NT>(x, FS3_R_BORDER, nt);                // wn_all is complete
         if (tid == 0) {
             double s = 0.0;
             if constexpr (GTILE) {       // millions of values: sixteen loads in flight per trip, the adds in the same order
@@ -1205,15 +1240,15 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         const int s_first = lm_lo + tid < lm_hi ? d.lmst[lm_lo + tid] : 0;
         bool exact = !cert;
         if (cert) {
-            fs3_grid_sync<NT>(d, 4, nt);                       // every c~_j and every CTA's verdict are visible
-            exact = __ldcg(d.flagsg + FS3_CERT_FLAG) != 0;
+            fs3_grid_sync<NT>(x, FS3_R_CERT, nt);              // every c~_j and every CTA's verdict are visible
+            exact = __ldcg(x.flagsg + FS3_CERT_FLAG) != 0;
             FS3_TRACE(5);
         }
         if (exact) {
             if (b == 0 && tid == 0) st->cdf_exact += 1;
             // ---------------- resample() re-normalises first (fs1.rs:207) ----------------
             const double toff2 = S > 0.0 ? fs3_div(toff, S) : toff;
-            S2 = fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff2, 2, 1, m32, nullptr, par, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
+            S2 = fs3_xsum<NT, GTILE>(x, sh, vals, K, nt, toff2, FS3_S2, FS3_R_S2, m32, nullptr, par, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
             FS3_TRACE(3);
             if (S2 > 0.0) {
 #pragma unroll 1
@@ -1221,8 +1256,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             }
             // ---------------- cum_sum fs1.rs:213-216 ----------------
             const double toff3 = S2 > 0.0 ? fs3_div(toff2, S2) : toff2;
-            (void)fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff3, 3, 2, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, 1, &run);
-            (void)fs3_xsum_emit<NT, GTILE>(d, sh, vals, K, m32, &run, 2, d.cum_all, 1, nullptr, 15);
+            (void)fs3_xsum<NT, GTILE>(x, sh, vals, K, nt, toff3, FS3_CDF, FS3_R_CDF, m32, d.cum_all, par, S2, 0.0, 0.0, 0.0, 1, &run);
+            (void)fs3_xsum_emit<NT, GTILE>(x, sh, vals, K, m32, &run, FS3_R_CDF, d.cum_all, 1, nullptr, 15);
             FS3_TRACE(4);
             // ---------------- the comb r, r + 1/n, ... accumulated sequentially (fs1.rs:219-230) ----------------
             if (log2n < 0) {                                   // n not a power of two: every add rounds -> exact scan
@@ -1230,10 +1265,10 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
                 for (unsigned k = 0; k < K; ++k) { const size_t i = g0 + k; vals[k * NT + tid] = i < ng ? (i == 0 ? r0 : inv) : 0.0; }
                 const double toff4 = b == 0 ? 0.0 : r0 + ((double)((size_t)b * T) - 1.0) * inv;
                 __syncthreads();
-                (void)fs3_xsum<NT, GTILE>(d, sh, vals, K, nt, toff4, 4, 3, m32, d.rcomb_all, par, S2, r0, inv, 0.0, 1, &run);
-                (void)fs3_xsum_emit<NT, GTILE>(d, sh, vals, K, m32, &run, 3, d.rcomb_all, 0, nullptr, -1);
+                (void)fs3_xsum<NT, GTILE>(x, sh, vals, K, nt, toff4, FS3_COMB, FS3_R_COMB, m32, d.rcomb_all, par, S2, r0, inv, 0.0, 1, &run);
+                (void)fs3_xsum_emit<NT, GTILE>(x, sh, vals, K, m32, &run, FS3_R_COMB, d.rcomb_all, 0, nullptr, -1);
             }
-            fs3_grid_sync<NT>(d, cert ? 5 : 4, nt);            // the whole CDF (and comb) is visible
+            fs3_grid_sync<NT>(x, FS3_R_CDF_DONE, nt);          // the whole CDF (and comb) is visible
             FS3_TRACE(5);
         }
         // ---------------- index walk, pose clone, lazy map clone for this CTA's share of the local slots ----------------
@@ -1246,7 +1281,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         const unsigned t_lo = b * per, t_hi = min(d.n, t_lo + per);
         const double* cdf = d.cum_all;
 #pragma unroll 1
-        for (unsigned t = tid; t < nt; t += NT) sh.tend[t] = __ldcg(d.tileEnd + t);
+        for (unsigned t = tid; t < nt; t += NT) sh.tend[t] = __ldcg(x.tileEnd + t);
         // the live rows: every CTA's fs3_row_scan (inside the S sum) is ordered before the grid barrier this CTA has just passed
         unsigned rpos; int nrows, newrow;
         fs3_row_count<NT>(d, sh, par, nt, &rpos, &nrows, &newrow);            // (also orders the tileEnd copy)
@@ -1372,15 +1407,15 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     if (tid == 0) sh.last = (atom_add_acq_rel_gpu(&st->post_done, 1u) + 1u == nt) ? 1 : 0;   // release my CTA's writes / acquire everybody's
     __syncthreads();
     if (!sh.last) return;
-    if (d.trace && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); d.trace[40] += t - d.trace[39]; }   // [40] the last CTA is through
-    if (tid < FS3_SLOTS) d.entCnt[tid] = 0u;
-    if (tid <= FS3_CERT_FLAG) d.flagsg[tid] = 0;
-    if (tid < 8) { d.bar[tid] = 0u; d.resflag[tid] = 0u; }
+    if (x.trace && tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); x.trace[40] += t - x.trace[39]; }   // [40] the last CTA is through
+    if (tid < FS3_SLOTS) x.entCnt[tid] = 0u;
+    if (tid <= FS3_CERT_FLAG) x.flagsg[tid] = 0;
+    if (tid < FS3_ROUNDS) { x.bar[tid] = 0u; x.resflag[tid] = 0u; }
     if (tid < 32) {
         // best particle: the last maximum over the tiles (no resample) / the last slot (after a resample every weight is 1/n)
         double bw2 = -INFINITY; unsigned bi2 = 0;
 #pragma unroll 1
-        for (unsigned x = tid; x < nt; x += 32) { const double ow = __ldcg(d.tileBw + x); const unsigned oi = __ldcg(d.tileBi + x); if (ow > bw2 || (ow == bw2 && oi > bi2)) { bw2 = ow; bi2 = oi; } }
+        for (unsigned u = tid; u < nt; u += 32) { const double ow = __ldcg(d.tileBw + u); const unsigned oi = __ldcg(d.tileBi + u); if (ow > bw2 || (ow == bw2 && oi > bi2)) { bw2 = ow; bi2 = oi; } }
 #pragma unroll 1
         for (int o = 16; o > 0; o >>= 1) {
             const double ow = __shfl_xor_sync(0xffffffffu, bw2, o); const unsigned oi = __shfl_xor_sync(0xffffffffu, bi2, o);
@@ -1409,7 +1444,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             if (gate) { st->cur ^= 1; st->rcur ^= 1; st->resamples += 1; }
             st->noise_call = NT >= 128 ? step + 2u : 0u;           // nz[] = noise of EKF call step + 1
             st->post_done = 0;
-            if (d.trace) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); d.trace[35] += t - d.trace[39]; d.trace[36] = t; }   // [35] this launch
+            if (x.trace) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); x.trace[35] += t - x.trace[39]; x.trace[36] = t; }   // [35] this launch
             // (no system fence in front of `seq`: the host reads the record only after it has synchronised with the stream, and a
             //  fence here waits for the PCIe writes above to land — inside every step's critical path)
             *reinterpret_cast<volatile unsigned long long*>(&rec->seq) = (unsigned long long)step + 1ull;

@@ -208,9 +208,7 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         d.peer[rank] = A; h->peer_ptr[rank] = A;
     }
     {
-        Fs3State* stp = nullptr;
-        FS_TRY(cudaMalloc(&stp, sizeof(Fs3State))); FS_TRY(cudaMemset(stp, 0, sizeof(Fs3State)));
-        d.st = stp;
+        FS_TRY(fs3_sum_alloc(d.x, (unsigned)n_global, getenv("PFGPU_POST_TRACE") != nullptr));
         FS_TRY(cudaMalloc(&d.lmst, mm * sizeof(int))); FS_TRY(cudaMemset(d.lmst, 0, mm * sizeof(int)));
         FS_TRY(cudaMalloc(&d.w, ld * sizeof(double))); FS_TRY(cudaMemset(d.w, 0, ld * sizeof(double)));
         for (int b = 0; b < 2; ++b) { FS_TRY(cudaMalloc(&d.nz[b], ld * sizeof(double))); FS_TRY(cudaMemset(d.nz[b], 0, ld * sizeof(double))); }
@@ -218,29 +216,14 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
         FS_TRY(cudaMalloc(&d.cum_all, (n_global + 64) * sizeof(double)));
         if (h->log2n < 0) FS_TRY(cudaMalloc(&d.rcomb_all, (n_global + 64) * sizeof(double)));
         FS_TRY(cudaMalloc(&d.idx, ld * sizeof(unsigned))); FS_TRY(cudaMemset(d.idx, 0, ld * sizeof(unsigned)));
-        const size_t nsl = (size_t)FS3_SLOTS * FS3_MAX_TILES, nen = (size_t)FS3_SLOTS * FS3_ENT_CAP;
-        FS_TRY(cudaMalloc(&d.tileP, nsl * sizeof(unsigned long long)));
-        FS_TRY(cudaMalloc(&d.tileQ, FS3_MAX_TILES * sizeof(double)));
-        FS_TRY(cudaMalloc(&d.entCnt, 8 * sizeof(unsigned))); FS_TRY(cudaMemset(d.entCnt, 0, 8 * sizeof(unsigned)));
-        FS_TRY(cudaMalloc(&d.entKey, nen * sizeof(unsigned))); FS_TRY(cudaMalloc(&d.entTile, nen * sizeof(unsigned)));
-        FS_TRY(cudaMalloc(&d.entP, nen * sizeof(unsigned long long))); FS_TRY(cudaMalloc(&d.entV, nen * sizeof(double)));
-        FS_TRY(cudaMalloc(&d.entL, nen * sizeof(int)));
-        FS_TRY(cudaMalloc(&d.bar, 8 * sizeof(unsigned))); FS_TRY(cudaMemset(d.bar, 0, 8 * sizeof(unsigned)));
-        FS_TRY(cudaMalloc(&d.resflag, 8 * sizeof(unsigned))); FS_TRY(cudaMemset(d.resflag, 0, 8 * sizeof(unsigned)));
-        FS_TRY(cudaMalloc(&d.res, 8 * sizeof(Fs3Res))); FS_TRY(cudaMemset(d.res, 0, 8 * sizeof(Fs3Res)));
-        FS_TRY(cudaMalloc(&d.resTP, (size_t)8 * FS3_MAX_TILES * sizeof(unsigned long long)));
-        FS_TRY(cudaMalloc(&d.resKey, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned))); FS_TRY(cudaMalloc(&d.resP, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned long long)));
-        FS_TRY(cudaMalloc(&d.resAft, (size_t)8 * FS3_ENT_CAP * sizeof(double)));
-        FS_TRY(cudaMalloc(&d.tileEnd, FS3_MAX_TILES * sizeof(double)));
+        d.st = d.x.st; d.x.raw[0] = d.wraw[0]; d.x.raw[1] = d.wraw[1]; d.x.wn = d.wn_all;
         const size_t nbm = (size_t)2 * fs3_bm_ld((unsigned)m);       // both parities start clear; each post kernel clears the other
         FS_TRY(cudaMalloc(&d.rowbm, nbm * sizeof(unsigned))); FS_TRY(cudaMemset(d.rowbm, 0, nbm * sizeof(unsigned)));
         FS_TRY(cudaMalloc(&d.tileBw, FS3_MAX_TILES * sizeof(double))); FS_TRY(cudaMalloc(&d.tileBi, FS3_MAX_TILES * sizeof(unsigned)));
-        FS_TRY(cudaMalloc(&d.flagsg, 8 * sizeof(int))); FS_TRY(cudaMemset(d.flagsg, 0, 8 * sizeof(int)));
         FS_TRY(cudaHostAlloc(&h->h_rec, sizeof(Fs3Rec), cudaHostAllocMapped));
         memset(h->h_rec, 0, sizeof(Fs3Rec));
         FS_TRY(cudaHostGetDevicePointer((void**)&d.rec, h->h_rec, 0));
         if (h->post_global) FS_TRY(cudaMalloc(&h->vtile, (size_t)h->post_tiles * h->post_K * 512 * sizeof(double)));
-        if (getenv("PFGPU_POST_TRACE")) { FS_TRY(cudaMalloc(&d.trace, 48 * sizeof(unsigned long long))); FS_TRY(cudaMemset(d.trace, 0, 48 * sizeof(unsigned long long))); }
     }
     { const char* e5 = getenv("PFGPU_PDL"); h->pdl = !(e5 && e5[0] == '0'); }
     { const char* e7 = getenv("PFGPU_EARLY_LAUNCH"); if (e7 && atoi(e7) == 1) h->early = true; }
@@ -313,11 +296,9 @@ extern "C" void pfgpu_fs_destroy(pfgpu_fs* h) {
     fs_unmap(h, h->hist_peer);
     fs_unmap(h, h->ex_peer);
     cudaFree(h->arena);
-    cudaFree(d.st); cudaFree(d.lmst); cudaFree(d.w); cudaFree(d.nz[0]); cudaFree(d.nz[1]); cudaFree(d.wn_all); cudaFree(d.cum_all); cudaFree(d.rcomb_all); cudaFree(d.idx);
-    cudaFree(d.tileP); cudaFree(d.tileQ); cudaFree(d.entCnt); cudaFree(d.entKey); cudaFree(d.entTile); cudaFree(d.entP); cudaFree(d.entV); cudaFree(d.entL);
-    cudaFree(d.bar); cudaFree(d.rowbm); cudaFree(d.resflag); cudaFree(d.res); cudaFree(d.resTP); cudaFree(d.resKey);
-    cudaFree(d.resP); cudaFree(d.resAft); cudaFree(d.tileEnd);
-    cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(d.flagsg); cudaFree(d.trace); cudaFree(h->vtile); cudaFree(h->stage); cudaFree(h->est);
+    cudaFree(d.lmst); cudaFree(d.w); cudaFree(d.nz[0]); cudaFree(d.nz[1]); cudaFree(d.wn_all); cudaFree(d.cum_all); cudaFree(d.rcomb_all); cudaFree(d.idx);
+    fs3_sum_free(d.x);
+    cudaFree(d.rowbm); cudaFree(d.tileBw); cudaFree(d.tileBi); cudaFree(h->vtile); cudaFree(h->stage); cudaFree(h->est);
     cudaFree(h->zbuf); cudaFree(h->acnt);
     cudaFree(h->hist); cudaFree(h->hs); cudaFree(h->ex);
     if (h->h_rec) cudaFreeHost(h->h_rec);
@@ -778,7 +759,7 @@ extern "C" int pfgpu_fs_post_trace(pfgpu_fs* h, unsigned long long* out32) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     for (int k = 0; k < 32; ++k) out32[k] = 0;
-    if (h->d.trace) PF_CUDA(cudaMemcpy(out32, h->d.trace, 32 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    if (h->d.x.trace) PF_CUDA(cudaMemcpy(out32, h->d.x.trace, 32 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     out32[31] = h->steps;
     {                     // [11] resamples that ran the exact S2 and CDF sums instead of the certified CDF
         Fs3State st;
@@ -787,9 +768,9 @@ extern "C" int pfgpu_fs_post_trace(pfgpu_fs* h, unsigned long long* out32) {
     }
     // step timeline [ns], folded into the free slot pairs: [7] idle before the EKF launch, [24..26] EKF launch, idle between the
     // launches, post launch
-    if (h->d.trace) {
+    if (h->d.x.trace) {
         unsigned long long t8[9] = {};
-        PF_CUDA(cudaMemcpy(t8, h->d.trace + 32, 9 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        PF_CUDA(cudaMemcpy(t8, h->d.x.trace + 32, 9 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
         out32[7] = t8[0]; out32[24] = t8[1]; out32[25] = t8[2]; out32[26] = t8[3]; out32[27] = t8[8];
     }
     return 0;

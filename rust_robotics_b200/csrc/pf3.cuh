@@ -7,7 +7,7 @@
 // clone the poses, and refresh the cached estimate + covariance (pf.rs:382-413, 499-503).  Run as separate kernels that is ~21
 // launches of a few microseconds each — the step is launch-latency bound below ~10^5 particles.  Here the
 // same arithmetic runs in one kernel of <= one co-resident CTA per SM, built on the FastSLAM post kernel's machinery: the exact
-// sequential sums are fs3_xsum (fs3.cuh) over tiles held in shared memory, grid barriers are arrival counters.
+// sequential sums are fs3_xsum (fs3.cuh) over tiles held in shared memory, grid barriers are arrival counters (workspace x).
 //
 // Bit-exactness: the three sums (S = sum w_raw, Q = sum w^2, the cumulative weights) are the reference's sequential f64 sums,
 // exactly (x3_core.h); the divisions are IEEE; the uniforms are the Philox stream the unfused path draws (same stream, call
@@ -29,7 +29,7 @@ struct Pf3Arg {
 
 template <int NT>
 __global__ void __launch_bounds__(NT, 1)
-pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg a) {
+pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg a) {
     extern __shared__ __align__(16) double vals[];            // [2][K][NT]: the tile's weights, their squares
     __shared__ Fs3Sh<NT> sh;
     const PfDev& pd = a.pd;
@@ -37,7 +37,7 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
     const unsigned b = blockIdx.x, nt = gridDim.x, K = a.K;
     const size_t n = pd.n, T = (size_t)NT * K, g0 = (size_t)b * T + (size_t)tid * K;
     double* vals2 = vals + (size_t)K * NT;
-    Fs3State* st = d.st;
+    Fs3State* st = x.st;
     const int cur = *pd.cur;
     // centre of the moment sums: the previous estimate (pf_moments_kernel)
     const double c0 = pf_finite_or_zero(pd.scal[4]), c1 = pf_finite_or_zero(pd.scal[5]), c2 = pf_finite_or_zero(pd.scal[6]), c3 = pf_finite_or_zero(pd.scal[7]);
@@ -47,14 +47,14 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
     for (unsigned k = 0; k < K; ++k) { const double v = g0 + k < n ? pd.w_raw[g0 + k] : 0.0; vals[k * NT + tid] = v; ts += v; tq += v * v; }
     fs3_block_sum2<NT>(ts, tq, sh.red[0], sh.red[1]);
     if (tid == 0) { a.tsum[b] = ts; a.tsq[b] = tq; }
-    fs3_grid_sync<NT>(d, 7, nt);
+    fs3_grid_sync<NT>(x, PF3_R_TILES, nt);
     double toff = 0.0, qoff = 0.0;
 #pragma unroll 2
     for (unsigned p = tid; p < b; p += NT) { toff += __ldcg(a.tsum + p); qoff += __ldcg(a.tsq + p); }
     fs3_block_sum2<NT>(toff, qoff, sh.red[0], sh.red[1]);      // (red[] is free again: the grid barrier above is also a block barrier;
                                                                //  wd[] is the first scratch fs3_xsum writes, with no barrier in between)
     // ---------------- S = sum w_raw, sequential (normalize_weights pf.rs:426-439) ----------------
-    const double S = fs3_xsum<NT>(d, sh, vals, K, nt, toff, 0, 0, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
+    const double S = fs3_xsum<NT>(x, sh, vals, K, nt, toff, FS3_S, PF3_R_S, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
     const double unif = 1.0 / (double)pd.n_global;
 #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) {
@@ -83,7 +83,7 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
         if (!scale_ok || !(fabs(neff - thr) > slack * fmax(fabs(thr), fabs(neff)))) {     // rare; the same decision in every CTA
             const double toffq = S > 0.0 ? fs3_div(fs3_div(qoff, S), S) : (double)((size_t)b * T) * unif * unif;
             __syncthreads();
-            Q = fs3_xsum<NT>(d, sh, vals2, K, nt, toffq, 1, 1, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
+            Q = fs3_xsum<NT>(x, sh, vals2, K, nt, toffq, FS3_Q, PF3_R_Q, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
             neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
         }
         gate = neff < thr ? 1 : 0;
@@ -92,14 +92,14 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
     if (gate) {
         // ---------------- cumulative weights (pf.rs:448-453 / mcl.rs:328-336), exact inclusive prefix of every weight ----------------
         const double toffc = S > 0.0 ? fs3_div(toff, S) : (double)((size_t)b * T) * unif;
-        __syncthreads();
+        __syncthreads();                                       // (without the Q sum, the S sum used the same scratch half)
         Fs3Run run;
-        ctot = fs3_xsum<NT>(d, sh, vals, K, nt, toffc, 3, 2, a.m32, pd.cum, 0, 0.0, 0.0, 0.0, 0.0, 1, &run);
-        (void)fs3_xsum_emit<NT>(d, sh, vals, K, a.m32, &run, 2, pd.cum, 1, nullptr, 15);
+        ctot = fs3_xsum<NT>(x, sh, vals, K, nt, toffc, FS3_CDF, PF3_R_CDF, a.m32, pd.cum, 0, 0.0, 0.0, 0.0, 0.0, 1, &run);
+        (void)fs3_xsum_emit<NT>(x, sh, vals, K, a.m32, &run, PF3_R_CDF, pd.cum, 1, nullptr, 15);
         __syncthreads();                                       // every prefix of this tile is stored before the last one is overridden
-        if (a.mode == 1 && b == (unsigned)((n - 1) / T) && tid == 0) { pd.cum[n - 1] = 1.0; d.tileEnd[b] = 1.0; }   // *last = 1.0 mcl.rs:334-336
-        fs3_grid_sync<NT>(d, 4, nt);                           // the whole CDF is visible
-        if ((unsigned)tid < nt) sh.tend[tid] = __ldcg(d.tileEnd + tid);
+        if (a.mode == 1 && b == (unsigned)((n - 1) / T) && tid == 0) { pd.cum[n - 1] = 1.0; x.tileEnd[b] = 1.0; }   // *last = 1.0 mcl.rs:334-336
+        fs3_grid_sync<NT>(x, PF3_R_CDF_DONE, nt);              // the whole CDF is visible
+        if ((unsigned)tid < nt) sh.tend[tid] = __ldcg(x.tileEnd + tid);
         __syncthreads();
         // ---------------- one uniform per output slot, first index with r <= c_i, clone (pf.rs:456-470, mcl.rs:344-361) ----------------
         const uint32_t call = pd.counters[0];
@@ -165,12 +165,12 @@ pf3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Pf3Arg
     if (tid == 0) sh.last = (atom_add_acq_rel_gpu(&st->post_done, 1u) + 1u == nt) ? 1 : 0;   // release my CTA's writes / acquire everybody's
     __syncthreads();
     if (!sh.last) return;
-    if (tid < FS3_SLOTS) { d.flagsg[tid] = 0; d.entCnt[tid] = 0u; }
-    if (tid < 8) { d.bar[tid] = 0u; d.resflag[tid] = 0u; }
+    if (tid < FS3_SLOTS) { x.flagsg[tid] = 0; x.entCnt[tid] = 0u; }
+    if (tid < FS3_ROUNDS) { x.bar[tid] = 0u; x.resflag[tid] = 0u; }
     if (tid < PF_MOM) {
         double s = 0.0;
 #pragma unroll 1
-        for (unsigned x = 0; x < nt; ++x) s += __ldcg(a.mom + (size_t)x * PF_MOM + tid);
+        for (unsigned c = 0; c < nt; ++c) s += __ldcg(a.mom + (size_t)c * PF_MOM + tid);
         sh.bef[tid] = s;
     }
     __syncthreads();

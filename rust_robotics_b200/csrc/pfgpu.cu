@@ -133,7 +133,8 @@ struct pfgpu_pf {
     // fused tail of the step (pf3.cuh): everything after the predict + likelihood kernel in one cooperative launch
     struct Fused {
         bool on = false;
-        Fs3Dev x = {};             // workspace of the exact-sum routine (fs3_xsum)
+        bool last = false;         // it ran the last exact sum (set by pfgpu_pf_step; cleared by pf_total, ahead of every other sum)
+        Fs3Sum x = {};             // its exact sums and grid barriers
         Pf3Arg arg = {};
         unsigned tiles = 0;
         size_t smem = 0;
@@ -283,27 +284,9 @@ static int pf3_setup(pfgpu_pf* h) {
     if (cudaFuncSetAttribute(pf3_post_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, pf3_post_kernel<256>, (int)NT, smem) != cudaSuccess || (size_t)nb * (size_t)h->ctx.num_sms < tiles) { cudaGetLastError(); return 0; }
-    Fs3Dev& x = h->fu.x;
-    x.n = (unsigned)n; x.n_glob = n; x.off = 0; x.G = 1; x.rank = 0; x.wait_inline = 1;
-    x.wraw[0] = h->d.w_raw; x.wraw[1] = h->d.w_raw; x.wn_all = h->d.w;
-    const size_t nsl = (size_t)FS3_SLOTS * FS3_MAX_TILES, nen = (size_t)FS3_SLOTS * FS3_ENT_CAP;
-    Fs3State* stp = nullptr;
-    PF_CUDA(cudaMalloc(&stp, sizeof(Fs3State))); PF_CUDA(cudaMemset(stp, 0, sizeof(Fs3State)));
-    x.st = stp;
-    PF_CUDA(cudaMalloc(&x.tileP, nsl * sizeof(unsigned long long)));
-    PF_CUDA(cudaMalloc(&x.tileQ, FS3_MAX_TILES * sizeof(double)));
-    PF_CUDA(cudaMalloc(&x.entCnt, 8 * sizeof(unsigned))); PF_CUDA(cudaMemset(x.entCnt, 0, 8 * sizeof(unsigned)));
-    PF_CUDA(cudaMalloc(&x.entKey, nen * sizeof(unsigned))); PF_CUDA(cudaMalloc(&x.entTile, nen * sizeof(unsigned)));
-    PF_CUDA(cudaMalloc(&x.entP, nen * sizeof(unsigned long long))); PF_CUDA(cudaMalloc(&x.entV, nen * sizeof(double)));
-    PF_CUDA(cudaMalloc(&x.entL, nen * sizeof(int)));
-    PF_CUDA(cudaMalloc(&x.bar, 8 * sizeof(unsigned))); PF_CUDA(cudaMemset(x.bar, 0, 8 * sizeof(unsigned)));
-    PF_CUDA(cudaMalloc(&x.resflag, 8 * sizeof(unsigned))); PF_CUDA(cudaMemset(x.resflag, 0, 8 * sizeof(unsigned)));
-    PF_CUDA(cudaMalloc(&x.res, 8 * sizeof(Fs3Res))); PF_CUDA(cudaMemset(x.res, 0, 8 * sizeof(Fs3Res)));
-    PF_CUDA(cudaMalloc(&x.resTP, (size_t)8 * FS3_MAX_TILES * sizeof(unsigned long long)));
-    PF_CUDA(cudaMalloc(&x.resKey, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned))); PF_CUDA(cudaMalloc(&x.resP, (size_t)8 * FS3_ENT_CAP * sizeof(unsigned long long)));
-    PF_CUDA(cudaMalloc(&x.resAft, (size_t)8 * FS3_ENT_CAP * sizeof(double)));
-    PF_CUDA(cudaMalloc(&x.tileEnd, FS3_MAX_TILES * sizeof(double)));
-    PF_CUDA(cudaMalloc(&x.flagsg, 8 * sizeof(int))); PF_CUDA(cudaMemset(x.flagsg, 0, 8 * sizeof(int)));
+    Fs3Sum& x = h->fu.x;
+    PF_CUDA(fs3_sum_alloc(x, (unsigned)n, false));
+    x.raw[0] = x.raw[1] = h->d.w_raw; x.wn = h->d.w;                                       // one raw buffer: PF steps have no parity
     Pf3Arg& a = h->fu.arg;
     a.pd = h->d; a.threshold = h->cfg.resample_threshold; a.mode = h->cfg.mode; a.seed = h->seed; a.K = K; a.m32 = x3_margin32(n);
     PF_CUDA(cudaMalloc(&a.tsum, FS3_MAX_TILES * sizeof(double))); PF_CUDA(cudaMalloc(&a.tsq, FS3_MAX_TILES * sizeof(double)));
@@ -313,10 +296,7 @@ static int pf3_setup(pfgpu_pf* h) {
     return 0;
 }
 static void pf3_free(pfgpu_pf* h) {
-    Fs3Dev& x = h->fu.x;
-    cudaFree(x.st); cudaFree(x.tileP); cudaFree(x.tileQ); cudaFree(x.entCnt); cudaFree(x.entKey); cudaFree(x.entTile); cudaFree(x.entP);
-    cudaFree(x.entV); cudaFree(x.entL); cudaFree(x.bar); cudaFree(x.resflag); cudaFree(x.res); cudaFree(x.resTP); cudaFree(x.resKey);
-    cudaFree(x.resP); cudaFree(x.resAft); cudaFree(x.tileEnd); cudaFree(x.flagsg);
+    fs3_sum_free(h->fu.x);
     cudaFree(h->fu.arg.tsum); cudaFree(h->fu.arg.tsq); cudaFree(h->fu.arg.mom);
 }
 
@@ -505,6 +485,7 @@ __global__ void __launch_bounds__(PF_NT) pf_gather_sharded_kernel(PfDev d, const
 }
 template <class F>
 static int pf_total(pfgpu_pf* h, F f, double* out) {
+    h->fu.last = false;
     if (h->world > 1) return xs_total_sharded(h->ctx, h->xs, h->sh, f, h->d.n, h->d.n_global, out);
     return xs_total(h->ctx, h->xs, f, h->d.n, h->d.n_global, 0.0, out);
 }
@@ -564,7 +545,7 @@ static int pf_resample_impl(pfgpu_pf* h) {
     PfDev& d = h->d;
     if (h->world > 1) return pf_resample_sharded(h);
     if (h->adaptive) return pf_resample_adaptive(h);
-    int rc = xs_total(h->ctx, h->xs, PfValWSq{d.w}, d.n, d.n_global, 0.0, d.scal + 1);        // calc_n_eff pf.rs:416-423
+    int rc = pf_total(h, PfValWSq{d.w}, d.scal + 1);                                           // calc_n_eff pf.rs:416-423
     if (rc) return rc;
     PF_LAUNCH(h->ctx, pf_gate_kernel, 1, 1, 0, d, h->cfg.resample_threshold, h->cfg.mode);
     // cumulative weights (pf.rs:448-453), exact; the kernels below are no-ops when the gate is closed
@@ -699,6 +680,7 @@ extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3,
         if (done) { rc = pf_graph_replay(h, u, obs3, k); if (rc) return rc; }
     }
     if (!done) { rc = pf_step_launches(h, u, obs3, k); if (rc) return rc; }
+    h->fu.last = h->fu.on;
     h->n_predict++;
     h->steps++;
     if (est) {
@@ -754,14 +736,6 @@ static void timer_drain(KernelTimer& t) {
     }
     t.pending.clear();
 }
-static int read_xs_flags(Ctx& ctx, XsWork& xs, pfgpu_stats* s) {
-    int f[4] = {0, 0, 0, 0};
-    PF_CUDA(cudaMemcpy(f, xs.flags + 4, 4 * sizeof(int), cudaMemcpyDeviceToHost));
-    s->serial_fallbacks = (uint64_t)f[0];
-    s->xsum_dirty_last = (uint64_t)(f[1] < 0 ? 0 : f[1]);
-    (void)ctx;
-    return 0;
-}
 extern "C" int pfgpu_pf_stats(pfgpu_pf* h, pfgpu_stats* s) {
     if (!h || !s) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
@@ -772,7 +746,15 @@ extern "C" int pfgpu_pf_stats(pfgpu_pf* h, pfgpu_stats* s) {
     PF_CUDA(cudaMemcpy(&cnt, h->d.counters, sizeof(unsigned int), cudaMemcpyDeviceToHost));
     s->kernel_launches = h->ctx.launches; s->steps = h->steps; s->resamples = cnt;
     s->main_kernel_ms_sum = h->timer.ms_sum; s->main_kernel_count = h->timer.count;
-    return read_xs_flags(h->ctx, h->xs, s);
+    int f[4] = {0, 0, 0, 0};                                   // the separate kernels' exact sums (xsum.cuh)
+    PF_CUDA(cudaMemcpy(f, h->xs.flags + 4, 4 * sizeof(int), cudaMemcpyDeviceToHost));
+    s->serial_fallbacks = (uint64_t)f[0];
+    s->xsum_dirty_last = (uint64_t)(f[1] < 0 ? 0 : f[1]);
+    if (!h->fu.on) return 0;
+    Fs3State st; PF_CUDA(cudaMemcpy(&st, h->fu.x.st, sizeof(st), cudaMemcpyDeviceToHost));     // the fused tail's (pf3.cuh)
+    s->serial_fallbacks += (uint64_t)st.serial_walks + (uint64_t)st.cert_fail;
+    if (h->fu.last) s->xsum_dirty_last = (uint64_t)st.dirty_last;
+    return 0;
 }
 extern "C" int pfgpu_pf_time_main_kernel(pfgpu_pf* h, int on) {
     if (!h) return PFGPU_ERR_INVALID;
