@@ -125,8 +125,20 @@ enum {
     PFC_STREAM_INIT_A      = 4,  /* pf.rs:182-183 / mcl.rs:191-192: x,y jitter of particle i            */
     PFC_STREAM_INIT_B      = 5,  /* pf.rs:184-185 / mcl.rs:193-194: yaw,v jitter of particle i          */
     PFC_STREAM_OBS         = 6,  /* synthetic observation noise (examples / bench drivers)              */
-    PFC_STREAM_FS2_POSE3   = 7   /* fs2.rs:234: the third N(0,1) of sample_pose (the first two use FS_PREDICT) */
+    PFC_STREAM_FS2_POSE3   = 7,  /* fs2.rs:234: the third N(0,1) of sample_pose (the first two use FS_PREDICT) */
+    /* augmented MCL (not in the reference; DESIGN §3.8), 53-bit uniforms, call = the predict's call index, index = global slot */
+    PFC_STREAM_PF_INJECT_A = 8,  /* (decision u < p, x fraction) of the slot                            */
+    PFC_STREAM_PF_INJECT_B = 9,  /* (y fraction, yaw fraction) of the slot                              */
+    PFC_STREAM_REGION_A    = 10, /* init_region, call 0: (x fraction, y fraction) of particle i         */
+    PFC_STREAM_REGION_B    = 11  /* init_region, call 0: (yaw fraction, unused) of particle i           */
 };
+/* A pose drawn uniformly over the box [x0, x1] x [y0, y1] from three 53-bit fractions (augmented MCL's injection and init_region):
+ * x = x0 + fx * (x1 - x0), y = y0 + fy * (y1 - y0), yaw = fyaw * 2 pi - pi. */
+PFC_HD void pfc_region_pose(const double r4[4], double fx, double fy, double fyaw, double* x, double* y, double* yaw) {
+    *x = r4[0] + fx * (r4[1] - r4[0]);
+    *y = r4[2] + fy * (r4[3] - r4[2]);
+    *yaw = fyaw * PFC_TWO_PI - PFC_PI;
+}
 
 /* One block per (seed, stream, call#, index): counter = (index_lo, index_hi, call#, stream). */
 PFC_HD pfc_u32x4 pfc_rng_block(uint64_t seed, uint32_t stream, uint32_t call, uint64_t index) {

@@ -88,6 +88,35 @@ int  pfgpu_pf_set_range_noise(pfgpu_pf*, double range_noise);                /* 
 /* parity hook: ancestry of the last step's resample (global indices); *n = 0 when the last step did not resample */
 int  pfgpu_pf_last_indices(pfgpu_pf*, uint32_t* idx, size_t cap, size_t* n);
 int  pfgpu_pf_sync(pfgpu_pf*);
+/* Global localisation and kidnapped-robot recovery: augmented MCL (not in the reference, whose cloud can only copy particles it
+ * already has; Probabilistic Robotics Table 8.3, ROS AMCL's recovery_alpha_slow / recovery_alpha_fast; DESIGN §3.8).  Recovery
+ * state: w_slow, w_fast (f64, both 0 at the start), 0 < alpha_slow < alpha_fast <= 1, and a box region = (x0, x1, y0, y1), finite,
+ * x0 < x1, y0 < y1.
+ *   filter     every time the engine computes S = sum w_raw (every pfgpu_pf_update and pfgpu_pf_step, on every path), with N the
+ *              global particle count those weights belong to (before a KLD resample changes it): w_avg = S / N,
+ *              w_slow = w_slow + alpha_slow * (w_avg - w_slow), w_fast = w_fast + alpha_fast * (w_avg - w_fast), in this order.  S NaN
+ *              or +-inf: skipped.  S = 0 (every likelihood underflowed) is not skipped.  Then p = max(0, 1 - w_fast / w_slow), and
+ *              p = 0 when w_slow <= 0 or the quotient is not finite.
+ *   injection  the first predict (pfgpu_pf_predict, or the predict half of pfgpu_pf_step) after a resample stage (pfgpu_pf_step or
+ *              pfgpu_pf_resample) that resampled, with no update in between, first replaces each slot independently with
+ *              probability p: with the 53-bit uniforms (a0, a1) of Philox stream PF_INJECT_A and (b0, b1) of PF_INJECT_B, keyed by the
+ *              predict's call index and the global slot, the slot is replaced when a0 < p, by x = x0 + a1 (x1 - x0),
+ *              y = y0 + b0 (y1 - y0), yaw = b1 * 2 pi - pi, v = 0; its weight (1/N after the resample) stays.  Then every slot is
+ *              predicted.  A PF step whose N_eff gate stays closed injects nothing in the next predict; nor does a second predict.
+ *              The estimate and the particles a step returns are the resampled set before injection (no uniform sample enters the
+ *              pose mean).  KLD-adaptive MCL: the slots of the new count.  Sharded: every rank holds the global S and the same p.
+ * pfgpu_pf_recovery_enable: alpha_slow = alpha_fast = 0 disables (region may be NULL); anything else outside the rules above:
+ *   PFGPU_ERR_INVALID.  Enabling (again), pfgpu_pf_upload, pfgpu_pf_init_state and pfgpu_pf_init_region reset w_slow = w_fast = 0
+ *   and disarm the injection.  Disabled (the default) nothing changes.  While enabled every predict adds one memset and every S one
+ *   single-thread launch; no host synchronisation.  On a sharded engine every rank makes the same calls.
+ * pfgpu_pf_recovery_state: out3 = (w_slow, w_fast, p) and the slots the last predict injected on this handle (both nullable);
+ *   synchronises.
+ * pfgpu_pf_init_region: every particle uniform over the region (x, y fractions from stream REGION_A, the yaw fraction from
+ *   REGION_B[0], call 0, the formulas above), v = 0, w = 1/N; KLD-adaptive MCL restarts at min_particles.  Works with recovery on or
+ *   off. */
+int  pfgpu_pf_recovery_enable(pfgpu_pf*, double alpha_slow, double alpha_fast, const double region[4]);
+int  pfgpu_pf_recovery_state(pfgpu_pf*, double out3[3], uint64_t* injected_last);
+int  pfgpu_pf_init_region(pfgpu_pf*, const double region[4]);
 
 /* ============================================ FastSLAM 1.0 ========================================== */
 

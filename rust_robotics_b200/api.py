@@ -80,6 +80,7 @@ EXPORTS = [
     "pfgpu_fs_moments", "pfgpu_fs_estimate_merge", "pfgpu_fs_step_unknown", "pfgpu_fs_assoc_counts",
     "pfgpu_fs_history_enable", "pfgpu_fs_history_window", "pfgpu_fs_path", "pfgpu_fs_path_moments",
     "pfgpu_fs_existence_enable", "pfgpu_fs_existence_counts", "pfgpu_fs_existence_removed",
+    "pfgpu_pf_recovery_enable", "pfgpu_pf_recovery_state", "pfgpu_pf_init_region",
 ]
 
 
@@ -119,6 +120,9 @@ def load_library():
     L.pfgpu_pf_set_range_noise.argtypes = [vp, C.c_double]
     L.pfgpu_pf_last_indices.argtypes = [vp, c_u32p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfgpu_pf_sync.argtypes = [vp]
+    L.pfgpu_pf_recovery_enable.argtypes = [vp, C.c_double, C.c_double, c_dp]
+    L.pfgpu_pf_recovery_state.argtypes = [vp, c_dp, C.POINTER(C.c_uint64)]
+    L.pfgpu_pf_init_region.argtypes = [vp, c_dp]
     L.pfgpu_fs_default_config.argtypes = [C.POINTER(_FsCfg)]
     L.pfgpu_fs_create.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, C.POINTER(vp)]
     L.pfgpu_fs_create_sharded.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, vp, C.c_int,
@@ -351,6 +355,43 @@ class _PfBase:
 
     def flush_l2(self):
         _check(self.L, self.L.pfgpu_pf_flush_l2(self.h))
+
+    # -- augmented MCL (not in the reference, whose cloud only copies particles it has; DESIGN §3.8) --
+    def enable_recovery(self, alpha_slow=0.001, alpha_fast=0.1, region=None):
+        """Random-particle injection for global localisation and kidnapped-robot recovery (Probabilistic Robotics Table 8.3; ROS
+        AMCL's recovery_alpha_slow / recovery_alpha_fast).  The filter tracks short- and long-term averages of the mean likelihood;
+        when the short one falls below the long one, the first predict after a resample replaces each particle with probability
+        p = max(0, 1 - w_fast / w_slow) by a pose drawn uniformly over region = (x0, x1, y0, y1).  alpha_slow = alpha_fast = 0
+        disables.  Resets w_slow = w_fast = 0 (so do set_particles, init_state and init_region).  On a sharded engine every rank
+        makes the same call."""
+        reg = _f64(region) if region is not None else None
+        if reg is not None and reg.size != 4:
+            raise InvalidParameter("region = (x0, x1, y0, y1)")
+        _check(self.L, self.L.pfgpu_pf_recovery_enable(self.h, float(alpha_slow), float(alpha_fast), _dp(reg) if reg is not None else None))
+
+    def disable_recovery(self):
+        self.enable_recovery(0.0, 0.0, None)
+
+    def recovery_state(self):
+        """(w_slow, w_fast, p, injected): the averages, the injection probability of the next armed predict, and the particles
+        this handle's last predict injected.  Synchronises."""
+        out, inj = np.empty(3), C.c_uint64()
+        _check(self.L, self.L.pfgpu_pf_recovery_state(self.h, _dp(out), C.byref(inj)))
+        return float(out[0]), float(out[1]), float(out[2]), int(inj.value)
+
+    def init_region(self, region):
+        """global initialisation: every particle uniform over region = (x0, x1, y0, y1), yaw uniform in [-pi, pi), v = 0, w = 1/n"""
+        reg = _f64(region)
+        if reg.size != 4:
+            raise InvalidParameter("region = (x0, x1, y0, y1)")
+        _check(self.L, self.L.pfgpu_pf_init_region(self.h, _dp(reg)))
+
+    @classmethod
+    def try_with_region(cls, region, config, **kw):
+        """a filter that does not know where it is: init_region(region) instead of try_with_initial_state's +-1 m cloud"""
+        f = cls(config, **kw)
+        f.init_region(region)
+        return f
 
 
 class ParticleFilterLocalizer(_PfBase):

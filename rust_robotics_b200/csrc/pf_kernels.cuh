@@ -49,13 +49,23 @@ __device__ __forceinline__ void pose_store(Pose4* p, size_t i, const Pose4& o) {
     q[0] = make_double2(o.x, o.y); q[1] = make_double2(o.yaw, o.v);
 }
 
+// Augmented MCL (DESIGN §3.8): the recovery state lives next to the step's scalars, the injection count next to the draw counter.
+#define PF_REC_SLOW 24             // scal[24] w_slow, scal[25] w_fast, scal[26] p (injection probability)
+#define PF_REC_FAST 25
+#define PF_REC_P 26
+#define PF_REC_COUNT 1             // counters[1]: slots injected by the last predict
+// injection arguments of a predict: the region (x0, x1, y0, y1) and whether this is the first predict after a resample stage
+struct PfInj { double r[4]; int arm; };
+
 // try_predict_with_control (pf.rs:279-296, mcl.rs:236-253) and/or the likelihood loop of
 // try_update_with_observations (pf.rs:316-329, mcl.rs:273-283), fused in one pass over the pose records.
-template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS>
+// INJ (augmented MCL): when `inj.arm` and the last resample stage resampled (*d.gate), each slot is first replaced with probability
+// p = scal[PF_REC_P] by a pose drawn uniformly over the region (weight unchanged), then predicted like any other.
+template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false>
 __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const __grid_constant__ PfObsParam po,
                                                                   double u0, double u1, double sv, double sw,
                                                                   double dt, uint64_t seed, uint32_t call,
-                                                                  int k_obs, double sigma) {
+                                                                  int k_obs, double sigma, PfInj inj) {
     extern __shared__ double s_obs_pf[];     // k_obs x (d, lx, ly): the observation vector staged once per CTA
     if (DO_WEIGHT) {
         for (int j = threadIdx.x; j < 3 * k_obs; j += PF_NT) s_obs_pf[j] = PARAM_OBS ? po.o[j] : d.obs[j];
@@ -66,6 +76,22 @@ __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const
     Pose4* pose = pf_pose(d, *d.cur);
     Pose4 p;
     pose_load(pose, i, p);
+    if constexpr (INJ) {
+        static_assert(DO_PREDICT, "injection happens in a predict");
+        const double pinj = d.scal[PF_REC_P];
+        if (inj.arm && *d.gate && pinj > 0.0) {                     // the same decision in every thread of the grid
+            const pfc_u32x4 a = pfc_rng_block(seed, PFC_STREAM_PF_INJECT_A, call, d.offset + i);
+            const bool hit = pfc_u01_53(pfc_blk_u64(a, 0)) < pinj;
+            if (hit) {
+                const pfc_u32x4 b = pfc_rng_block(seed, PFC_STREAM_PF_INJECT_B, call, d.offset + i);
+                pfc_region_pose(inj.r, pfc_u01_53(pfc_blk_u64(a, 1)), pfc_u01_53(pfc_blk_u64(b, 0)), pfc_u01_53(pfc_blk_u64(b, 1)),
+                                &p.x, &p.y, &p.yaw);
+                p.v = 0.0;
+            }
+            const unsigned act = __activemask(), votes = __ballot_sync(act, hit);   // one integer atomic per warp
+            if (votes && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(d.counters + PF_REC_COUNT, (unsigned)__popc(votes));
+        }
+    }
     if (DO_PREDICT) {
         double z0, z1;
         pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_PF_PREDICT, call, d.offset + i), &z0, &z1);
@@ -103,6 +129,40 @@ __global__ void __launch_bounds__(PF_NT) pf_normalize_kernel(PfDev d) {
     if (i >= d.n) return;
     const double S = d.scal[0];
     d.w[i] = S > 0.0 ? d.w_raw[i] / S : 1.0 / (double)d.n_global;
+}
+
+// augmented MCL's averages (Probabilistic Robotics Table 8.3) from S = scal[0] over the n_global weights S sums, then the injection
+// probability the next armed predict uses.  Non-finite S: no update.
+__global__ void pf_recovery_filter_kernel(PfDev d, double a_slow, double a_fast) {
+    const double S = d.scal[0];
+    double ws = d.scal[PF_REC_SLOW], wf = d.scal[PF_REC_FAST];
+    if (S - S == 0.0) {
+        const double w_avg = S / (double)d.n_global;
+        ws = ws + a_slow * (w_avg - ws);
+        wf = wf + a_fast * (w_avg - wf);
+        d.scal[PF_REC_SLOW] = ws; d.scal[PF_REC_FAST] = wf;
+    }
+    double p = 0.0;
+    if (ws > 0.0) {
+        const double q = wf / ws;
+        if (q - q == 0.0) { p = 1.0 - q; if (!(p > 0.0)) p = 0.0; }
+    }
+    d.scal[PF_REC_P] = p;
+}
+
+// global initialisation: every particle uniform over the region r4 = (x0, x1, y0, y1), v = 0, w = 1/n
+__global__ void pf_init_region_kernel(PfDev d, double x0, double x1, double y0, double y1, uint64_t seed) {
+    const size_t i = (size_t)blockIdx.x * PF_NT + threadIdx.x;
+    if (i >= d.n) return;
+    const double r4[4] = { x0, x1, y0, y1 };
+    const pfc_u32x4 a = pfc_rng_block(seed, PFC_STREAM_REGION_A, 0, d.offset + i);
+    const pfc_u32x4 b = pfc_rng_block(seed, PFC_STREAM_REGION_B, 0, d.offset + i);
+    Pose4 p;
+    pfc_region_pose(r4, pfc_u01_53(pfc_blk_u64(a, 0)), pfc_u01_53(pfc_blk_u64(a, 1)), pfc_u01_53(pfc_blk_u64(b, 0)), &p.x, &p.y, &p.yaw);
+    p.v = 0.0;
+    pose_store(pf_pose(d, *d.cur), i, p);
+    d.w[i] = 1.0 / (double)d.n_global;
+    d.w_raw[i] = d.w[i];
 }
 
 struct PfValWSq { const double* w; __device__ __forceinline__ double operator()(size_t i) const { double x = w[i]; return x * x; } };

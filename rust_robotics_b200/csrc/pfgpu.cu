@@ -149,6 +149,13 @@ struct pfgpu_pf {
         int captures = 0;          // an observation count that keeps changing would re-capture every step: give up after a few
         bool off = false;          // PFGPU_PF_GRAPH=0, capture failed, or too many re-captures: plain launches from then on
     } sg;
+    // augmented MCL (DESIGN §3.8): w_slow, w_fast and p live in d.scal[PF_REC_*], the injection count in d.counters[PF_REC_COUNT]
+    struct Recovery {
+        bool on = false;
+        bool armed = false;        // the last stage was a resample stage: the next predict injects if that stage resampled (*d.gate)
+        double a_slow = 0.0, a_fast = 0.0;
+        double region[4] = {0.0, 0.0, 0.0, 0.0};     // x0, x1, y0, y1
+    } rec;
 };
 
 extern "C" void pfgpu_pf_default_config(pfgpu_pf_config* c, int mode) {
@@ -227,6 +234,18 @@ static int pf_refresh_cache(pfgpu_pf* h) {      // refresh_cache pf.rs:499-503
         PF_NCCL(ncclAllReduce(h->mom15, h->mom15, PF_MOM, ncclDouble, ncclSum, h->sh.comm, h->ctx.stream));
     PF_LAUNCH(h->ctx, pf_moments_final_kernel, 1, 32, 0, h->d, h->mom15);
     return 0;
+}
+// augmented MCL: w_slow = w_fast = p = 0, injection count 0, disarmed
+static int pf_recovery_reset(pfgpu_pf* h) {
+    h->rec.armed = false;
+    PF_CUDA(cudaMemsetAsync(h->d.scal + PF_REC_SLOW, 0, 3 * sizeof(double), h->ctx.stream));
+    PF_CUDA(cudaMemsetAsync(h->d.counters + PF_REC_COUNT, 0, sizeof(unsigned int), h->ctx.stream));
+    return 0;
+}
+static bool pf_region_ok(const double* r) {      // finite, x0 < x1, y0 < y1
+    if (!r) return false;
+    for (int j = 0; j < 4; ++j) if (!finite_d(r[j])) return false;
+    return r[0] < r[1] && r[2] < r[3];
 }
 
 static int pf_alloc(pfgpu_pf* h, size_t cap) {
@@ -387,6 +406,7 @@ extern "C" int pfgpu_pf_init_state(pfgpu_pf* h, const double s[4]) {
     for (int k = 0; k < 4; ++k) if (!finite_d(s[k])) return PFGPU_ERR_INVALID;     // validate_state pf.rs:505-513
     PF_CUDA(cudaSetDevice(h->ctx.device));
     PF_LAUNCH(h->ctx, pf_init_state_kernel, cdiv_u(h->d.n, PF_NT), PF_NT, 0, h->d, s[0], s[1], s[2], s[3], h->seed, h->cfg.mode);
+    if (h->rec.on) { int rc = pf_recovery_reset(h); if (rc) return rc; }
     return pf_refresh_cache(h);
 }
 // device temporary of the bulk transfers: released on every exit path (PF_CUDA / PF_LAUNCH return early on errors)
@@ -402,6 +422,7 @@ extern "C" int pfgpu_pf_upload(pfgpu_pf* h, const double* aos5, size_t n) {
     double* tmp = t.p;
     PF_CUDA(cudaMemcpyAsync(tmp, aos5, n * 5 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     PF_LAUNCH(h->ctx, pf_unpack_kernel, cdiv_u(n, PF_NT), PF_NT, 0, h->d, tmp);
+    if (h->rec.on) { int rc = pf_recovery_reset(h); if (rc) return rc; }
     int rc = pf_refresh_cache(h);
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     return rc;
@@ -440,24 +461,46 @@ static int pf_stage_obs(pfgpu_pf* h, const double* obs3, size_t k) {
 }
 static size_t pf_obs_smem(size_t k) { return (k ? k : 1) * 3 * sizeof(double); }
 
-template <bool P, bool W>
-static int pf_launch_main(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
+// the injection arguments of the next predict (augmented MCL, DESIGN §3.8)
+static PfInj pf_inj(const pfgpu_pf* h) {
+    PfInj a = {};
+    if (h->rec.on) { for (int j = 0; j < 4; ++j) a.r[j] = h->rec.region[j]; a.arm = h->rec.armed ? 1 : 0; }
+    return a;
+}
+template <bool P, bool W, bool INJ>
+static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
     size_t smem = W ? pf_obs_smem(k) : 0;
     const bool param = !W || k <= PF_PARAM_OBS;
     PfObsParam po;
     if (W && param) for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
     if (smem > 48 * 1024) {
-        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
+    const PfInj inj = pf_inj(h);
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
     if (param)
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise);
+        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true, INJ>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
+                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj);
     else
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise);
+        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false, INJ>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
+                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj);
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
+    return 0;
+}
+template <bool P, bool W>
+static int pf_launch_main(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
+    if constexpr (P) {
+        if (h->rec.on) {                                             // every predict counts its injections afresh
+            PF_CUDA(cudaMemsetAsync(h->d.counters + PF_REC_COUNT, 0, sizeof(unsigned int), h->ctx.stream));
+            return pf_launch_kernel<P, W, true>(h, u, obs3, k);
+        }
+    }
+    return pf_launch_kernel<P, W, false>(h, u, obs3, k);
+}
+// augmented MCL's filter, right after S = sum w_raw has landed in scal[0]
+static int pf_recovery_filter(pfgpu_pf* h) {
+    if (h->rec.on) PF_LAUNCH(h->ctx, pf_recovery_filter_kernel, 1, 1, 0, h->d, h->rec.a_slow, h->rec.a_fast);
     return 0;
 }
 // normalize_weights: exact sequential sum of the raw weights, then the division pass
@@ -518,7 +561,7 @@ static int pf_normalize(pfgpu_pf* h) {
     int rc = pf_total(h, XsValArray{h->d.w_raw}, h->d.scal + 0);
     if (rc) return rc;
     PF_LAUNCH(h->ctx, pf_normalize_kernel, cdiv_u(h->d.n, PF_NT), PF_NT, 0, h->d);
-    return 0;
+    return pf_recovery_filter(h);
 }
 // resample_adaptive with a changing particle count (mcl.rs:322-365), see pf_kld.cuh
 static int pf_resample_adaptive(pfgpu_pf* h) {
@@ -576,6 +619,7 @@ extern "C" int pfgpu_pf_predict(pfgpu_pf* h, const double u[2]) {
     int rc = pf_launch_main<true, false>(h, u, nullptr, 0);
     if (rc) return rc;
     h->n_predict++;
+    h->rec.armed = false;
     return pf_refresh_cache(h);                                                      // pf.rs:299
 }
 extern "C" int pfgpu_pf_update(pfgpu_pf* h, const double* obs3, size_t k) {
@@ -585,6 +629,7 @@ extern "C" int pfgpu_pf_update(pfgpu_pf* h, const double* obs3, size_t k) {
     if (rc) return rc;
     rc = pf_launch_main<false, true>(h, nullptr, obs3, k);
     if (rc) return rc;
+    h->rec.armed = false;                                                            // the weights are no longer uniform
     rc = pf_normalize(h);                                                            // pf.rs:331
     if (rc) return rc;
     return pf_refresh_cache(h);                                                      // pf.rs:332
@@ -594,6 +639,7 @@ extern "C" int pfgpu_pf_resample(pfgpu_pf* h, int* did) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
     int rc = pf_resample_impl(h);
     if (rc) return rc;
+    h->rec.armed = true;
     rc = pf_refresh_cache(h);                                                        // pf.rs:343 (same values when the gate was closed)
     if (rc) return rc;
     if (did) { int g = 0; rc = pf_read_gate(h, &g); if (rc) return rc; *did = g; }
@@ -607,7 +653,7 @@ static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, 
         h->fu.arg.pd = h->d;
         h->fu.arg.threshold = h->cfg.resample_threshold;
         PF_LAUNCH(h->ctx, pf3_post_kernel<256>, h->fu.tiles, 256, h->fu.smem, h->fu.x, h->fu.arg);
-        return 0;
+        return pf_recovery_filter(h);                                                // S is in scal[0] once the launch ends
     }
     rc = pf_normalize(h);
     if (rc) return rc;
@@ -636,7 +682,7 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
     if (cudaGraphGetNodes(g, nullptr, &nn) != cudaSuccess || nn == 0) { cudaGetLastError(); pf_graph_drop(h); return 1; }
     std::vector<cudaGraphNode_t> nodes(nn);
     if (cudaGraphGetNodes(g, nodes.data(), &nn) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    const void* want = (const void*)pf_predict_weight_kernel<true, true, true>;
+    const void* want = h->rec.on ? (const void*)pf_predict_weight_kernel<true, true, true, true> : (const void*)pf_predict_weight_kernel<true, true, true>;
     for (cudaGraphNode_t nd : nodes) {
         cudaGraphNodeType ty;
         if (cudaGraphNodeGetType(nd, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
@@ -654,7 +700,8 @@ static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, s
     for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
     double u0 = u[0], u1 = u[1], sv = h->cfg.velocity_noise, sw = h->cfg.yaw_rate_noise, dt = h->cfg.dt, sigma = h->cfg.range_noise;
     uint64_t seed = h->seed; uint32_t call = h->n_predict; int kk = (int)k;
-    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma };
+    PfInj inj = pf_inj(h);
+    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma, &inj };
     cudaKernelNodeParams kp = h->sg.main_params;
     kp.kernelParams = args; kp.extra = nullptr;
     PF_CUDA(cudaGraphExecKernelNodeSetParams(h->sg.exec, h->sg.main_node, &kp));
@@ -683,6 +730,7 @@ extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3,
     h->fu.last = h->fu.on;
     h->n_predict++;
     h->steps++;
+    h->rec.armed = true;                                                             // the step ended with its resample stage
     if (est) {
         PF_CUDA(cudaMemcpyAsync(h->h_pin, h->d.scal + 4, 4 * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
@@ -726,6 +774,38 @@ extern "C" int pfgpu_pf_last_indices(pfgpu_pf* h, uint32_t* idx, size_t cap, siz
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     if (n) *n = c;
     return 0;
+}
+
+// ---- augmented MCL: random-particle injection for global localisation and kidnapped-robot recovery (DESIGN §3.8) ----
+extern "C" int pfgpu_pf_recovery_enable(pfgpu_pf* h, double alpha_slow, double alpha_fast, const double region[4]) {
+    if (!h) return PFGPU_ERR_INVALID;
+    const bool off = alpha_slow == 0.0 && alpha_fast == 0.0;
+    if (!off && (!(alpha_slow > 0.0) || !(alpha_slow < alpha_fast) || !(alpha_fast <= 1.0) || !pf_region_ok(region))) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    pf_graph_drop(h);                          // the captured step holds the predict instantiation and the filter's alphas
+    h->rec.on = !off;
+    h->rec.a_slow = off ? 0.0 : alpha_slow; h->rec.a_fast = off ? 0.0 : alpha_fast;
+    for (int j = 0; j < 4; ++j) h->rec.region[j] = off ? 0.0 : region[j];
+    return pf_recovery_reset(h);
+}
+extern "C" int pfgpu_pf_recovery_state(pfgpu_pf* h, double out3[3], uint64_t* injected_last) {
+    if (!h) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    double* hp = h->h_pin + 40;
+    PF_CUDA(cudaMemcpyAsync(hp, h->d.scal + PF_REC_SLOW, 3 * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaMemcpyAsync(hp + 3, h->d.counters + PF_REC_COUNT, sizeof(unsigned int), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    if (out3) for (int j = 0; j < 3; ++j) out3[j] = hp[j];
+    if (injected_last) { unsigned int c; memcpy(&c, hp + 3, sizeof(c)); *injected_last = c; }
+    return 0;
+}
+extern "C" int pfgpu_pf_init_region(pfgpu_pf* h, const double region[4]) {
+    if (!h || !pf_region_ok(region)) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    if (h->adaptive) h->d.n = h->d.n_global = h->cfg.n_particles;           // a fresh start: min_particles, like try_new
+    PF_LAUNCH(h->ctx, pf_init_region_kernel, cdiv_u(h->d.n, PF_NT), PF_NT, 0, h->d, region[0], region[1], region[2], region[3], h->seed);
+    if (h->rec.on) { int rc = pf_recovery_reset(h); if (rc) return rc; }
+    return pf_refresh_cache(h);
 }
 
 static void timer_drain(KernelTimer& t) {

@@ -81,6 +81,19 @@ public:
         return mirror_;
     }
     void init_state(const PFState& s) { check(pfgpu_pf_init_state(h_, s.data()), "initial state"); dirty_ = true; }
+    // augmented MCL (not in the reference; DESIGN §3.8): region = (x0, x1, y0, y1); alpha_slow = alpha_fast = 0 disables
+    using Region = std::array<double, 4>;
+    struct RecoveryState { double w_slow, w_fast, p; uint64_t injected; };
+    void enable_recovery(double alpha_slow, double alpha_fast, const Region& region) {
+        check(pfgpu_pf_recovery_enable(h_, alpha_slow, alpha_fast, region.data()), "recovery");
+    }
+    void disable_recovery() { check(pfgpu_pf_recovery_enable(h_, 0.0, 0.0, nullptr), "recovery"); }
+    RecoveryState recovery_state() const {
+        double w[3] = {0.0, 0.0, 0.0}; uint64_t inj = 0;
+        check(pfgpu_pf_recovery_state(h_, w, &inj), "recovery state");
+        return {w[0], w[1], w[2], inj};
+    }
+    void init_region(const Region& region) { check(pfgpu_pf_init_region(h_, region.data()), "initial region"); dirty_ = true; }
 };
 }  // namespace detail
 

@@ -72,6 +72,9 @@ extern "C" {
     pub fn pfgpu_pf_step(h: *mut pfgpu_pf, u: *const f64, obs3: *const f64, k: usize, est: *mut f64) -> c_int;
     pub fn pfgpu_pf_estimate(h: *mut pfgpu_pf, est: *mut f64, cov16_colmajor: *mut f64) -> c_int;
     pub fn pfgpu_pf_set_range_noise(h: *mut pfgpu_pf, range_noise: f64) -> c_int;
+    pub fn pfgpu_pf_recovery_enable(h: *mut pfgpu_pf, alpha_slow: f64, alpha_fast: f64, region: *const f64) -> c_int;
+    pub fn pfgpu_pf_recovery_state(h: *mut pfgpu_pf, out3: *mut f64, injected_last: *mut u64) -> c_int;
+    pub fn pfgpu_pf_init_region(h: *mut pfgpu_pf, region: *const f64) -> c_int;
     pub fn pfgpu_fs_default_config(cfg: *mut pfgpu_fs_config);
     pub fn pfgpu_fs_create(cfg: *const pfgpu_fs_config, n_particles: usize, n_landmarks: usize, seed: u64, device: c_int,
                            out: *mut *mut pfgpu_fs) -> c_int;

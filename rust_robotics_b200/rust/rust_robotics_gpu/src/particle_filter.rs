@@ -103,6 +103,27 @@ impl ParticleFilterLocalizer {
         s.refresh_cache()?;
         Ok(s)
     }
+    /// Augmented MCL (not in the reference; DESIGN §3.8): random-particle injection for global localisation and kidnapped-robot
+    /// recovery.  region = [x0, x1, y0, y1]; alpha_slow = alpha_fast = 0 disables.
+    pub fn enable_recovery(&mut self, alpha_slow: f64, alpha_fast: f64, region: [f64; 4]) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_recovery_enable(self.h, alpha_slow, alpha_fast, region.as_ptr()) })
+    }
+    /// (w_slow, w_fast, p, particles injected by the last predict)
+    pub fn recovery_state(&self) -> RoboticsResult<(f64, f64, f64, u64)> {
+        let (mut w, mut inj) = ([0.0f64; 3], 0u64);
+        status(unsafe { sys::pfgpu_pf_recovery_state(self.h, w.as_mut_ptr(), &mut inj) })?;
+        Ok((w[0], w[1], w[2], inj))
+    }
+    /// every particle uniform over region = [x0, x1, y0, y1], yaw uniform in [-pi, pi), v = 0, w = 1/n
+    pub fn init_region(&mut self, region: [f64; 4]) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_init_region(self.h, region.as_ptr()) })?;
+        self.refresh_cache()
+    }
+    pub fn try_with_region(region: [f64; 4], config: ParticleFilterConfig) -> RoboticsResult<Self> {
+        let mut s = Self::try_new(config)?;
+        s.init_region(region)?;
+        Ok(s)
+    }
     pub fn try_predict_with_control(&mut self, control: &PFControl) -> RoboticsResult<()> {      // pf.rs:255-301
         status(unsafe { sys::pfgpu_pf_predict(self.h, control.as_ptr()) })?;
         self.refresh_cache()

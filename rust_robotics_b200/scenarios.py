@@ -115,3 +115,41 @@ class PfScenario:
             self.controls.append(u)
             self.obs.append(np.stack([d, self.landmarks[:, 0], self.landmarks[:, 1]], axis=1))
         self.truth = t
+
+
+class KidnapScenario:
+    """Config 2's world (landmarks every `pitch_deg` degrees on a 30 m circle, range noise 0.25, u = (1.0, 0.03), dt 0.1) with a
+    kidnap: the robot starts at (0, 0, 0), drives `before` steps, is carried by `jump` = (dx, dy, dyaw) and drives `after` more
+    steps.  truth[t] = the pose the observations of step t are taken at.  before = 0: a robot that starts at start + jump,
+    the global-localisation case (init_region)."""
+    REGION = (-25.0, 25.0, -25.0, 25.0)          # where a lost robot may be: the box inside the landmark circle
+
+    def __init__(self, before=30, after=60, jump=(12.0, -9.0, 0.5), pitch_deg=1.0, seed=7):
+        rng = np.random.default_rng(seed)
+        ang = np.deg2rad(np.arange(0.0, 360.0, pitch_deg))
+        self.landmarks = np.stack([30.0 * np.cos(ang), 30.0 * np.sin(ang)], axis=1)
+        self.init = [0.0, 0.0, 0.0, 1.0]
+        self.before, self.dt = before, 0.1
+        t = [0.0, 0.0, 0.0] if before else [jump[0], jump[1], jump[2]]
+        self.controls, self.obs, self.truth = [], [], []
+        for k in range(before + after):
+            if before and k == before:
+                t = [t[0] + jump[0], t[1] + jump[1], t[2] + jump[2]]
+            u = (1.0, 0.03)
+            t[0] += u[0] * math.cos(t[2]) * self.dt
+            t[1] += u[0] * math.sin(t[2]) * self.dt
+            t[2] += u[1] * self.dt
+            rngd = np.hypot(t[0] - self.landmarks[:, 0], t[1] - self.landmarks[:, 1])
+            d = np.maximum(rngd + rng.normal(0.0, 0.25, rngd.shape), 0.0)
+            self.controls.append(u)
+            self.obs.append(np.ascontiguousarray(np.stack([d, self.landmarks[:, 0], self.landmarks[:, 1]], axis=1)))
+            self.truth.append(list(t))
+
+    @staticmethod
+    def config(n):
+        """config 2's MonteCarloLocalizationConfig arguments at n particles (fixed count): (min, max, eps, z, range, v, yaw, dt)"""
+        return (n, n, 0.05, 2.326, 0.25, 0.05, 0.02, 0.1)
+
+    def error(self, k, est):
+        """position error of the estimate after step k [m]"""
+        return math.hypot(est[0] - self.truth[k][0], est[1] - self.truth[k][1])
