@@ -117,6 +117,47 @@ int  pfgpu_pf_sync(pfgpu_pf*);
 int  pfgpu_pf_recovery_enable(pfgpu_pf*, double alpha_slow, double alpha_fast, const double region[4]);
 int  pfgpu_pf_recovery_state(pfgpu_pf*, double out3[3], uint64_t* injected_last);
 int  pfgpu_pf_init_region(pfgpu_pf*, const double region[4]);
+/* Localisation in an occupancy grid from a laser scan: the likelihood-field measurement model (not in the reference, whose MCL
+ * only ranges to known landmarks; Probabilistic Robotics Table 6.3, ROS AMCL's likelihood_field; DESIGN §3.9).
+ *   map        mask[ix * H + iy], W x H bytes, nonzero = obstacle; 1 <= W, H <= 65536, W * H <= 2^28.  World (0, 0) is the grid
+ *              centre: ix = floor(x / res + W / 2.0) as i32 (Rust's saturating cast: NaN -> 0), likewise iy with H; inside when
+ *              0 <= ix < W and 0 <= iy < H (world_to_grid, rust_robotics_mapping/src/occupancy_grid_map.rs:144-153).
+ *   table      D = the Euclidean distance field in cells (compute_udf, distance_map.rs:15-100: INF = 1e20, dt_1d over every ix, then
+ *              every iy, then sqrt; dt_1d's final loop reads the line's input, see DESIGN §3.9); per cell t = D * res,
+ *              g = coeff * exp(-(t * t) / (2 * (sigma_hit * sigma_hit))) with coeff = 1 / sqrt(2 pi * (sigma_hit * sigma_hit)),
+ *              q = z_hit * g + q_out, q_out = z_rand / max_range.  An endpoint outside the grid scores q_out.
+ *   beams      ranges r_0 .. r_{B-1}: candidates i = 0, s, 2s, .. < B with s = max(1, (B - 1) / (max_beams - 1)) (integer
+ *              division); a candidate is used unless r <= 0, r is not finite or r >= max_range.  a_i = i as f64 * angle_inc.
+ *   weight     per particle, over the used beams in ascending i: angle = (yaw + angle_min) + a_i, ex = x + r cos(angle),
+ *              ey = y + r sin(angle), w = w * q(ex, ey) from w = 1; w overwrites w_raw (no used beam: w = 1).  The rest of the
+ *              update (normalisation, recovery filter) and of the step (gate, resample, estimate) is the landmark path's.
+ *   bound      L = the largest count <= 4096 for which q_out^(L+1) >= DBL_MIN and q_max^(L+1) <= DBL_MAX (powers by repeated f64
+ *              multiplication; q_max = z_hit * coeff + q_out); so every w_raw is a positive normal number.  A scan with more than L
+ *              used beams is PFGPU_ERR_INVALID, and so is a map with L < 1.
+ * pfgpu_pf_lfield_set: res, sigma_hit, z_rand, max_range positive and finite, z_hit >= 0 and finite, max_beams >= 2, else
+ *   PFGPU_ERR_INVALID.  Replaces any map; builds the table on the device and synchronises.  On a sharded engine every rank makes the
+ *   same call and holds its own table.  pfgpu_pf_lfield_clear frees it.  Setting or clearing the map does not touch the particles.
+ * pfgpu_pf_lfield_info: W, H and L of the loaded map (all 0 without one).  pfgpu_pf_lfield_download: D and q (both nullable),
+ *   cells = W * H entries each, f64, ix * H + iy.
+ * pfgpu_pf_update_scan / pfgpu_pf_step_scan: pfgpu_pf_update / pfgpu_pf_step with the scan model; they may be mixed freely with the
+ *   landmark calls.  No map loaded, angle_min or angle_inc not finite, ranges NULL with B > 0, or more than L used beams:
+ *   PFGPU_ERR_INVALID. */
+typedef struct {
+    double   resolution;         /* metres per cell                                         */
+    double   sigma_hit;          /* 0.2  (AMCL laser_sigma_hit)                             */
+    double   z_hit;              /* 0.95 (AMCL laser_z_hit)                                 */
+    double   z_rand;             /* 0.05 (AMCL laser_z_rand)                                */
+    double   max_range;          /* 30   (AMCL laser_max_range)                             */
+    uint32_t max_beams;          /* 60   (AMCL laser_max_beams)                             */
+    uint32_t _pad;
+} pfgpu_lfield_config;
+int  pfgpu_pf_lfield_set(pfgpu_pf*, const uint8_t* mask, size_t width, size_t height, const pfgpu_lfield_config* cfg);
+int  pfgpu_pf_lfield_clear(pfgpu_pf*);
+int  pfgpu_pf_lfield_info(pfgpu_pf*, size_t* width, size_t* height, uint64_t* max_used_beams);
+int  pfgpu_pf_lfield_download(pfgpu_pf*, double* D, double* q, size_t cells);
+int  pfgpu_pf_update_scan(pfgpu_pf*, const double* ranges, size_t n_ranges, double angle_min, double angle_inc);
+int  pfgpu_pf_step_scan(pfgpu_pf*, const double u[2], const double* ranges, size_t n_ranges, double angle_min, double angle_inc,
+                        double est[4]);
 
 /* ============================================ FastSLAM 1.0 ========================================== */
 

@@ -41,6 +41,11 @@ class _FsCfg(C.Structure):
                 ("q11", C.c_double), ("r00", C.c_double), ("r11", C.c_double), ("init_weight", C.c_double)]
 
 
+class _LfCfg(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("sigma_hit", C.c_double), ("z_hit", C.c_double), ("z_rand", C.c_double),
+                ("max_range", C.c_double), ("max_beams", C.c_uint32), ("_pad", C.c_uint32)]
+
+
 class _FsObs(C.Structure):
     _fields_ = [("d", C.c_double), ("angle", C.c_double), ("lm_id", C.c_uint64)]
 
@@ -81,6 +86,8 @@ EXPORTS = [
     "pfgpu_fs_history_enable", "pfgpu_fs_history_window", "pfgpu_fs_path", "pfgpu_fs_path_moments",
     "pfgpu_fs_existence_enable", "pfgpu_fs_existence_counts", "pfgpu_fs_existence_removed",
     "pfgpu_pf_recovery_enable", "pfgpu_pf_recovery_state", "pfgpu_pf_init_region",
+    "pfgpu_pf_lfield_set", "pfgpu_pf_lfield_clear", "pfgpu_pf_lfield_info", "pfgpu_pf_lfield_download", "pfgpu_pf_update_scan",
+    "pfgpu_pf_step_scan",
 ]
 
 
@@ -123,6 +130,12 @@ def load_library():
     L.pfgpu_pf_recovery_enable.argtypes = [vp, C.c_double, C.c_double, c_dp]
     L.pfgpu_pf_recovery_state.argtypes = [vp, c_dp, C.POINTER(C.c_uint64)]
     L.pfgpu_pf_init_region.argtypes = [vp, c_dp]
+    L.pfgpu_pf_lfield_set.argtypes = [vp, C.POINTER(C.c_uint8), C.c_size_t, C.c_size_t, C.POINTER(_LfCfg)]
+    L.pfgpu_pf_lfield_clear.argtypes = [vp]
+    L.pfgpu_pf_lfield_info.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]
+    L.pfgpu_pf_lfield_download.argtypes = [vp, c_dp, c_dp, C.c_size_t]
+    L.pfgpu_pf_update_scan.argtypes = [vp, c_dp, C.c_size_t, C.c_double, C.c_double]
+    L.pfgpu_pf_step_scan.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
     L.pfgpu_fs_default_config.argtypes = [C.POINTER(_FsCfg)]
     L.pfgpu_fs_create.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, C.POINTER(vp)]
     L.pfgpu_fs_create_sharded.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, vp, C.c_int,
@@ -392,6 +405,65 @@ class _PfBase:
         f = cls(config, **kw)
         f.init_region(region)
         return f
+
+    # -- likelihood-field scan model (not in the reference, whose MCL only ranges to known landmarks; DESIGN §3.9) --
+    def set_likelihood_field(self, obstacles, resolution, sigma_hit=0.2, z_hit=0.95, z_rand=0.05, max_range=30.0, max_beams=60):
+        """Load an occupancy map for scan updates: obstacles[ix, iy] (W x H, nonzero = obstacle; obstacles_from_log_odds turns an
+        OccupancyGridMap's log-odds into one), `resolution` metres per cell, world (0, 0) at the grid centre.  Builds the distance
+        field and the per-cell likelihood q = z_hit * N(d; 0, sigma_hit) + z_rand / max_range on the device (ROS AMCL's
+        likelihood_field with its defaults).  On a sharded engine every rank makes the same call."""
+        m = np.ascontiguousarray(np.asarray(obstacles) != 0, dtype=np.uint8)
+        if m.ndim != 2:
+            raise InvalidParameter("obstacles: a 2-D (W, H) mask")
+        if not (max_beams >= 2 and max_beams < 2 ** 32):
+            raise InvalidParameter("max_beams >= 2")
+        cfg = _LfCfg(float(resolution), float(sigma_hit), float(z_hit), float(z_rand), float(max_range), int(max_beams), 0)
+        _check(self.L, self.L.pfgpu_pf_lfield_set(self.h, m.ctypes.data_as(C.POINTER(C.c_uint8)), m.shape[0], m.shape[1], C.byref(cfg)))
+
+    def clear_likelihood_field(self):
+        _check(self.L, self.L.pfgpu_pf_lfield_clear(self.h))
+
+    def likelihood_field_info(self):
+        """(W, H, L): the map's shape and the most beams a scan may use (0, 0, 0 without a map)"""
+        W, H, L = C.c_size_t(), C.c_size_t(), C.c_uint64()
+        _check(self.L, self.L.pfgpu_pf_lfield_info(self.h, C.byref(W), C.byref(H), C.byref(L)))
+        return W.value, H.value, L.value
+
+    def likelihood_field(self):
+        """(D, q, L): the distance field in cells and the per-cell likelihood, both (W, H) f64, and the beam limit"""
+        W, H, L = self.likelihood_field_info()
+        if not W:
+            raise InvalidParameter("no likelihood field loaded")
+        D, q = np.empty((W, H)), np.empty((W, H))
+        _check(self.L, self.L.pfgpu_pf_lfield_download(self.h, _dp(D), _dp(q), W * H))
+        return D, q, L
+
+    def try_update_with_scan(self, ranges, angle_min, angle_increment):
+        """The measurement update from a laser scan (ranges[i] at angle_min + i * angle_increment from the heading; the
+        convention of OccupancyGridMap::update_with_scan): every particle's weight becomes the likelihood field of the used beams"""
+        r = _f64(ranges).ravel()
+        _check(self.L, self.L.pfgpu_pf_update_scan(self.h, _dp(r), r.size, float(angle_min), float(angle_increment)))
+
+    update_with_scan = try_update_with_scan
+
+    def try_step_scan(self, control, ranges, angle_min, angle_increment, want_estimate=True):
+        """try_step with a laser scan in place of the landmark observations"""
+        u = control if isinstance(control, np.ndarray) and control.dtype == np.float64 else _f64(control)
+        r = _f64(ranges).ravel()
+        est = np.empty(4)
+        _check(self.L, self.L.pfgpu_pf_step_scan(self.h, _dp(u), _dp(r), r.size, float(angle_min), float(angle_increment),
+                                                 _dp(est) if want_estimate else None))
+        return est if want_estimate else None
+
+    step_scan = try_step_scan
+
+
+def obstacles_from_log_odds(grid, threshold=0.5):
+    """Obstacle mask of an occupancy grid of log-odds l (OccupancyGridMap's grid[ix][iy], rust_robotics_mapping/src/
+    occupancy_grid_map.rs): is_occupied's rule 1 - 1 / (1 + exp(l)) > threshold (:136-159), on the host"""
+    g = np.asarray(grid, dtype=np.float64)
+    with np.errstate(over="ignore"):
+        return (1.0 - 1.0 / (1.0 + np.exp(g))) > threshold
 
 
 class ParticleFilterLocalizer(_PfBase):

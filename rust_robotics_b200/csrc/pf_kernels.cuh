@@ -57,18 +57,51 @@ __device__ __forceinline__ void pose_store(Pose4* p, size_t i, const Pose4& o) {
 // injection arguments of a predict: the region (x0, x1, y0, y1) and whether this is the first predict after a resample stage
 struct PfInj { double r[4]; int arm; };
 
+// Likelihood-field scan model (DESIGN §3.9).  The table q (f64, cell ix * H + iy) is built at set time (pf_lfield.cuh); a scan
+// step reads one cell per used beam.  Lists of up to PF_PARAM_BEAMS (r_i, a_i = i * angle_increment) pairs travel in the launch
+// parameters (the first 48 in the observation block, which a scan does not use, the rest in PfBeamParam), longer ones through d.obs.
+#define PF_PARAM_BEAMS 64
+struct PfBeamParam { double b[2 * PF_PARAM_BEAMS - 3 * PF_PARAM_OBS]; };
+struct PfScan {
+    const double* q = nullptr;
+    double res = 1.0, half_w = 0.0, half_h = 0.0;   // half_w = W as f64 / 2.0 (world_to_grid, occupancy_grid_map.rs:144-153)
+    double q_out = 0.0, angle_min = 0.0;
+    int W = 0, H = 0;
+};
+// Rust's `as i32` of a float: saturating, NaN -> 0
+__device__ __forceinline__ int pf_lf_sat_i32(double v) {
+    if (v != v) return 0;
+    if (v >= 2147483647.0) return 2147483647;
+    if (v <= -2147483648.0) return -2147483647 - 1;
+    return (int)v;
+}
+// the factor of one beam endpoint: q[ix][iy] inside the grid, q_out outside
+__device__ __forceinline__ double pf_lf_factor(const PfScan& sc, const pfc_rcp_t& rres, double ex, double ey) {
+    const int ix = pf_lf_sat_i32(floor(pfc_div_by(ex, rres) + sc.half_w));
+    const int iy = pf_lf_sat_i32(floor(pfc_div_by(ey, rres) + sc.half_h));
+    if (ix < 0 || ix >= sc.W || iy < 0 || iy >= sc.H) return sc.q_out;
+    return __ldg(sc.q + ((size_t)ix * (size_t)sc.H + (size_t)iy));
+}
+
 // try_predict_with_control (pf.rs:279-296, mcl.rs:236-253) and/or the likelihood loop of
 // try_update_with_observations (pf.rs:316-329, mcl.rs:273-283), fused in one pass over the pose records.
 // INJ (augmented MCL): when `inj.arm` and the last resample stage resampled (*d.gate), each slot is first replaced with probability
 // p = scal[PF_REC_P] by a pose drawn uniformly over the region (weight unchanged), then predicted like any other.
-template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false>
+// SCAN: the weight is the likelihood field of k_obs beams (r_i, a_i) instead of the landmark ranges (DESIGN §3.9).
+template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false, bool SCAN = false>
 __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const __grid_constant__ PfObsParam po,
                                                                   double u0, double u1, double sv, double sw,
                                                                   double dt, uint64_t seed, uint32_t call,
-                                                                  int k_obs, double sigma, PfInj inj) {
-    extern __shared__ double s_obs_pf[];     // k_obs x (d, lx, ly): the observation vector staged once per CTA
+                                                                  int k_obs, double sigma, PfInj inj, PfScan sc,
+                                                                  const __grid_constant__ PfBeamParam pb) {
+    extern __shared__ double s_obs_pf[];     // k_obs x (d, lx, ly): the observation vector staged once per CTA; SCAN: k_obs x (r, a)
     if (DO_WEIGHT) {
-        for (int j = threadIdx.x; j < 3 * k_obs; j += PF_NT) s_obs_pf[j] = PARAM_OBS ? po.o[j] : d.obs[j];
+        if constexpr (SCAN) {
+            for (int j = threadIdx.x; j < 2 * k_obs; j += PF_NT)
+                s_obs_pf[j] = PARAM_OBS ? (j < 3 * PF_PARAM_OBS ? po.o[j] : pb.b[j - 3 * PF_PARAM_OBS]) : d.obs[j];
+        } else {
+            for (int j = threadIdx.x; j < 3 * k_obs; j += PF_NT) s_obs_pf[j] = PARAM_OBS ? po.o[j] : d.obs[j];
+        }
         __syncthreads();
     }
     const size_t i = (size_t)blockIdx.x * PF_NT + threadIdx.x;
@@ -107,7 +140,19 @@ __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const
         p.v = v_noisy;                                              // pf.rs:295
         pose_store(pose, i, p);
     }
-    if (DO_WEIGHT) {
+    if constexpr (SCAN) {
+        static_assert(DO_WEIGHT, "a scan is a weight");
+        const pfc_rcp_t rres = pfc_rcp_make(sc.res);                // one reciprocal for every IEEE quotient x / res
+        const double base = p.yaw + sc.angle_min;                   // (yaw + angle_min) + i * angle_increment
+        double w = 1.0;
+        for (int j = 0; j < k_obs; ++j) {
+            const double r = s_obs_pf[2 * j];
+            double s, c;
+            pfc_sincos(base + s_obs_pf[2 * j + 1], &s, &c);
+            w = w * pf_lf_factor(sc, rres, p.x + r * c, p.y + r * s);
+        }
+        d.w_raw[i] = w;
+    } else if (DO_WEIGHT) {
         const double coeff = 1.0 / sqrt(2.0 * PFC_PI * (sigma * sigma));   // gauss_likelihood pf.rs:476-479
         const double denom = 2.0 * (sigma * sigma);
         const pfc_rcp_t rdenom = pfc_rcp_make(denom);               // one reciprocal for all k_obs IEEE quotients

@@ -5,12 +5,14 @@
 #include "pf_kernels.cuh"
 #include "pf3.cuh"
 #include "pf_kld.cuh"
+#include "pf_lfield.cuh"
 #include "xsum_sharded.cuh"
 #include <cstdlib>
 #include <new>
 #include <vector>
 #include <cmath>
 #include <algorithm>
+#include <cfloat>
 
 thread_local char g_pfgpu_err[512] = {0};
 
@@ -145,6 +147,7 @@ struct pfgpu_pf {
         cudaGraphNode_t main_node = nullptr;
         cudaKernelNodeParams main_params = {};
         size_t k = ~(size_t)0;
+        bool scan = false;         // a scan step's graph serves every beam count up to PF_PARAM_BEAMS (k is patched like u)
         uint64_t launches = 0;
         int captures = 0;          // an observation count that keeps changing would re-capture every step: give up after a few
         bool off = false;          // PFGPU_PF_GRAPH=0, capture failed, or too many re-captures: plain launches from then on
@@ -156,6 +159,17 @@ struct pfgpu_pf {
         double a_slow = 0.0, a_fast = 0.0;
         double region[4] = {0.0, 0.0, 0.0, 0.0};     // x0, x1, y0, y1
     } rec;
+    // likelihood-field scan model (DESIGN §3.9): the map's tables and parameters; on = a map is loaded
+    struct LField {
+        bool on = false;
+        size_t W = 0, H = 0;
+        uint64_t L = 0;            // the most used beams a scan may have
+        double* D = nullptr;       // distance field [cells], ix * H + iy
+        double* q = nullptr;       // per-cell factor
+        pfgpu_lfield_config cfg = {};
+        double q_out = 0.0;
+        std::vector<double> pairs; // the used beams of the current call: (r_i, a_i)
+    } lf;
 };
 
 extern "C" void pfgpu_pf_default_config(pfgpu_pf_config* c, int mode) {
@@ -378,6 +392,7 @@ extern "C" void pfgpu_pf_destroy(pfgpu_pf* h) {
     PfDev& d = h->d;
     cudaFree(d.pose[0]); cudaFree(d.pose[1]); cudaFree(d.cur); cudaFree(d.w_raw); cudaFree(d.w); cudaFree(d.cum);
     cudaFree(d.idx); cudaFree(d.scal); cudaFree(d.gate); cudaFree(d.partial); cudaFree(d.obs); cudaFree(h->mom15); cudaFree(d.counters);
+    cudaFree(h->lf.D); cudaFree(h->lf.q);
     if (h->h_pin) cudaFreeHost(h->h_pin);
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
@@ -459,7 +474,55 @@ static int pf_stage_obs(pfgpu_pf* h, const double* obs3, size_t k) {
     if (k > 0) PF_CUDA(cudaMemcpyAsync(h->d.obs, obs3, k * 3 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     return 0;
 }
-static size_t pf_obs_smem(size_t k) { return (k ? k : 1) * 3 * sizeof(double); }
+// The scan model's used beams (DESIGN §3.9) -> h->lf.pairs = (r_i, a_i); *k = their count.  Long lists go to d.obs.
+static int pf_stage_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
+    if (!h->lf.on || (B && !ranges) || !finite_d(angle_min) || !finite_d(angle_inc)) return PFGPU_ERR_INVALID;
+    const pfgpu_lfield_config& c = h->lf.cfg;
+    std::vector<double>& pr = h->lf.pairs;
+    pr.clear();
+    if (B) {
+        const size_t s = std::max<size_t>(1, (B - 1) / (size_t)(c.max_beams - 1));      // AMCL's laser_max_beams stride
+        for (size_t i = 0; i < B; i += s) {
+            const double r = ranges[i];
+            if (r <= 0.0 || !finite_d(r) || r >= c.max_range) continue;                  // occupancy_grid_map.rs:84; AMCL's max range
+            pr.push_back(r);
+            pr.push_back((double)i * angle_inc);
+        }
+    }
+    *k = pr.size() / 2;
+    if (*k > h->lf.L) return PFGPU_ERR_INVALID;
+    if (*k <= PF_PARAM_BEAMS) return 0;
+    if (3 * h->obs_cap < pr.size()) {
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+        cudaFree(h->d.obs);
+        h->obs_cap = *k;
+        PF_CUDA(cudaMalloc(&h->d.obs, h->obs_cap * 3 * sizeof(double)));
+    }
+    PF_CUDA(cudaMemcpyAsync(h->d.obs, pr.data(), pr.size() * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+    return 0;
+}
+static PfScan pf_scan_arg(const pfgpu_pf* h, double angle_min) {
+    PfScan s;
+    s.q = h->lf.q; s.res = h->lf.cfg.resolution;
+    s.half_w = (double)h->lf.W / 2.0; s.half_h = (double)h->lf.H / 2.0;
+    s.q_out = h->lf.q_out; s.angle_min = angle_min;
+    s.W = (int)h->lf.W; s.H = (int)h->lf.H;
+    return s;
+}
+// the launch-parameter form of k <= PF_PARAM_BEAMS used beams: the first pairs in the observation block, the rest in pb
+static void pf_fill_beams(const pfgpu_pf* h, size_t k, PfObsParam& po, PfBeamParam& pb) {
+    for (size_t j = 0; j < 2 * k; ++j) {
+        if (j < 3 * PF_PARAM_OBS) po.o[j] = h->lf.pairs[j];
+        else pb.b[j - 3 * PF_PARAM_OBS] = h->lf.pairs[j];
+    }
+}
+// the smem a weight pass stages: k observations (d, lx, ly), or the beams (r, a) of a scan (a fixed size up to PF_PARAM_BEAMS,
+// so that one captured scan step serves every beam count)
+template <bool SCAN>
+static size_t pf_obs_smem(size_t k) {
+    if (SCAN) return (k <= PF_PARAM_BEAMS ? PF_PARAM_BEAMS : k) * 2 * sizeof(double);
+    return (k ? k : 1) * 3 * sizeof(double);
+}
 
 // the injection arguments of the next predict (augmented MCL, DESIGN §3.8)
 static PfInj pf_inj(const pfgpu_pf* h) {
@@ -467,36 +530,42 @@ static PfInj pf_inj(const pfgpu_pf* h) {
     if (h->rec.on) { for (int j = 0; j < 4; ++j) a.r[j] = h->rec.region[j]; a.arm = h->rec.armed ? 1 : 0; }
     return a;
 }
-template <bool P, bool W, bool INJ>
-static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
-    size_t smem = W ? pf_obs_smem(k) : 0;
-    const bool param = !W || k <= PF_PARAM_OBS;
+// obs: k x (d, lx, ly), or with SCAN the k used beams (r, a) in h->lf.pairs (angle_min: the scan's)
+template <bool P, bool W, bool INJ, bool SCAN>
+static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+    size_t smem = W ? pf_obs_smem<SCAN>(k) : 0;
+    const bool param = !W || k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS);
     PfObsParam po;
-    if (W && param) for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
+    PfBeamParam pb;
+    if (W && param) {
+        if (SCAN) pf_fill_beams(h, k, po, pb);
+        else for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
+    }
     if (smem > 48 * 1024) {
-        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ, SCAN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     const PfInj inj = pf_inj(h);
+    const PfScan sc = SCAN ? pf_scan_arg(h, angle_min) : PfScan{};
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
     if (param)
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true, INJ>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj);
+        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true, INJ, SCAN>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
+                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb);
     else
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false, INJ>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj);
+        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false, INJ, SCAN>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
+                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb);
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     return 0;
 }
-template <bool P, bool W>
-static int pf_launch_main(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
+template <bool P, bool W, bool SCAN = false>
+static int pf_launch_main(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min = 0.0) {
     if constexpr (P) {
         if (h->rec.on) {                                             // every predict counts its injections afresh
             PF_CUDA(cudaMemsetAsync(h->d.counters + PF_REC_COUNT, 0, sizeof(unsigned int), h->ctx.stream));
-            return pf_launch_kernel<P, W, true>(h, u, obs3, k);
+            return pf_launch_kernel<P, W, true, SCAN>(h, u, obs3, k, angle_min);
         }
     }
-    return pf_launch_kernel<P, W, false>(h, u, obs3, k);
+    return pf_launch_kernel<P, W, false, SCAN>(h, u, obs3, k, angle_min);
 }
 // augmented MCL's filter, right after S = sum w_raw has landed in scal[0]
 static int pf_recovery_filter(pfgpu_pf* h) {
@@ -645,9 +714,10 @@ extern "C" int pfgpu_pf_resample(pfgpu_pf* h, int* did) {
     if (did) { int g = 0; rc = pf_read_gate(h, &g); if (rc) return rc; *did = g; }
     return 0;
 }
-// the launches of one fused step, in stream order (what the graph captures)
-static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
-    int rc = pf_launch_main<true, true>(h, u, obs3, k);                              // predict + likelihood, one pass
+// the launches of one fused step, in stream order (what the graph captures).  SCAN: the used beams are in h->lf.pairs.
+template <bool SCAN>
+static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+    int rc = pf_launch_main<true, true, SCAN>(h, u, obs3, k, angle_min);            // predict + likelihood, one pass
     if (rc) return rc;
     if (h->fu.on) {                                                                  // normalise .. refresh_cache: one launch (pf3.cuh)
         h->fu.arg.pd = h->d;
@@ -664,14 +734,15 @@ static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, 
 static void pf_graph_drop(pfgpu_pf* h) {
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
-    h->sg.exec = nullptr; h->sg.graph = nullptr; h->sg.main_node = nullptr; h->sg.k = ~(size_t)0;
+    h->sg.exec = nullptr; h->sg.graph = nullptr; h->sg.main_node = nullptr; h->sg.k = ~(size_t)0; h->sg.scan = false;
 }
-// capture the step at observation count k (no work is executed by the capture itself)
-static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
+// capture the step at observation count k, or a scan step (no work is executed by the capture itself)
+template <bool SCAN>
+static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
     pf_graph_drop(h);
     const uint64_t l0 = h->ctx.launches;
     if (cudaStreamBeginCapture(h->ctx.stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); return 1; }
-    const int rc = pf_step_launches(h, u, obs3, k);
+    const int rc = pf_step_launches<SCAN>(h, u, obs3, k, angle_min);
     cudaGraph_t g = nullptr;
     const cudaError_t e = cudaStreamEndCapture(h->ctx.stream, &g);
     h->sg.launches = h->ctx.launches - l0;
@@ -682,7 +753,8 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
     if (cudaGraphGetNodes(g, nullptr, &nn) != cudaSuccess || nn == 0) { cudaGetLastError(); pf_graph_drop(h); return 1; }
     std::vector<cudaGraphNode_t> nodes(nn);
     if (cudaGraphGetNodes(g, nodes.data(), &nn) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    const void* want = h->rec.on ? (const void*)pf_predict_weight_kernel<true, true, true, true> : (const void*)pf_predict_weight_kernel<true, true, true>;
+    const void* want = h->rec.on ? (const void*)pf_predict_weight_kernel<true, true, true, true, SCAN>
+                                 : (const void*)pf_predict_weight_kernel<true, true, true, false, SCAN>;
     for (cudaGraphNode_t nd : nodes) {
         cudaGraphNodeType ty;
         if (cudaGraphNodeGetType(nd, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
@@ -691,17 +763,21 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
         if (kp.func == want) { h->sg.main_node = nd; h->sg.main_params = kp; break; }
     }
     if (!h->sg.main_node || cudaGraphInstantiate(&h->sg.exec, g, 0) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    h->sg.k = k;
+    h->sg.k = k; h->sg.scan = SCAN;
     return 0;
 }
 // replay with this step's arguments patched into the first kernel
-static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, size_t k) {
+template <bool SCAN>
+static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
     PfObsParam po;
-    for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
+    PfBeamParam pb;
+    if (SCAN) pf_fill_beams(h, k, po, pb);
+    else for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
     double u0 = u[0], u1 = u[1], sv = h->cfg.velocity_noise, sw = h->cfg.yaw_rate_noise, dt = h->cfg.dt, sigma = h->cfg.range_noise;
     uint64_t seed = h->seed; uint32_t call = h->n_predict; int kk = (int)k;
     PfInj inj = pf_inj(h);
-    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma, &inj };
+    PfScan sc = SCAN ? pf_scan_arg(h, angle_min) : PfScan{};
+    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma, &inj, &sc, &pb };
     cudaKernelNodeParams kp = h->sg.main_params;
     kp.kernelParams = args; kp.extra = nullptr;
     PF_CUDA(cudaGraphExecKernelNodeSetParams(h->sg.exec, h->sg.main_node, &kp));
@@ -709,24 +785,23 @@ static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, s
     h->ctx.launches += h->sg.launches;
     return 0;
 }
-
-extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double est[4]) {
-    if (!h || !u || (k && !obs3)) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    int rc = pf_stage_obs(h, obs3, k);
-    if (rc) return rc;
+// try_step once the measurement is staged: landmarks obs3 (k x 3), or with SCAN the k beams in h->lf.pairs
+template <bool SCAN>
+static int pf_step_impl(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min, double est[4]) {
+    int rc = 0;
     // graph replay: fixed particle count, one GPU, observations short enough to ride in the launch parameters, no per-kernel
-    // timing events; the first step of a handle runs plainly (lazy set-up such as function attributes happens there)
-    const bool graphable = !h->sg.off && h->world == 1 && !h->adaptive && k <= PF_PARAM_OBS && !h->timer.on && h->steps > 0;
+    // timing events; the first step of a handle runs plainly (lazy set-up such as function attributes happens there).  The graph
+    // is keyed by the kind of step and, for landmark steps, the observation count
+    const bool graphable = !h->sg.off && h->world == 1 && !h->adaptive && k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS) && !h->timer.on &&
+                           h->steps > 0;
     bool done = false;
     if (graphable) {
-        if (h->sg.exec && h->sg.k == k) done = true;
-        else if (++h->sg.captures <= 16 && pf_graph_capture(h, u, obs3, k) == 0) done = true;
+        if (h->sg.exec && h->sg.scan == SCAN && (SCAN || h->sg.k == k)) done = true;
+        else if (++h->sg.captures <= 16 && pf_graph_capture<SCAN>(h, u, obs3, k, angle_min) == 0) done = true;
         else { h->sg.off = true; pf_graph_drop(h); }
-        if (done) { rc = pf_graph_replay(h, u, obs3, k); if (rc) return rc; }
+        if (done) { rc = pf_graph_replay<SCAN>(h, u, obs3, k, angle_min); if (rc) return rc; }
     }
-    if (!done) { rc = pf_step_launches(h, u, obs3, k); if (rc) return rc; }
+    if (!done) { rc = pf_step_launches<SCAN>(h, u, obs3, k, angle_min); if (rc) return rc; }
     h->fu.last = h->fu.on;
     h->n_predict++;
     h->steps++;
@@ -737,6 +812,14 @@ extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3,
         for (int a = 0; a < 4; ++a) est[a] = h->h_pin[a];
     }
     return 0;
+}
+extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double est[4]) {
+    if (!h || !u || (k && !obs3)) return PFGPU_ERR_INVALID;
+    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    int rc = pf_stage_obs(h, obs3, k);
+    if (rc) return rc;
+    return pf_step_impl<false>(h, u, obs3, k, 0.0, est);
 }
 extern "C" int pfgpu_pf_estimate(pfgpu_pf* h, double est[4], double cov_cm[16]) {
     if (!h) return PFGPU_ERR_INVALID;
@@ -806,6 +889,108 @@ extern "C" int pfgpu_pf_init_region(pfgpu_pf* h, const double region[4]) {
     PF_LAUNCH(h->ctx, pf_init_region_kernel, cdiv_u(h->d.n, PF_NT), PF_NT, 0, h->d, region[0], region[1], region[2], region[3], h->seed);
     if (h->rec.on) { int rc = pf_recovery_reset(h); if (rc) return rc; }
     return pf_refresh_cache(h);
+}
+
+// ---- likelihood-field scan model: localisation in an occupancy grid from a laser scan (DESIGN §3.9) ----
+#define PF_LF_MAX_L 4096           // the beams a scan may use at most (their (r, a) pairs are staged in shared memory)
+// L: the largest count <= PF_LF_MAX_L with q_lo^(L+1) >= DBL_MIN and q_hi^(L+1) <= DBL_MAX, powers by repeated multiplication
+static uint64_t pf_lf_limit(double q_lo, double q_hi) {
+    double pmin = 1.0, pmax = 1.0;
+    uint64_t L = 0;
+    for (uint64_t m = 1; m <= PF_LF_MAX_L + 1; ++m) {
+        pmin = pmin * q_lo;
+        pmax = pmax * q_hi;
+        if (!(pmin >= DBL_MIN) || !(pmax <= DBL_MAX)) break;
+        L = m - 1;
+    }
+    return L;
+}
+static void pf_lf_free(pfgpu_pf* h) {
+    cudaFree(h->lf.D); cudaFree(h->lf.q);
+    h->lf.D = h->lf.q = nullptr;
+    h->lf.on = false; h->lf.W = h->lf.H = 0; h->lf.L = 0;
+}
+struct PfScopedBuf {
+    void* p = nullptr;
+    ~PfScopedBuf() { if (p) cudaFree(p); }
+};
+extern "C" int pfgpu_pf_lfield_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_lfield_config* c) {
+    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
+    if (W < 1 || H < 1 || W > 65536 || H > 65536 || W * H > ((size_t)1 << 28)) return PFGPU_ERR_INVALID;
+    auto positive = [](double v) { return finite_d(v) && v > 0.0; };
+    if (!positive(c->resolution) || !positive(c->sigma_hit) || !positive(c->z_rand) || !positive(c->max_range) || !finite_d(c->z_hit) ||
+        c->z_hit < 0.0 || c->max_beams < 2)
+        return PFGPU_ERR_INVALID;
+    const double q_out = c->z_rand / c->max_range;
+    const double coeff = 1.0 / sqrt(2.0 * PFC_PI * (c->sigma_hit * c->sigma_hit));
+    const uint64_t L = pf_lf_limit(q_out, c->z_hit * coeff + q_out);
+    if (L < 1) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    pf_graph_drop(h);                          // the captured step holds the old table's address
+    pf_lf_free(h);
+    const size_t cells = W * H, scratch = std::max(W * (H + 1), H * (W + 1));
+    PF_CUDA(cudaMalloc(&h->lf.D, cells * sizeof(double)));
+    PF_CUDA(cudaMalloc(&h->lf.q, cells * sizeof(double)));
+    PfScopedBuf m, v, z;
+    PF_CUDA(cudaMalloc(&m.p, cells));
+    PF_CUDA(cudaMalloc(&v.p, scratch * sizeof(int)));
+    PF_CUDA(cudaMalloc(&z.p, scratch * sizeof(double)));
+    PF_CUDA(cudaMemcpyAsync(m.p, mask, cells, cudaMemcpyHostToDevice, h->ctx.stream));
+    // rows into q (as scratch), columns into D, then D = sqrt and the factor table
+    PF_LAUNCH(h->ctx, pf_lf_edt_rows_kernel, cdiv_u(W, 32), 32, 0, (const unsigned char*)m.p, h->lf.q, (int)W, (int)H, (int*)v.p, (double*)z.p);
+    PF_LAUNCH(h->ctx, pf_lf_edt_cols_kernel, cdiv_u(H, 32), 32, 0, h->lf.q, h->lf.D, (int)W, (int)H, (int*)v.p, (double*)z.p);
+    PF_LAUNCH(h->ctx, pf_lf_table_kernel, cdiv_u(cells, 256), 256, 0, h->lf.D, h->lf.q, cells, c->resolution, c->sigma_hit, c->z_hit, q_out);
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    h->lf.W = W; h->lf.H = H; h->lf.L = L; h->lf.cfg = *c; h->lf.q_out = q_out;
+    h->lf.on = true;
+    return 0;
+}
+extern "C" int pfgpu_pf_lfield_clear(pfgpu_pf* h) {
+    if (!h) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    pf_graph_drop(h);
+    pf_lf_free(h);
+    return 0;
+}
+extern "C" int pfgpu_pf_lfield_info(pfgpu_pf* h, size_t* W, size_t* H, uint64_t* L) {
+    if (!h) return PFGPU_ERR_INVALID;
+    if (W) *W = h->lf.W;
+    if (H) *H = h->lf.H;
+    if (L) *L = h->lf.L;
+    return 0;
+}
+extern "C" int pfgpu_pf_lfield_download(pfgpu_pf* h, double* D, double* q, size_t cells) {
+    if (!h || !h->lf.on || cells != h->lf.W * h->lf.H) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    if (D) PF_CUDA(cudaMemcpyAsync(D, h->lf.D, cells * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    if (q) PF_CUDA(cudaMemcpyAsync(q, h->lf.q, cells * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_pf_update_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc) {
+    if (!h) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    size_t k = 0;
+    int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
+    if (rc) return rc;
+    rc = pf_launch_main<false, true, true>(h, nullptr, nullptr, k, angle_min);
+    if (rc) return rc;
+    h->rec.armed = false;                                                            // the weights are no longer uniform
+    rc = pf_normalize(h);
+    if (rc) return rc;
+    return pf_refresh_cache(h);
+}
+extern "C" int pfgpu_pf_step_scan(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
+                                  double est[4]) {
+    if (!h || !u) return PFGPU_ERR_INVALID;
+    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    size_t k = 0;
+    int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
+    if (rc) return rc;
+    return pf_step_impl<true>(h, u, nullptr, k, angle_min, est);
 }
 
 static void timer_drain(KernelTimer& t) {

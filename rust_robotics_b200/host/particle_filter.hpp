@@ -94,6 +94,26 @@ public:
         return {w[0], w[1], w[2], inj};
     }
     void init_region(const Region& region) { check(pfgpu_pf_init_region(h_, region.data()), "initial region"); dirty_ = true; }
+    // likelihood-field scan model (not in the reference; DESIGN §3.9): mask[ix * height + iy], nonzero = obstacle
+    static pfgpu_lfield_config lfield_defaults(double resolution) {                   // ROS AMCL's likelihood_field defaults
+        pfgpu_lfield_config c{};
+        c.resolution = resolution; c.sigma_hit = 0.2; c.z_hit = 0.95; c.z_rand = 0.05; c.max_range = 30.0; c.max_beams = 60;
+        return c;
+    }
+    void set_likelihood_field(const std::vector<uint8_t>& mask, size_t width, size_t height, const pfgpu_lfield_config& c) {
+        if (mask.size() != width * height) throw RoboticsError(RoboticsError::InvalidParameter, "likelihood field: mask size != width * height");
+        check(pfgpu_pf_lfield_set(h_, mask.data(), width, height, &c), "likelihood field");
+    }
+    void clear_likelihood_field() { check(pfgpu_pf_lfield_clear(h_), "likelihood field"); }
+    void try_update_with_scan(const std::vector<double>& ranges, double angle_min, double angle_increment) {
+        check(pfgpu_pf_update_scan(h_, ranges.data(), ranges.size(), angle_min, angle_increment), "scan update"); dirty_ = true;
+    }
+    PFState try_step_scan(const PFControl& u, const std::vector<double>& ranges, double angle_min, double angle_increment) {
+        PFState est{};
+        check(pfgpu_pf_step_scan(h_, u.data(), ranges.data(), ranges.size(), angle_min, angle_increment, est.data()), "scan step");
+        dirty_ = true;
+        return est;
+    }
 };
 }  // namespace detail
 

@@ -50,6 +50,18 @@ pub struct pfgpu_fs_obs {
     pub angle: f64,
     pub lm_id: u64,
 }
+/// the likelihood-field scan model's parameters (pfgpu_pf_lfield_set; ROS AMCL's defaults 0.2, 0.95, 0.05, 30, 60)
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct pfgpu_lfield_config {
+    pub resolution: f64,
+    pub sigma_hit: f64,
+    pub z_hit: f64,
+    pub z_rand: f64,
+    pub max_range: f64,
+    pub max_beams: u32,
+    pub _pad: u32,
+}
 pub enum pfgpu_pf {}
 pub enum pfgpu_fs {}
 
@@ -75,6 +87,13 @@ extern "C" {
     pub fn pfgpu_pf_recovery_enable(h: *mut pfgpu_pf, alpha_slow: f64, alpha_fast: f64, region: *const f64) -> c_int;
     pub fn pfgpu_pf_recovery_state(h: *mut pfgpu_pf, out3: *mut f64, injected_last: *mut u64) -> c_int;
     pub fn pfgpu_pf_init_region(h: *mut pfgpu_pf, region: *const f64) -> c_int;
+    pub fn pfgpu_pf_lfield_set(h: *mut pfgpu_pf, mask: *const u8, width: usize, height: usize, cfg: *const pfgpu_lfield_config) -> c_int;
+    pub fn pfgpu_pf_lfield_clear(h: *mut pfgpu_pf) -> c_int;
+    pub fn pfgpu_pf_lfield_info(h: *mut pfgpu_pf, width: *mut usize, height: *mut usize, max_used_beams: *mut u64) -> c_int;
+    pub fn pfgpu_pf_lfield_download(h: *mut pfgpu_pf, d: *mut f64, q: *mut f64, cells: usize) -> c_int;
+    pub fn pfgpu_pf_update_scan(h: *mut pfgpu_pf, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64) -> c_int;
+    pub fn pfgpu_pf_step_scan(h: *mut pfgpu_pf, u: *const f64, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64,
+                              est: *mut f64) -> c_int;
     pub fn pfgpu_fs_default_config(cfg: *mut pfgpu_fs_config);
     pub fn pfgpu_fs_create(cfg: *const pfgpu_fs_config, n_particles: usize, n_landmarks: usize, seed: u64, device: c_int,
                            out: *mut *mut pfgpu_fs) -> c_int;

@@ -124,6 +124,30 @@ impl ParticleFilterLocalizer {
         s.init_region(region)?;
         Ok(s)
     }
+    /// Likelihood-field scan model (not in the reference; DESIGN §3.9): obstacles[ix * height + iy], nonzero = obstacle; world
+    /// (0, 0) at the grid centre.  Builds the distance field and the per-cell likelihood on the device.
+    pub fn set_likelihood_field(&mut self, obstacles: &[u8], width: usize, height: usize, cfg: &sys::pfgpu_lfield_config) -> RoboticsResult<()> {
+        if obstacles.len() != width * height {
+            return Err(RoboticsError::InvalidParameter("likelihood field: obstacles.len() != width * height".to_string()));
+        }
+        status(unsafe { sys::pfgpu_pf_lfield_set(self.h, obstacles.as_ptr(), width, height, cfg) })
+    }
+    pub fn clear_likelihood_field(&mut self) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_lfield_clear(self.h) })
+    }
+    /// the measurement update from a laser scan: ranges[i] at angle_min + i * angle_increment from the heading
+    pub fn try_update_with_scan(&mut self, ranges: &[f64], angle_min: f64, angle_increment: f64) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_update_scan(self.h, ranges.as_ptr(), ranges.len(), angle_min, angle_increment) })?;
+        self.refresh_cache()
+    }
+    /// try_step with a laser scan in place of the landmark observations
+    pub fn try_step_scan(&mut self, control: &PFControl, ranges: &[f64], angle_min: f64, angle_increment: f64) -> RoboticsResult<PFState> {
+        let mut est = [0.0f64; 4];
+        status(unsafe { sys::pfgpu_pf_step_scan(self.h, control.as_ptr(), ranges.as_ptr(), ranges.len(), angle_min, angle_increment,
+                                                est.as_mut_ptr()) })?;
+        self.refresh_cache()?;
+        Ok(self.state_estimate)
+    }
     pub fn try_predict_with_control(&mut self, control: &PFControl) -> RoboticsResult<()> {      // pf.rs:255-301
         status(unsafe { sys::pfgpu_pf_predict(self.h, control.as_ptr()) })?;
         self.refresh_cache()

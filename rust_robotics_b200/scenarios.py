@@ -153,3 +153,97 @@ class KidnapScenario:
     def error(self, k, est):
         """position error of the estimate after step k [m]"""
         return math.hypot(est[0] - self.truth[k][0], est[1] - self.truth[k][1])
+
+
+def _boxes(mask, res, boxes):
+    """mark the axis-aligned boxes (x0, x1, y0, y1) [m] in a mask whose world (0, 0) is the grid centre"""
+    W, H = mask.shape
+    for x0, x1, y0, y1 in boxes:
+        i0, i1 = int(math.floor(x0 / res + W / 2.0)), int(math.ceil(x1 / res + W / 2.0))
+        j0, j1 = int(math.floor(y0 / res + H / 2.0)), int(math.ceil(y1 / res + H / 2.0))
+        mask[max(i0, 0):max(i1, 0), max(j0, 0):max(j1, 0)] = True
+
+
+class ScanScenario:
+    """A robot with a 360-beam laser in a floor plan (the likelihood-field model, DESIGN §3.9).  The plan is 40 m x 30 m at 5 cm
+    (800 x 600 cells, world (0, 0) at the grid centre): outer walls, four rooms off an open hall, doors and pillars, laid out without
+    symmetry so that global localisation has one answer.  The robot starts at `start` and drives u = (1.0, 0.05) for `steps` steps
+    (dt 0.1).  scans[t] = B = 360 ranges from angle_min = -pi in steps of 1 degree, ray-cast against the mask from the pose
+    truth[t] (no mount offset) every res / 4, plus N(0, range_noise) from numpy's PCG64 `seed`; no obstacle within max_range: inf.
+    cells > 0: the plan centred in a cells x cells grid tiled with copies of it, each copy outside the centre one with an extra
+    pillar of its own (the large maps of bench_scan.py); the scans are the same, since the outer walls are closed."""
+    RES = 0.05
+    REGION = (-19.7, 19.7, -14.7, 14.7)       # the plan's interior: where a lost robot may be
+    B, ANGLE_MIN, ANGLE_INC, MAX_RANGE = 360, -math.pi, math.pi / 180.0, 30.0
+
+    @staticmethod
+    def plan(res=0.05):
+        W, H = int(round(40.0 / res)), int(round(30.0 / res))
+        m = np.zeros((W, H), dtype=bool)
+        t = 0.2                                                         # wall thickness
+        walls = [(-20.0, 20.0, -15.0, -15.0 + t), (-20.0, 20.0, 15.0 - t, 15.0), (-20.0, -20.0 + t, -15.0, 15.0), (20.0 - t, 20.0, -15.0, 15.0),
+                 (-6.0, -6.0 + t, -15.0, -9.0), (-6.0, -6.0 + t, -7.5, 5.0),                     # west rooms, door at y -9 .. -7.5
+                 (-20.0, -14.0, 5.0, 5.0 + t), (-12.5, 2.0, 5.0, 5.0 + t), (3.5, 8.0, 5.0, 5.0 + t),  # north wall, doors
+                 (8.0, 8.0 + t, 5.0, 9.0), (8.0, 8.0 + t, 10.5, 15.0),                           # north-east room
+                 (6.0, 12.0, -6.0, -6.0 + t), (13.5, 20.0, -6.0, -6.0 + t),                      # south-east room
+                 (-20.0, -10.0, -4.0, -4.0 + t), (-8.5, -6.0, -4.0, -4.0 + t),                   # the west rooms' partition
+                 (12.0, 12.0 + t, -15.0, -10.5)]
+        pillars = [(x, x + 0.4, y, y + 0.4) for x, y in ((1.5, -8.0), (-12.0, -10.0), (14.0, 1.0), (3.0, 10.0), (-15.0, 10.0),
+                                                         (16.0, -11.0), (-2.5, 2.0), (5.5, -1.5), (-9.0, 0.0))]
+        _boxes(m, res, walls + pillars)
+        return m
+
+    def __init__(self, steps=60, start=(-3.0, -4.0, 0.3), control=(1.0, 0.05), seed=11, range_noise=0.05, cells=0):
+        base = self.plan(self.RES)
+        self.obstacles = base if not cells else self.tiled(base, cells)
+        self.dt = 0.1
+        rng = np.random.default_rng(seed)
+        t = list(start)
+        self.controls, self.truth, self.scans = [], [], []
+        ang = self.ANGLE_MIN + np.arange(self.B) * self.ANGLE_INC
+        ds = np.arange(1, int(self.MAX_RANGE / (self.RES / 4.0)) + 1) * (self.RES / 4.0)
+        W, H = base.shape
+        for _ in range(steps):
+            t[0] += control[0] * math.cos(t[2]) * self.dt
+            t[1] += control[0] * math.sin(t[2]) * self.dt
+            t[2] += control[1] * self.dt
+            ex = t[0] + np.cos(t[2] + ang)[:, None] * ds[None, :]
+            ey = t[1] + np.sin(t[2] + ang)[:, None] * ds[None, :]
+            ix, iy = np.floor(ex / self.RES + W / 2.0).astype(np.int64), np.floor(ey / self.RES + H / 2.0).astype(np.int64)
+            inside = (ix >= 0) & (ix < W) & (iy >= 0) & (iy < H)
+            hit = inside & base[np.clip(ix, 0, W - 1), np.clip(iy, 0, H - 1)]
+            first = np.where(hit.any(axis=1), hit.argmax(axis=1), -1)
+            r = np.where(first >= 0, ds[first] + rng.normal(0.0, range_noise, self.B), np.inf)
+            self.controls.append(tuple(control))
+            self.truth.append(list(t))
+            self.scans.append(np.ascontiguousarray(r))
+        assert not any(base[int(math.floor(x / self.RES + W / 2.0)), int(math.floor(y / self.RES + H / 2.0))] for x, y, _ in self.truth)
+        self.region = self.REGION if not cells else (-cells * self.RES / 2.0, cells * self.RES / 2.0) * 2
+
+    @staticmethod
+    def tiled(base, cells):
+        W, H = base.shape
+        ix = (np.arange(cells) - cells // 2 + W // 2) % W
+        iy = (np.arange(cells) - cells // 2 + H // 2) % H
+        m = base[ix[:, None], iy[None, :]]
+        tx = (np.arange(cells) - cells // 2 + W // 2) // W                # the copy each cell belongs to
+        ty = (np.arange(cells) - cells // 2 + H // 2) // H
+        for a in np.unique(tx):
+            for b in np.unique(ty):
+                if a == 0 and b == 0:
+                    continue
+                ca, cb = np.flatnonzero(tx == a), np.flatnonzero(ty == b)
+                px, py = int((a * 7919 + b * 104729) % max(W - 100, 1)) + 50, int((a * 6271 + b * 3571) % max(H - 100, 1)) + 50
+                sx, sy = ca[(ca - ca[0] >= px) & (ca - ca[0] < px + 8)], cb[(cb - cb[0] >= py) & (cb - cb[0] < py + 8)]
+                m[np.ix_(sx, sy)] = True
+        return m
+
+    def scan_args(self, t):
+        """(ranges, angle_min, angle_inc) of step t"""
+        return self.scans[t], self.ANGLE_MIN, self.ANGLE_INC
+
+    def error(self, k, est):
+        """(position error [m], heading error [rad], wrapped) of the estimate after step k"""
+        return (math.hypot(est[0] - self.truth[k][0], est[1] - self.truth[k][1]),
+                abs(normalize_angle(est[2] - self.truth[k][2])))
+
