@@ -158,6 +158,37 @@ int  pfgpu_pf_lfield_download(pfgpu_pf*, double* D, double* q, size_t cells);
 int  pfgpu_pf_update_scan(pfgpu_pf*, const double* ranges, size_t n_ranges, double angle_min, double angle_inc);
 int  pfgpu_pf_step_scan(pfgpu_pf*, const double u[2], const double* ranges, size_t n_ranges, double angle_min, double angle_inc,
                         double est[4]);
+/* Pose hypotheses: the particle cloud clustered in a fixed (x, y, yaw) histogram, each cluster's weight, mean and covariance (not in
+ * the reference; ROS AMCL's pose hypotheses; DESIGN §3.10).  A query: no step computes anything differently or launches more.
+ *   set        the particles and weights pfgpu_pf_estimate describes and pfgpu_pf_download returns (after a step, before any
+ *              injection); KLD-adaptive MCL: the current generation; sharded: the global set in rank order (global slot indices).
+ *   member     x, y, yaw and v finite and 0 < w < inf.  Other particles belong to no cluster.
+ *   bin        r = xy_res, K = yaw_bins, T = PFC_TWO_PI (2 pi rounded to f64): kx = floor(x / r) and ky = floor(y / r) as i32 (Rust's
+ *              saturating cast), theta = yaw - T * floor(yaw / T) (two rounded operations, no fused multiply-add),
+ *              kt = floor(theta / (T / K)) clamped to [0, K - 1].  Single IEEE operations: the same bins in CUDA, C and Python.
+ *   adjacency  two occupied bins (holding a member) with |dkx| <= 1, |dky| <= 1 and dkt in {-1, 0, 1} mod K: 26-connectivity, cyclic
+ *              in yaw, not in x / y; neighbour keys beyond the i32 range do not exist.
+ *   cluster    a connected component of occupied bins and the members in them: mass M = sum w, count, bins, label = the smallest
+ *              global slot among its members, mean x, y, v = sum w (x, y, v) / M and yaw = atan2(sum w sin yaw, sum w cos yaw) (the
+ *              contract math; 0 when both sums are 0), cov = sum (w / M) d d^T with d = (x - mean x, y - mean y, wrap(yaw - mean yaw),
+ *              v - mean v), wrap(a) = a - T * floor((a + pi) / T) into [-pi, pi), column-major like pfgpu_pf_estimate's.
+ *   order      mass descending, ties by ascending label.
+ *   bits       the same particle set gives the same bits on every call, and a sharded engine gives on every rank the bits a single
+ *              GPU holding the same global set gives (every rank clusters the gathered set).  No floating-point atomics.
+ * pfgpu_pf_hypotheses: out = the first min(cap, total) clusters in that order; *n_total (nullable) = the number of clusters;
+ *   rank_of_slot (nullable, n_local entries) = each local slot's cluster rank, UINT32_MAX for a non-member.  xy_res not positive and
+ *   finite, yaw_bins 0 or above 65536, or cap > 0 with out NULL: PFGPU_ERR_INVALID; more than 2^31 - 1 particles:
+ *   PFGPU_ERR_UNSUPPORTED.  No member: zero clusters.  Synchronises;
+ *   collective on a sharded engine.  The workspace is allocated on the first call (DESIGN §3.10 gives its size); when that fails the
+ *   call returns PFGPU_ERR_CUDA and the handle stays usable.  The captured step graph is kept. */
+typedef struct {
+    double   mass;
+    double   mean[4];      /* x, y, circular-mean yaw in (-pi, pi], v */
+    double   cov[16];      /* column-major, over (x, y, wrapped yaw deviation, v) */
+    uint64_t count, bins, label;
+} pfgpu_pf_hypothesis;
+int  pfgpu_pf_hypotheses(pfgpu_pf*, double xy_res, uint32_t yaw_bins, pfgpu_pf_hypothesis* out, size_t cap, size_t* n_total,
+                         uint32_t* rank_of_slot);
 
 /* ============================================ FastSLAM 1.0 ========================================== */
 

@@ -46,6 +46,11 @@ class _LfCfg(C.Structure):
                 ("max_range", C.c_double), ("max_beams", C.c_uint32), ("_pad", C.c_uint32)]
 
 
+class _Hyp(C.Structure):
+    _fields_ = [("mass", C.c_double), ("mean", C.c_double * 4), ("cov", C.c_double * 16), ("count", C.c_uint64),
+                ("bins", C.c_uint64), ("label", C.c_uint64)]
+
+
 class _FsObs(C.Structure):
     _fields_ = [("d", C.c_double), ("angle", C.c_double), ("lm_id", C.c_uint64)]
 
@@ -68,6 +73,9 @@ FsEstimate = collections.namedtuple("FsEstimate", ["pose", "pose_cov", "mass", "
 FsPath = collections.namedtuple("FsPath", ["steps", "slots", "poses"])
 # FastSlam1.path_estimate(): steps (L,), pose (L, 3) weighted mean of the lineage poses, pose_cov (L, 3, 3); oldest first
 FsPathEstimate = collections.namedtuple("FsPathEstimate", ["steps", "pose", "pose_cov"])
+# _PfBase.hypotheses(): one cluster of the particle cloud: weight (its mass), count, bins, label (smallest global slot), mean (4,) =
+# (x, y, circular-mean yaw, v), cov (4, 4) over (x, y, wrapped yaw deviation, v)
+PfHypothesis = collections.namedtuple("PfHypothesis", ["weight", "count", "bins", "label", "mean", "cov"])
 
 
 EXPORTS = [
@@ -87,7 +95,7 @@ EXPORTS = [
     "pfgpu_fs_existence_enable", "pfgpu_fs_existence_counts", "pfgpu_fs_existence_removed",
     "pfgpu_pf_recovery_enable", "pfgpu_pf_recovery_state", "pfgpu_pf_init_region",
     "pfgpu_pf_lfield_set", "pfgpu_pf_lfield_clear", "pfgpu_pf_lfield_info", "pfgpu_pf_lfield_download", "pfgpu_pf_update_scan",
-    "pfgpu_pf_step_scan",
+    "pfgpu_pf_step_scan", "pfgpu_pf_hypotheses",
 ]
 
 
@@ -136,6 +144,7 @@ def load_library():
     L.pfgpu_pf_lfield_download.argtypes = [vp, c_dp, c_dp, C.c_size_t]
     L.pfgpu_pf_update_scan.argtypes = [vp, c_dp, C.c_size_t, C.c_double, C.c_double]
     L.pfgpu_pf_step_scan.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
+    L.pfgpu_pf_hypotheses.argtypes = [vp, C.c_double, C.c_uint32, C.POINTER(_Hyp), C.c_size_t, C.POINTER(C.c_size_t), c_u32p]
     L.pfgpu_fs_default_config.argtypes = [C.POINTER(_FsCfg)]
     L.pfgpu_fs_create.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, C.POINTER(vp)]
     L.pfgpu_fs_create_sharded.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, vp, C.c_int,
@@ -456,6 +465,27 @@ class _PfBase:
         return est if want_estimate else None
 
     step_scan = try_step_scan
+
+    # -- pose hypotheses (not in the reference; ROS AMCL's pose hypotheses; DESIGN §3.10) --
+    def hypotheses(self, max_count=16, xy_res=0.5, yaw_bins=24, labels=False):
+        """The particle cloud clustered in a fixed histogram of xy_res x xy_res x (2 pi / yaw_bins) bins (26-connected, cyclic in yaw):
+        ([PfHypothesis] of the max_count heaviest clusters, heaviest first, total number of clusters), and with labels=True also an
+        int64 rank per local particle (-1: not a member: a non-finite pose or a weight not in (0, inf)).  The set estimate() describes;
+        the same bits on every call.  Synchronises; on a sharded engine every rank makes the same call and gets the same clusters."""
+        if not (max_count >= 0 and yaw_bins >= 0 and yaw_bins < 2 ** 32):
+            raise InvalidParameter("max_count >= 0, 0 < yaw_bins <= 65536")
+        out = (_Hyp * max(int(max_count), 1))()
+        total = C.c_size_t()
+        rk = np.empty(self.particle_count(local=True), dtype=np.uint32) if labels else None
+        _check(self.L, self.L.pfgpu_pf_hypotheses(self.h, float(xy_res), int(yaw_bins), out, int(max_count), C.byref(total),
+                                                  rk.ctypes.data_as(c_u32p) if labels else None))
+        hs = [PfHypothesis(out[i].mass, int(out[i].count), int(out[i].bins), int(out[i].label), np.array(out[i].mean[:]),
+                           np.array(out[i].cov[:]).reshape(4, 4).T) for i in range(min(int(max_count), total.value))]
+        if not labels:
+            return hs, total.value
+        r = rk.astype(np.int64)
+        r[rk == 0xFFFFFFFF] = -1
+        return hs, total.value, r
 
 
 def obstacles_from_log_odds(grid, threshold=0.5):

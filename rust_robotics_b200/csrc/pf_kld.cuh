@@ -54,19 +54,41 @@ __global__ void __launch_bounds__(PF_NT) pf_kld_draw_kernel(PfDev d, uint64_t se
     k.keys[2 * k.cap + t] = pf_sat_i32(floor(p.yaw / YAW_BIN));
 }
 
+// The open-addressing bin hash set shared by the KLD resample and the pose hypotheses (pf_cluster.cuh).  keys = [3][cap]
+// (x, y, yaw bin of item t at t, cap + t, 2 cap + t); owner[tcap] = an item that carries the slot's key, -1 = empty; tcap is a power
+// of two at least twice the number of distinct keys, so a probe always meets an empty slot.
+__device__ __forceinline__ unsigned pf_bin_hash(int a, int b, int c) {
+    const unsigned long long h = (unsigned long long)(unsigned)a * 0x9E3779B97F4A7C15ull ^ (unsigned long long)(unsigned)b * 0xC2B2AE3D27D4EB4Full ^
+                                 (unsigned long long)(unsigned)c * 0x165667B19E3779F9ull;
+    return (unsigned)(h >> 17);
+}
+// insert item t with key (a, b, c); returns the slot that stands for the key
+__device__ __forceinline__ unsigned pf_bin_insert(int* owner, unsigned tcap, const int* keys, size_t cap, size_t t, int a, int b, int c) {
+    unsigned i = pf_bin_hash(a, b, c) & (tcap - 1);
+    for (;;) {
+        int o = atomicCAS(&owner[i], -1, (int)t);
+        if (o == -1) break;                                    // the slot is mine: it now stands for my key
+        if (keys[o] == a && keys[cap + o] == b && keys[2 * cap + o] == c) break;   // same bin
+        i = (i + 1) & (tcap - 1);                              // another bin lives here (the table is never more than half full)
+    }
+    return i;
+}
+// the slot of key (a, b, c), -1 when no item carries it (the insertions have completed)
+__device__ __forceinline__ int pf_bin_find(const int* owner, unsigned tcap, const int* keys, size_t cap, int a, int b, int c) {
+    unsigned i = pf_bin_hash(a, b, c) & (tcap - 1);
+    for (;;) {
+        const int o = owner[i];
+        if (o == -1) return -1;
+        if (keys[o] == a && keys[cap + o] == b && keys[2 * cap + o] == c) return (int)i;
+        i = (i + 1) & (tcap - 1);
+    }
+}
+
 __global__ void __launch_bounds__(PF_NT) pf_kld_insert_kernel(PfKld k) {
     const size_t t = (size_t)blockIdx.x * PF_NT + threadIdx.x;
     if (t >= k.cap) return;
     const int a = k.keys[t], b = k.keys[k.cap + t], c = k.keys[2 * k.cap + t];
-    const unsigned long long h = (unsigned long long)(unsigned)a * 0x9E3779B97F4A7C15ull ^ (unsigned long long)(unsigned)b * 0xC2B2AE3D27D4EB4Full ^
-                                 (unsigned long long)(unsigned)c * 0x165667B19E3779F9ull;
-    unsigned i = (unsigned)(h >> 17) & (k.tcap - 1);
-    for (;;) {
-        int o = atomicCAS(&k.owner[i], -1, (int)t);
-        if (o == -1) break;                                    // the slot is mine: it now stands for my key
-        if (k.keys[o] == a && k.keys[k.cap + o] == b && k.keys[2 * k.cap + o] == c) break;   // same bin
-        i = (i + 1) & (k.tcap - 1);                            // another bin lives here (the table is never more than half full)
-    }
+    const unsigned i = pf_bin_insert(k.owner, k.tcap, k.keys, k.cap, t, a, b, c);
     atomicMin(&k.mint[i], (unsigned)t);
     k.slot[t] = (int)i;
 }

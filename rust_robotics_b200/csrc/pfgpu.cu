@@ -6,6 +6,7 @@
 #include "pf3.cuh"
 #include "pf_kld.cuh"
 #include "pf_lfield.cuh"
+#include "pf_cluster.cuh"
 #include "xsum_sharded.cuh"
 #include <cstdlib>
 #include <new>
@@ -170,6 +171,7 @@ struct pfgpu_pf {
         double q_out = 0.0;
         std::vector<double> pairs; // the used beams of the current call: (r_i, a_i)
     } lf;
+    PfClu clu;                     // pose hypotheses' workspace (DESIGN §3.10), allocated by the first query
 };
 
 extern "C" void pfgpu_pf_default_config(pfgpu_pf_config* c, int mode) {
@@ -398,6 +400,7 @@ extern "C" void pfgpu_pf_destroy(pfgpu_pf* h) {
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
     pf3_free(h);
     cudaFree(h->kld.keys); cudaFree(h->kld.owner); cudaFree(h->kld.mint); cudaFree(h->kld.slot); cudaFree(h->kld.n_new);
+    pf_clu_free(h->clu);
     {
         FsShard& sh = h->sh;
         cudaFree(sh.t_loc); cudaFree(sh.t_all); cudaFree(sh.approx_off); cudaFree(sh.sum_loc); cudaFree(sh.sum_all); cudaFree(sh.s_start);
@@ -991,6 +994,73 @@ extern "C" int pfgpu_pf_step_scan(pfgpu_pf* h, const double u[2], const double* 
     int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
     if (rc) return rc;
     return pf_step_impl<true>(h, u, nullptr, k, angle_min, est);
+}
+
+// ---- pose hypotheses: the cloud clustered in a fixed (x, y, yaw) histogram (DESIGN §3.10, pf_cluster.cuh) ----
+extern "C" int pfgpu_pf_hypotheses(pfgpu_pf* h, double xy_res, uint32_t yaw_bins, pfgpu_pf_hypothesis* out, size_t cap, size_t* n_total,
+                                   uint32_t* rank_of_slot) {
+    if (!h || !finite_d(xy_res) || !(xy_res > 0.0) || yaw_bins == 0 || yaw_bins > 65536 || (cap > 0 && !out)) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PfDev& d = h->d; PfClu& c = h->clu; Ctx& ctx = h->ctx;
+    const size_t most = h->adaptive ? (size_t)h->cfg.max_particles : (size_t)d.n_global;     // the largest global set
+    if (most > 0x7FFFFFFFull) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "pose hypotheses: more than 2^31 - 1 particles");
+        return PFGPU_ERR_UNSUPPORTED;
+    }
+    if (!c.keys) { int rc = pf_clu_alloc(c, most, h->world > 1); if (rc) return rc; }
+    const size_t N = d.n_global;
+    const Pose4* P_all = nullptr;
+    const double* W_all = nullptr;
+    if (h->world > 1) {                                  // every rank clusters the global set in rank order
+        PF_NCCL(ncclAllGather(d.pose[h->cur_host], h->sh.pose_all, 4 * d.n, ncclDouble, h->sh.comm, ctx.stream));
+        PF_NCCL(ncclAllGather(d.w, c.w_all, d.n, ncclDouble, h->sh.comm, ctx.stream));
+        P_all = reinterpret_cast<const Pose4*>(h->sh.pose_all); W_all = c.w_all;
+    }
+    PF_CUDA(cudaMemsetAsync(c.owner, 0xFF, (size_t)c.tcap * sizeof(int), ctx.stream));
+    PF_CUDA(cudaMemsetAsync(c.mint, 0xFF, (size_t)c.tcap * sizeof(unsigned), ctx.stream));
+    PF_CUDA(cudaMemsetAsync(c.parent, 0xFF, (size_t)c.tcap * sizeof(int), ctx.stream));
+    const double bw = PFC_TWO_PI / (double)yaw_bins;
+    PF_LAUNCH(ctx, pf_clu_key_kernel, cdiv_u(N, PF_NT), PF_NT, 0, d, P_all, W_all, N, c, xy_res, bw, (int)yaw_bins);
+    PF_LAUNCH(ctx, pf_clu_insert_kernel, cdiv_u(N, PF_NT), PF_NT, 0, c, N);
+    PF_LAUNCH(ctx, pf_clu_link_kernel, cdiv_u(c.tcap, PF_NT), PF_NT, 0, c, (int)yaw_bins);
+    PF_LAUNCH(ctx, pf_clu_label_kernel, cdiv_u(N, PF_NT), PF_NT, 0, c, N);
+    int bits = 1;
+    while (((size_t)1 << bits) <= N) ++bits;             // labels are <= N (N: not a member)
+    size_t tb = c.tmp_bytes;
+    PF_CUDA(cub::DeviceRadixSort::SortPairs(c.tmp, tb, c.lab, c.lab_s, c.iota, c.perm, (int)N, 0, bits, ctx.stream));
+    tb = c.tmp_bytes;
+    PF_CUDA(cub::DeviceRunLengthEncode::Encode(c.tmp, tb, c.lab_s, c.uniq, c.cnt, c.scal, (int)N, ctx.stream));
+    PF_LAUNCH(ctx, pf_clu_count_kernel, 1, 1, 0, c, N);
+    unsigned* hp = reinterpret_cast<unsigned*>(h->h_pin + 50);
+    PF_CUDA(cudaMemcpyAsync(hp, c.scal + 1, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(ctx.stream));          // the launches below are sized by the number of clusters
+    const unsigned nc = *hp;
+    const unsigned m = (unsigned)std::min<size_t>(cap, nc);
+    if (nc > 0) {
+        tb = c.tmp_bytes;
+        PF_CUDA(cub::DeviceScan::ExclusiveSum(c.tmp, tb, c.cnt, c.off, (int)nc, ctx.stream));
+        PF_LAUNCH(ctx, pf_clu_ntiles_kernel, cdiv_u(nc, PF_NT), PF_NT, 0, c, nc);
+        tb = c.tmp_bytes;
+        PF_CUDA(cub::DeviceScan::ExclusiveSum(c.tmp, tb, c.rank, c.toff, (int)nc, ctx.stream));
+        const size_t warps_per_cta = PF_NT / 32, tiles_max = N / PF_CLU_TILE + nc;
+        const unsigned g_tile = (unsigned)std::min<size_t>(cdiv_u(tiles_max, warps_per_cta), (size_t)ctx.num_sms * 16);
+        const unsigned g_clu = (unsigned)std::min<size_t>(cdiv_u(nc, warps_per_cta), (size_t)ctx.num_sms * 16);
+        PF_LAUNCH(ctx, pf_clu_tile_kernel<1>, g_tile, PF_NT, 0, d, P_all, W_all, c, nc, rank_of_slot ? 1 : 0);
+        PF_LAUNCH(ctx, pf_clu_final_kernel<1>, g_clu, PF_NT, 0, c, nc);
+        PF_LAUNCH(ctx, pf_clu_tile_kernel<2>, g_tile, PF_NT, 0, d, P_all, W_all, c, nc, 0);
+        PF_LAUNCH(ctx, pf_clu_final_kernel<2>, g_clu, PF_NT, 0, c, nc);
+        tb = c.tmp_bytes;
+        PF_CUDA(cub::DeviceRadixSort::SortPairs(c.tmp, tb, c.mkey, c.mkey_s, c.iota, c.order, (int)nc, 0, 64, ctx.stream));
+        PF_LAUNCH(ctx, pf_clu_rank_kernel, cdiv_u(nc, PF_NT), PF_NT, 0, c, nc, m);
+        if (m) PF_CUDA(cudaMemcpyAsync(out, c.part, (size_t)m * sizeof(pfgpu_pf_hypothesis), cudaMemcpyDeviceToHost, ctx.stream));
+    }
+    if (rank_of_slot) {
+        PF_LAUNCH(ctx, pf_clu_slot_rank_kernel, cdiv_u(d.n, PF_NT), PF_NT, 0, c, d.offset, d.n, nc);
+        PF_CUDA(cudaMemcpyAsync(rank_of_slot, c.lab, d.n * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx.stream));
+    }
+    PF_CUDA(cudaStreamSynchronize(ctx.stream));
+    if (n_total) *n_total = nc;
+    return 0;
 }
 
 static void timer_drain(KernelTimer& t) {

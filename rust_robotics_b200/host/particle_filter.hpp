@@ -114,6 +114,20 @@ public:
         dirty_ = true;
         return est;
     }
+    // pose hypotheses (not in the reference; ROS AMCL's pose hypotheses; DESIGN §3.10): the max_count heaviest clusters of the
+    // cloud in xy_res x xy_res x (2 pi / yaw_bins) bins, heaviest first; *total = the number of clusters; rank_of_slot (when given)
+    // = each local particle's cluster rank, UINT32_MAX for a non-member
+    std::vector<pfgpu_pf_hypothesis> hypotheses(size_t max_count = 16, double xy_res = 0.5, uint32_t yaw_bins = 24, size_t* total = nullptr,
+                                                std::vector<uint32_t>* rank_of_slot = nullptr) const {
+        std::vector<pfgpu_pf_hypothesis> out(max_count);
+        size_t n = 0, nl = 0, ng = 0;
+        if (rank_of_slot) { check(pfgpu_pf_count(h_, &nl, &ng), "count"); rank_of_slot->resize(nl); }
+        check(pfgpu_pf_hypotheses(h_, xy_res, yaw_bins, out.data(), max_count, &n, rank_of_slot ? rank_of_slot->data() : nullptr),
+              "hypotheses");
+        out.resize(n < max_count ? n : max_count);
+        if (total) *total = n;
+        return out;
+    }
 };
 }  // namespace detail
 

@@ -62,6 +62,17 @@ pub struct pfgpu_lfield_config {
     pub max_beams: u32,
     pub _pad: u32,
 }
+/// one cluster of the particle cloud (pfgpu_pf_hypotheses): mass, mean (x, y, circular-mean yaw, v), column-major covariance
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct pfgpu_pf_hypothesis {
+    pub mass: f64,
+    pub mean: [f64; 4],
+    pub cov: [f64; 16],
+    pub count: u64,
+    pub bins: u64,
+    pub label: u64,
+}
 pub enum pfgpu_pf {}
 pub enum pfgpu_fs {}
 
@@ -94,6 +105,8 @@ extern "C" {
     pub fn pfgpu_pf_update_scan(h: *mut pfgpu_pf, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64) -> c_int;
     pub fn pfgpu_pf_step_scan(h: *mut pfgpu_pf, u: *const f64, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64,
                               est: *mut f64) -> c_int;
+    pub fn pfgpu_pf_hypotheses(h: *mut pfgpu_pf, xy_res: f64, yaw_bins: u32, out: *mut pfgpu_pf_hypothesis, cap: usize,
+                               n_total: *mut usize, rank_of_slot: *mut u32) -> c_int;
     pub fn pfgpu_fs_default_config(cfg: *mut pfgpu_fs_config);
     pub fn pfgpu_fs_create(cfg: *const pfgpu_fs_config, n_particles: usize, n_landmarks: usize, seed: u64, device: c_int,
                            out: *mut *mut pfgpu_fs) -> c_int;

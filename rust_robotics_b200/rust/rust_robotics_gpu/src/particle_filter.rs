@@ -148,6 +148,15 @@ impl ParticleFilterLocalizer {
         self.refresh_cache()?;
         Ok(self.state_estimate)
     }
+    /// Pose hypotheses (not in the reference; ROS AMCL's pose hypotheses; DESIGN §3.10): the max_count heaviest clusters of the cloud
+    /// in xy_res x xy_res x (2 pi / yaw_bins) bins, heaviest first, and the total number of clusters
+    pub fn hypotheses(&self, max_count: usize, xy_res: f64, yaw_bins: u32) -> RoboticsResult<(Vec<sys::pfgpu_pf_hypothesis>, usize)> {
+        let mut out = vec![sys::pfgpu_pf_hypothesis { mass: 0.0, mean: [0.0; 4], cov: [0.0; 16], count: 0, bins: 0, label: 0 }; max_count];
+        let mut total = 0usize;
+        status(unsafe { sys::pfgpu_pf_hypotheses(self.h, xy_res, yaw_bins, out.as_mut_ptr(), max_count, &mut total, std::ptr::null_mut()) })?;
+        out.truncate(total.min(max_count));
+        Ok((out, total))
+    }
     pub fn try_predict_with_control(&mut self, control: &PFControl) -> RoboticsResult<()> {      // pf.rs:255-301
         status(unsafe { sys::pfgpu_pf_predict(self.h, control.as_ptr()) })?;
         self.refresh_cache()

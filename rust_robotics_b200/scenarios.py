@@ -171,7 +171,9 @@ class ScanScenario:
     (dt 0.1).  scans[t] = B = 360 ranges from angle_min = -pi in steps of 1 degree, ray-cast against the mask from the pose
     truth[t] (no mount offset) every res / 4, plus N(0, range_noise) from numpy's PCG64 `seed`; no obstacle within max_range: inf.
     cells > 0: the plan centred in a cells x cells grid tiled with copies of it, each copy outside the centre one with an extra
-    pillar of its own (the large maps of bench_scan.py); the scans are the same, since the outer walls are closed."""
+    pillar of its own (the large maps of bench_scan.py); the scans are the same, since the outer walls are closed.
+    symmetric: the plan united with its point mirror (plan | plan[::-1, ::-1]), so that a pose (x, y, yaw) and its mirror
+    (-x, -y, yaw + pi) see the same scan: a localisation problem with two answers (the pose hypotheses, DESIGN §3.10)."""
     RES = 0.05
     REGION = (-19.7, 19.7, -14.7, 14.7)       # the plan's interior: where a lost robot may be
     B, ANGLE_MIN, ANGLE_INC, MAX_RANGE = 360, -math.pi, math.pi / 180.0, 30.0
@@ -193,10 +195,13 @@ class ScanScenario:
         _boxes(m, res, walls + pillars)
         return m
 
-    def __init__(self, steps=60, start=(-3.0, -4.0, 0.3), control=(1.0, 0.05), seed=11, range_noise=0.05, cells=0):
+    def __init__(self, steps=60, start=(-3.0, -4.0, 0.3), control=(1.0, 0.05), seed=11, range_noise=0.05, cells=0, symmetric=False):
         base = self.plan(self.RES)
+        if symmetric:
+            base = base | base[::-1, ::-1]
         self.obstacles = base if not cells else self.tiled(base, cells)
         self.dt = 0.1
+        self.start = tuple(start)
         rng = np.random.default_rng(seed)
         t = list(start)
         self.controls, self.truth, self.scans = [], [], []
