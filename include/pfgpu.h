@@ -189,6 +189,55 @@ typedef struct {
 } pfgpu_pf_hypothesis;
 int  pfgpu_pf_hypotheses(pfgpu_pf*, double xy_res, uint32_t yaw_bins, pfgpu_pf_hypothesis* out, size_t cap, size_t* n_total,
                          uint32_t* rank_of_slot);
+/* The beam measurement model: every particle's expected range along every used beam is ray-cast in the occupancy grid and compared
+ * with the measured one (not in the reference; Probabilistic Robotics Table 6.1, ROS AMCL's laser_model_type beam; DESIGN §3.11).
+ *   map        the likelihood field's conventions unchanged (mask[ix * H + iy], limits, world_to_grid with the saturating cast).  The
+ *              beam map is separate state: a handle may hold both maps, and each step uses the model its entry point names.
+ *   clearance  per cell, the Chebyshev (L-infinity) distance in cells to the nearest cell that is occupied or outside the grid, capped
+ *              at 255 (0 = occupied); built on the device at set time.
+ *   ray        pose (x, y, yaw), beam i: angle = (yaw + angle_min) + a_i, a_i = i as f64 * angle_inc; c0 = world_to_grid(x, y),
+ *              c1 = world_to_grid(x + max_range * cos(angle), y + max_range * sin(angle)) (one sincos).  The cells are those of
+ *              bresenham_line(c0, c1) (rust_robotics_mapping/src/occupancy_grid_map.rs:164-193, both ends included).  The first cell
+ *              occupied or outside the grid stops the ray: r_hat = res * sqrt((f64)(dx * dx + dy * dy)), (dx, dy) its integer offset
+ *              from c0, the sum of squares in int64.  No such cell up to and including c1: r_hat = max_range.  c0 occupied or outside:
+ *              r_hat = 0.  max_range / res <= 2^20 keeps every integer product exact.
+ *   beams      candidates i = 0, s, 2s, .. < B, s = max(1, (B - 1) / (max_beams - 1)); NaN or r <= 0: unused; r >= max_range (+inf
+ *              included) is a max reading, used only when z_max > 0 and then scored with r = max_range.
+ *   factor     per used beam, z = r - r_hat, coeff = 1 / sqrt(2 pi * (sigma_hit * sigma_hit)), in this order:
+ *                q = (z_hit * coeff) * exp(-(z * z) / (2 * (sigma_hit * sigma_hit)))
+ *                if z < 0:  q = q + (z_short * lambda_short) * exp(-(lambda_short * r))      (AMCL's short term, unnormalised)
+ *                q = q + (max reading ? z_max : z_rand / max_range)
+ *              w = w * q over the used beams in ascending i from w = 1; w overwrites w_raw.  The rest of the update and of the step is
+ *              the landmark path's.
+ *   bound      the likelihood field's rule with q_lo = z_rand / max_range (min(that, z_max) when z_max > 0) and
+ *              q_hi = z_hit * coeff + z_short * lambda_short + max(z_rand / max_range, z_max).  More than L used beams:
+ *              PFGPU_ERR_INVALID, so every w_raw is a positive normal number.
+ * pfgpu_pf_beam_set: res, sigma_hit, z_rand, max_range, lambda_short positive and finite; z_hit, z_short, z_max >= 0 and finite;
+ *   max_beams >= 2; max_range / res <= 2^20; L >= 1; else PFGPU_ERR_INVALID.  Replaces any beam map, builds the clearance on the
+ *   device and synchronises.  On a sharded engine every rank makes the same call.  pfgpu_pf_beam_clear frees it.
+ * pfgpu_pf_beam_info: W, H and L (all 0 without a beam map).  pfgpu_pf_beam_download: the clearance bytes, cells = W * H.
+ * pfgpu_pf_update_beam / pfgpu_pf_step_beam: pfgpu_pf_update_scan / pfgpu_pf_step_scan with the beam model and the same refusals.
+ * pfgpu_pf_beam_raycast: r_hat of n poses (x, y, yaw) x B beams at angle_min + b * angle_inc into out[p * B + b]; needs a beam map. */
+typedef struct {
+    double   resolution;         /* metres per cell                                         */
+    double   sigma_hit;          /* 0.2  (AMCL laser_sigma_hit)                             */
+    double   z_hit;              /* 0.95 (AMCL laser_z_hit)                                 */
+    double   z_short;            /* 0.1  (AMCL laser_z_short)                               */
+    double   z_max;              /* 0.05 (AMCL laser_z_max)                                 */
+    double   z_rand;             /* 0.05 (AMCL laser_z_rand)                                */
+    double   lambda_short;       /* 0.1  (AMCL laser_lambda_short)                          */
+    double   max_range;          /* 30   (AMCL laser_max_range)                             */
+    uint32_t max_beams;          /* 60   (AMCL laser_max_beams)                             */
+    uint32_t _pad;
+} pfgpu_beam_config;
+int  pfgpu_pf_beam_set(pfgpu_pf*, const uint8_t* mask, size_t width, size_t height, const pfgpu_beam_config* cfg);
+int  pfgpu_pf_beam_clear(pfgpu_pf*);
+int  pfgpu_pf_beam_info(pfgpu_pf*, size_t* width, size_t* height, uint64_t* max_used_beams);
+int  pfgpu_pf_beam_download(pfgpu_pf*, uint8_t* clearance, size_t cells);
+int  pfgpu_pf_update_beam(pfgpu_pf*, const double* ranges, size_t n_ranges, double angle_min, double angle_inc);
+int  pfgpu_pf_step_beam(pfgpu_pf*, const double u[2], const double* ranges, size_t n_ranges, double angle_min, double angle_inc,
+                        double est[4]);
+int  pfgpu_pf_beam_raycast(pfgpu_pf*, const double* poses3, size_t n, size_t n_beams, double angle_min, double angle_inc, double* out);
 
 /* ============================================ FastSLAM 1.0 ========================================== */
 

@@ -46,6 +46,12 @@ class _LfCfg(C.Structure):
                 ("max_range", C.c_double), ("max_beams", C.c_uint32), ("_pad", C.c_uint32)]
 
 
+class _BmCfg(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("sigma_hit", C.c_double), ("z_hit", C.c_double), ("z_short", C.c_double),
+                ("z_max", C.c_double), ("z_rand", C.c_double), ("lambda_short", C.c_double), ("max_range", C.c_double),
+                ("max_beams", C.c_uint32), ("_pad", C.c_uint32)]
+
+
 class _Hyp(C.Structure):
     _fields_ = [("mass", C.c_double), ("mean", C.c_double * 4), ("cov", C.c_double * 16), ("count", C.c_uint64),
                 ("bins", C.c_uint64), ("label", C.c_uint64)]
@@ -96,6 +102,8 @@ EXPORTS = [
     "pfgpu_pf_recovery_enable", "pfgpu_pf_recovery_state", "pfgpu_pf_init_region",
     "pfgpu_pf_lfield_set", "pfgpu_pf_lfield_clear", "pfgpu_pf_lfield_info", "pfgpu_pf_lfield_download", "pfgpu_pf_update_scan",
     "pfgpu_pf_step_scan", "pfgpu_pf_hypotheses",
+    "pfgpu_pf_beam_set", "pfgpu_pf_beam_clear", "pfgpu_pf_beam_info", "pfgpu_pf_beam_download", "pfgpu_pf_update_beam",
+    "pfgpu_pf_step_beam", "pfgpu_pf_beam_raycast",
 ]
 
 
@@ -145,6 +153,13 @@ def load_library():
     L.pfgpu_pf_update_scan.argtypes = [vp, c_dp, C.c_size_t, C.c_double, C.c_double]
     L.pfgpu_pf_step_scan.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
     L.pfgpu_pf_hypotheses.argtypes = [vp, C.c_double, C.c_uint32, C.POINTER(_Hyp), C.c_size_t, C.POINTER(C.c_size_t), c_u32p]
+    L.pfgpu_pf_beam_set.argtypes = [vp, C.POINTER(C.c_uint8), C.c_size_t, C.c_size_t, C.POINTER(_BmCfg)]
+    L.pfgpu_pf_beam_clear.argtypes = [vp]
+    L.pfgpu_pf_beam_info.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]
+    L.pfgpu_pf_beam_download.argtypes = [vp, C.POINTER(C.c_uint8), C.c_size_t]
+    L.pfgpu_pf_update_beam.argtypes = [vp, c_dp, C.c_size_t, C.c_double, C.c_double]
+    L.pfgpu_pf_step_beam.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
+    L.pfgpu_pf_beam_raycast.argtypes = [vp, c_dp, C.c_size_t, C.c_size_t, C.c_double, C.c_double, c_dp]
     L.pfgpu_fs_default_config.argtypes = [C.POINTER(_FsCfg)]
     L.pfgpu_fs_create.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, C.POINTER(vp)]
     L.pfgpu_fs_create_sharded.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, vp, C.c_int,
@@ -465,6 +480,69 @@ class _PfBase:
         return est if want_estimate else None
 
     step_scan = try_step_scan
+
+    # -- beam scan model (not in the reference; Probabilistic Robotics Table 6.1, ROS AMCL's beam model; DESIGN §3.11) --
+    def set_beam_model(self, obstacles, resolution, sigma_hit=0.2, z_hit=0.95, z_short=0.1, z_max=0.05, z_rand=0.05, lambda_short=0.1,
+                       max_range=30.0, max_beams=60):
+        """Load an occupancy map for beam-model scan updates (the likelihood field's conventions: obstacles[ix, iy], W x H, nonzero =
+        obstacle, `resolution` metres per cell, world (0, 0) at the grid centre).  Every particle's expected range along every used
+        beam is ray-cast in the map and compared with the measured one (ROS AMCL's beam model with its defaults).  Builds the
+        clearance table on the device.  Separate from the likelihood field; on a sharded engine every rank makes the same call."""
+        m = np.ascontiguousarray(np.asarray(obstacles) != 0, dtype=np.uint8)
+        if m.ndim != 2:
+            raise InvalidParameter("obstacles: a 2-D (W, H) mask")
+        if not (max_beams >= 2 and max_beams < 2 ** 32):
+            raise InvalidParameter("max_beams >= 2")
+        cfg = _BmCfg(float(resolution), float(sigma_hit), float(z_hit), float(z_short), float(z_max), float(z_rand), float(lambda_short),
+                     float(max_range), int(max_beams), 0)
+        _check(self.L, self.L.pfgpu_pf_beam_set(self.h, m.ctypes.data_as(C.POINTER(C.c_uint8)), m.shape[0], m.shape[1], C.byref(cfg)))
+
+    def clear_beam_model(self):
+        _check(self.L, self.L.pfgpu_pf_beam_clear(self.h))
+
+    def beam_model_info(self):
+        """(W, H, L): the beam map's shape and the most beams a scan may use (0, 0, 0 without one)"""
+        W, H, L = C.c_size_t(), C.c_size_t(), C.c_uint64()
+        _check(self.L, self.L.pfgpu_pf_beam_info(self.h, C.byref(W), C.byref(H), C.byref(L)))
+        return W.value, H.value, L.value
+
+    def beam_model(self):
+        """the clearance table, (W, H) uint8: Chebyshev distance in cells to the nearest occupied or outside cell, capped at 255"""
+        W, H, _ = self.beam_model_info()
+        if not W:
+            raise InvalidParameter("no beam model loaded")
+        out = np.empty((W, H), dtype=np.uint8)
+        _check(self.L, self.L.pfgpu_pf_beam_download(self.h, out.ctypes.data_as(C.POINTER(C.c_uint8)), W * H))
+        return out
+
+    def try_update_with_beam_scan(self, ranges, angle_min, angle_increment):
+        """try_update_with_scan under the beam model"""
+        r = _f64(ranges).ravel()
+        _check(self.L, self.L.pfgpu_pf_update_beam(self.h, _dp(r), r.size, float(angle_min), float(angle_increment)))
+
+    update_with_beam_scan = try_update_with_beam_scan
+
+    def try_step_beam_scan(self, control, ranges, angle_min, angle_increment, want_estimate=True):
+        """try_step with a laser scan under the beam model"""
+        u = control if isinstance(control, np.ndarray) and control.dtype == np.float64 else _f64(control)
+        r = _f64(ranges).ravel()
+        est = np.empty(4)
+        _check(self.L, self.L.pfgpu_pf_step_beam(self.h, _dp(u), _dp(r), r.size, float(angle_min), float(angle_increment),
+                                                 _dp(est) if want_estimate else None))
+        return est if want_estimate else None
+
+    step_beam_scan = try_step_beam_scan
+
+    def expected_scan(self, poses, n_beams, angle_min, angle_increment):
+        """(n, n_beams) expected ranges of poses (n, 3) = (x, y, yaw) in the beam map, ray-cast on the device: beam b at
+        (yaw + angle_min) + b * angle_increment; 0 from a pose in an obstacle or outside the grid, max_range when nothing is hit"""
+        p = np.ascontiguousarray(_f64(poses).reshape(-1, 3))
+        B = int(n_beams)
+        if B < 0:
+            raise InvalidParameter("n_beams >= 0")
+        out = np.empty((p.shape[0], B))
+        _check(self.L, self.L.pfgpu_pf_beam_raycast(self.h, _dp(p), p.shape[0], B, float(angle_min), float(angle_increment), _dp(out)))
+        return out
 
     # -- pose hypotheses (not in the reference; ROS AMCL's pose hypotheses; DESIGN §3.10) --
     def hypotheses(self, max_count=16, xy_res=0.5, yaw_bins=24, labels=False):

@@ -82,18 +82,20 @@ __device__ __forceinline__ double pf_lf_factor(const PfScan& sc, const pfc_rcp_t
     if (ix < 0 || ix >= sc.W || iy < 0 || iy >= sc.H) return sc.q_out;
     return __ldg(sc.q + ((size_t)ix * (size_t)sc.H + (size_t)iy));
 }
+#include "pf_beam.cuh"              // the beam model (DESIGN §3.11): PfBeam, the ray caster and the factor
 
 // try_predict_with_control (pf.rs:279-296, mcl.rs:236-253) and/or the likelihood loop of
 // try_update_with_observations (pf.rs:316-329, mcl.rs:273-283), fused in one pass over the pose records.
 // INJ (augmented MCL): when `inj.arm` and the last resample stage resampled (*d.gate), each slot is first replaced with probability
 // p = scal[PF_REC_P] by a pose drawn uniformly over the region (weight unchanged), then predicted like any other.
 // SCAN: the weight is the likelihood field of k_obs beams (r_i, a_i) instead of the landmark ranges (DESIGN §3.9).
-template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false, bool SCAN = false>
+// SCAN and BEAM: the weight is the beam model of those beams instead (ray-cast in the clearance table bm, DESIGN §3.11).
+template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false, bool SCAN = false, bool BEAM = false>
 __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const __grid_constant__ PfObsParam po,
                                                                   double u0, double u1, double sv, double sw,
                                                                   double dt, uint64_t seed, uint32_t call,
                                                                   int k_obs, double sigma, PfInj inj, PfScan sc,
-                                                                  const __grid_constant__ PfBeamParam pb) {
+                                                                  const __grid_constant__ PfBeamParam pb, PfBeam bm) {
     extern __shared__ double s_obs_pf[];     // k_obs x (d, lx, ly): the observation vector staged once per CTA; SCAN: k_obs x (r, a)
     if (DO_WEIGHT) {
         if constexpr (SCAN) {
@@ -140,7 +142,19 @@ __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const
         p.v = v_noisy;                                              // pf.rs:295
         pose_store(pose, i, p);
     }
-    if constexpr (SCAN) {
+    if constexpr (SCAN && BEAM) {
+        static_assert(DO_WEIGHT, "a scan is a weight");
+        const pfc_rcp_t rres = pfc_rcp_make(bm.res), rdenom = pfc_rcp_make(bm.denom);
+        const double base = p.yaw + bm.angle_min;                   // (yaw + angle_min) + i * angle_increment
+        int ix0, iy0;
+        pf_beam_start(bm, rres, p.x, p.y, &ix0, &iy0);
+        double w = 1.0;
+        for (int j = 0; j < k_obs; ++j) {
+            const double rhat = pf_beam_cast(bm, rres, p.x, p.y, ix0, iy0, base + s_obs_pf[2 * j + 1]);
+            w = w * pf_beam_factor(bm, rdenom, s_obs_pf[2 * j], rhat);
+        }
+        d.w_raw[i] = w;
+    } else if constexpr (SCAN) {
         static_assert(DO_WEIGHT, "a scan is a weight");
         const pfc_rcp_t rres = pfc_rcp_make(sc.res);                // one reciprocal for every IEEE quotient x / res
         const double base = p.yaw + sc.angle_min;                   // (yaw + angle_min) + i * angle_increment

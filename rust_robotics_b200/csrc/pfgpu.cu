@@ -17,6 +17,11 @@
 
 thread_local char g_pfgpu_err[512] = {0};
 
+// the measurement model of a weight pass: landmark ranges, the likelihood field (DESIGN §3.9) or the beam model (DESIGN §3.11)
+#define PF_KIND_LM 0
+#define PF_KIND_LF 1
+#define PF_KIND_BEAM 2
+
 extern "C" const char* pfgpu_last_error(void) { return g_pfgpu_err; }
 extern "C" const char* pfgpu_strerror(int s) {
     switch (s) {
@@ -148,7 +153,7 @@ struct pfgpu_pf {
         cudaGraphNode_t main_node = nullptr;
         cudaKernelNodeParams main_params = {};
         size_t k = ~(size_t)0;
-        bool scan = false;         // a scan step's graph serves every beam count up to PF_PARAM_BEAMS (k is patched like u)
+        int kind = PF_KIND_LM;     // a scan step's graph (either model) serves every beam count up to PF_PARAM_BEAMS (k is patched like u)
         uint64_t launches = 0;
         int captures = 0;          // an observation count that keeps changing would re-capture every step: give up after a few
         bool off = false;          // PFGPU_PF_GRAPH=0, capture failed, or too many re-captures: plain launches from then on
@@ -169,8 +174,17 @@ struct pfgpu_pf {
         double* q = nullptr;       // per-cell factor
         pfgpu_lfield_config cfg = {};
         double q_out = 0.0;
-        std::vector<double> pairs; // the used beams of the current call: (r_i, a_i)
     } lf;
+    // beam model (DESIGN §3.11): the clearance table and parameters; on = a map is loaded.  Separate from the likelihood field's.
+    struct BeamMap {
+        bool on = false;
+        size_t W = 0, H = 0;
+        uint64_t L = 0;            // the most used beams a scan may have
+        unsigned char* clr = nullptr;   // clearance [cells], ix * H + iy
+        pfgpu_beam_config cfg = {};
+        int skip = 1;              // PFGPU_BEAM_SKIP=0 at set time: the caster steps one cell at a time
+    } bm;
+    std::vector<double> pairs;     // the used beams of the current scan call (either model): (r_i, a_i)
     PfClu clu;                     // pose hypotheses' workspace (DESIGN §3.10), allocated by the first query
 };
 
@@ -394,7 +408,7 @@ extern "C" void pfgpu_pf_destroy(pfgpu_pf* h) {
     PfDev& d = h->d;
     cudaFree(d.pose[0]); cudaFree(d.pose[1]); cudaFree(d.cur); cudaFree(d.w_raw); cudaFree(d.w); cudaFree(d.cum);
     cudaFree(d.idx); cudaFree(d.scal); cudaFree(d.gate); cudaFree(d.partial); cudaFree(d.obs); cudaFree(h->mom15); cudaFree(d.counters);
-    cudaFree(h->lf.D); cudaFree(h->lf.q);
+    cudaFree(h->lf.D); cudaFree(h->lf.q); cudaFree(h->bm.clr);
     if (h->h_pin) cudaFreeHost(h->h_pin);
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
@@ -477,23 +491,29 @@ static int pf_stage_obs(pfgpu_pf* h, const double* obs3, size_t k) {
     if (k > 0) PF_CUDA(cudaMemcpyAsync(h->d.obs, obs3, k * 3 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     return 0;
 }
-// The scan model's used beams (DESIGN §3.9) -> h->lf.pairs = (r_i, a_i); *k = their count.  Long lists go to d.obs.
-static int pf_stage_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
-    if (!h->lf.on || (B && !ranges) || !finite_d(angle_min) || !finite_d(angle_inc)) return PFGPU_ERR_INVALID;
-    const pfgpu_lfield_config& c = h->lf.cfg;
-    std::vector<double>& pr = h->lf.pairs;
+// A scan's used beams -> h->pairs = (r_i, a_i); *k = their count.  Long lists go to d.obs.  Candidates i = 0, s, 2s, .. (AMCL's
+// laser_max_beams stride); NaN or r <= 0 is unused (occupancy_grid_map.rs:84); r >= max_range is a max reading: unused, or with
+// keep_max (the beam model with z_max > 0) used as r = max_range.
+static int pf_stage_pairs(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, uint32_t max_beams,
+                          double max_range, bool keep_max, uint64_t L, size_t* k) {
+    if ((B && !ranges) || !finite_d(angle_min) || !finite_d(angle_inc)) return PFGPU_ERR_INVALID;
+    std::vector<double>& pr = h->pairs;
     pr.clear();
     if (B) {
-        const size_t s = std::max<size_t>(1, (B - 1) / (size_t)(c.max_beams - 1));      // AMCL's laser_max_beams stride
+        const size_t s = std::max<size_t>(1, (B - 1) / (size_t)(max_beams - 1));
         for (size_t i = 0; i < B; i += s) {
-            const double r = ranges[i];
-            if (r <= 0.0 || !finite_d(r) || r >= c.max_range) continue;                  // occupancy_grid_map.rs:84; AMCL's max range
+            double r = ranges[i];
+            if (r != r || r <= 0.0) continue;
+            if (r >= max_range) {
+                if (!keep_max) continue;
+                r = max_range;
+            }
             pr.push_back(r);
             pr.push_back((double)i * angle_inc);
         }
     }
     *k = pr.size() / 2;
-    if (*k > h->lf.L) return PFGPU_ERR_INVALID;
+    if (*k > L) return PFGPU_ERR_INVALID;
     if (*k <= PF_PARAM_BEAMS) return 0;
     if (3 * h->obs_cap < pr.size()) {
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
@@ -504,6 +524,17 @@ static int pf_stage_scan(pfgpu_pf* h, const double* ranges, size_t B, double ang
     PF_CUDA(cudaMemcpyAsync(h->d.obs, pr.data(), pr.size() * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     return 0;
 }
+// the likelihood field's used beams (DESIGN §3.9)
+static int pf_stage_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
+    if (!h->lf.on) return PFGPU_ERR_INVALID;
+    return pf_stage_pairs(h, ranges, B, angle_min, angle_inc, h->lf.cfg.max_beams, h->lf.cfg.max_range, false, h->lf.L, k);
+}
+// the beam model's used beams (DESIGN §3.11): max readings count when z_max > 0
+static int pf_stage_beam(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
+    if (!h->bm.on) return PFGPU_ERR_INVALID;
+    const pfgpu_beam_config& c = h->bm.cfg;
+    return pf_stage_pairs(h, ranges, B, angle_min, angle_inc, c.max_beams, c.max_range, c.z_max > 0.0, h->bm.L, k);
+}
 static PfScan pf_scan_arg(const pfgpu_pf* h, double angle_min) {
     PfScan s;
     s.q = h->lf.q; s.res = h->lf.cfg.resolution;
@@ -512,11 +543,24 @@ static PfScan pf_scan_arg(const pfgpu_pf* h, double angle_min) {
     s.W = (int)h->lf.W; s.H = (int)h->lf.H;
     return s;
 }
+static PfBeam pf_beam_arg(const pfgpu_pf* h, double angle_min) {
+    const pfgpu_beam_config& c = h->bm.cfg;
+    PfBeam b;
+    b.clr = h->bm.clr; b.res = c.resolution;
+    b.half_w = (double)h->bm.W / 2.0; b.half_h = (double)h->bm.H / 2.0;
+    b.max_range = c.max_range; b.angle_min = angle_min;
+    b.hit = c.z_hit * (1.0 / sqrt(2.0 * PFC_PI * (c.sigma_hit * c.sigma_hit)));
+    b.denom = 2.0 * (c.sigma_hit * c.sigma_hit);
+    b.shrt = c.z_short * c.lambda_short; b.lambda = c.lambda_short;
+    b.q_rand = c.z_rand / c.max_range; b.z_max = c.z_max;
+    b.W = (int)h->bm.W; b.H = (int)h->bm.H; b.skip = h->bm.skip;
+    return b;
+}
 // the launch-parameter form of k <= PF_PARAM_BEAMS used beams: the first pairs in the observation block, the rest in pb
 static void pf_fill_beams(const pfgpu_pf* h, size_t k, PfObsParam& po, PfBeamParam& pb) {
     for (size_t j = 0; j < 2 * k; ++j) {
-        if (j < 3 * PF_PARAM_OBS) po.o[j] = h->lf.pairs[j];
-        else pb.b[j - 3 * PF_PARAM_OBS] = h->lf.pairs[j];
+        if (j < 3 * PF_PARAM_OBS) po.o[j] = h->pairs[j];
+        else pb.b[j - 3 * PF_PARAM_OBS] = h->pairs[j];
     }
 }
 // the smem a weight pass stages: k observations (d, lx, ly), or the beams (r, a) of a scan (a fixed size up to PF_PARAM_BEAMS,
@@ -533,9 +577,10 @@ static PfInj pf_inj(const pfgpu_pf* h) {
     if (h->rec.on) { for (int j = 0; j < 4; ++j) a.r[j] = h->rec.region[j]; a.arm = h->rec.armed ? 1 : 0; }
     return a;
 }
-// obs: k x (d, lx, ly), or with SCAN the k used beams (r, a) in h->lf.pairs (angle_min: the scan's)
-template <bool P, bool W, bool INJ, bool SCAN>
+// obs: k x (d, lx, ly), or for a scan (KIND != PF_KIND_LM) the k used beams (r, a) in h->pairs (angle_min: the scan's)
+template <bool P, bool W, bool INJ, int KIND>
 static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+    constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
     size_t smem = W ? pf_obs_smem<SCAN>(k) : 0;
     const bool param = !W || k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS);
     PfObsParam po;
@@ -545,30 +590,31 @@ static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, 
         else for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
     }
     if (smem > 48 * 1024) {
-        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ, SCAN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     const PfInj inj = pf_inj(h);
-    const PfScan sc = SCAN ? pf_scan_arg(h, angle_min) : PfScan{};
+    const PfScan sc = KIND == PF_KIND_LF ? pf_scan_arg(h, angle_min) : PfScan{};
+    const PfBeam bm = BEAM ? pf_beam_arg(h, angle_min) : PfBeam{};
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
     if (param)
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true, INJ, SCAN>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb);
+        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true, INJ, SCAN, BEAM>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
+                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb, bm);
     else
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false, INJ, SCAN>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb);
+        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
+                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb, bm);
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     return 0;
 }
-template <bool P, bool W, bool SCAN = false>
+template <bool P, bool W, int KIND = PF_KIND_LM>
 static int pf_launch_main(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min = 0.0) {
     if constexpr (P) {
         if (h->rec.on) {                                             // every predict counts its injections afresh
             PF_CUDA(cudaMemsetAsync(h->d.counters + PF_REC_COUNT, 0, sizeof(unsigned int), h->ctx.stream));
-            return pf_launch_kernel<P, W, true, SCAN>(h, u, obs3, k, angle_min);
+            return pf_launch_kernel<P, W, true, KIND>(h, u, obs3, k, angle_min);
         }
     }
-    return pf_launch_kernel<P, W, false, SCAN>(h, u, obs3, k, angle_min);
+    return pf_launch_kernel<P, W, false, KIND>(h, u, obs3, k, angle_min);
 }
 // augmented MCL's filter, right after S = sum w_raw has landed in scal[0]
 static int pf_recovery_filter(pfgpu_pf* h) {
@@ -717,10 +763,10 @@ extern "C" int pfgpu_pf_resample(pfgpu_pf* h, int* did) {
     if (did) { int g = 0; rc = pf_read_gate(h, &g); if (rc) return rc; *did = g; }
     return 0;
 }
-// the launches of one fused step, in stream order (what the graph captures).  SCAN: the used beams are in h->lf.pairs.
-template <bool SCAN>
+// the launches of one fused step, in stream order (what the graph captures).  A scan's used beams are in h->pairs.
+template <int KIND>
 static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
-    int rc = pf_launch_main<true, true, SCAN>(h, u, obs3, k, angle_min);            // predict + likelihood, one pass
+    int rc = pf_launch_main<true, true, KIND>(h, u, obs3, k, angle_min);            // predict + likelihood, one pass
     if (rc) return rc;
     if (h->fu.on) {                                                                  // normalise .. refresh_cache: one launch (pf3.cuh)
         h->fu.arg.pd = h->d;
@@ -737,15 +783,15 @@ static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, 
 static void pf_graph_drop(pfgpu_pf* h) {
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
-    h->sg.exec = nullptr; h->sg.graph = nullptr; h->sg.main_node = nullptr; h->sg.k = ~(size_t)0; h->sg.scan = false;
+    h->sg.exec = nullptr; h->sg.graph = nullptr; h->sg.main_node = nullptr; h->sg.k = ~(size_t)0; h->sg.kind = PF_KIND_LM;
 }
-// capture the step at observation count k, or a scan step (no work is executed by the capture itself)
-template <bool SCAN>
+// capture the step at observation count k, or a scan step of either model (no work is executed by the capture itself)
+template <int KIND>
 static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
     pf_graph_drop(h);
     const uint64_t l0 = h->ctx.launches;
     if (cudaStreamBeginCapture(h->ctx.stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); return 1; }
-    const int rc = pf_step_launches<SCAN>(h, u, obs3, k, angle_min);
+    const int rc = pf_step_launches<KIND>(h, u, obs3, k, angle_min);
     cudaGraph_t g = nullptr;
     const cudaError_t e = cudaStreamEndCapture(h->ctx.stream, &g);
     h->sg.launches = h->ctx.launches - l0;
@@ -756,8 +802,9 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
     if (cudaGraphGetNodes(g, nullptr, &nn) != cudaSuccess || nn == 0) { cudaGetLastError(); pf_graph_drop(h); return 1; }
     std::vector<cudaGraphNode_t> nodes(nn);
     if (cudaGraphGetNodes(g, nodes.data(), &nn) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    const void* want = h->rec.on ? (const void*)pf_predict_weight_kernel<true, true, true, true, SCAN>
-                                 : (const void*)pf_predict_weight_kernel<true, true, true, false, SCAN>;
+    constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
+    const void* want = h->rec.on ? (const void*)pf_predict_weight_kernel<true, true, true, true, SCAN, BEAM>
+                                 : (const void*)pf_predict_weight_kernel<true, true, true, false, SCAN, BEAM>;
     for (cudaGraphNode_t nd : nodes) {
         cudaGraphNodeType ty;
         if (cudaGraphNodeGetType(nd, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
@@ -766,21 +813,22 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
         if (kp.func == want) { h->sg.main_node = nd; h->sg.main_params = kp; break; }
     }
     if (!h->sg.main_node || cudaGraphInstantiate(&h->sg.exec, g, 0) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    h->sg.k = k; h->sg.scan = SCAN;
+    h->sg.k = k; h->sg.kind = KIND;
     return 0;
 }
 // replay with this step's arguments patched into the first kernel
-template <bool SCAN>
+template <int KIND>
 static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
     PfObsParam po;
     PfBeamParam pb;
-    if (SCAN) pf_fill_beams(h, k, po, pb);
+    if (KIND != PF_KIND_LM) pf_fill_beams(h, k, po, pb);
     else for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
     double u0 = u[0], u1 = u[1], sv = h->cfg.velocity_noise, sw = h->cfg.yaw_rate_noise, dt = h->cfg.dt, sigma = h->cfg.range_noise;
     uint64_t seed = h->seed; uint32_t call = h->n_predict; int kk = (int)k;
     PfInj inj = pf_inj(h);
-    PfScan sc = SCAN ? pf_scan_arg(h, angle_min) : PfScan{};
-    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma, &inj, &sc, &pb };
+    PfScan sc = KIND == PF_KIND_LF ? pf_scan_arg(h, angle_min) : PfScan{};
+    PfBeam bm = KIND == PF_KIND_BEAM ? pf_beam_arg(h, angle_min) : PfBeam{};
+    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma, &inj, &sc, &pb, &bm };
     cudaKernelNodeParams kp = h->sg.main_params;
     kp.kernelParams = args; kp.extra = nullptr;
     PF_CUDA(cudaGraphExecKernelNodeSetParams(h->sg.exec, h->sg.main_node, &kp));
@@ -788,23 +836,24 @@ static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, s
     h->ctx.launches += h->sg.launches;
     return 0;
 }
-// try_step once the measurement is staged: landmarks obs3 (k x 3), or with SCAN the k beams in h->lf.pairs
-template <bool SCAN>
+// try_step once the measurement is staged: landmarks obs3 (k x 3), or for a scan the k beams in h->pairs
+template <int KIND>
 static int pf_step_impl(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min, double est[4]) {
     int rc = 0;
     // graph replay: fixed particle count, one GPU, observations short enough to ride in the launch parameters, no per-kernel
     // timing events; the first step of a handle runs plainly (lazy set-up such as function attributes happens there).  The graph
-    // is keyed by the kind of step and, for landmark steps, the observation count
+    // is keyed by the kind of step (landmark / likelihood field / beam) and, for landmark steps, the observation count
+    constexpr bool SCAN = KIND != PF_KIND_LM;
     const bool graphable = !h->sg.off && h->world == 1 && !h->adaptive && k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS) && !h->timer.on &&
                            h->steps > 0;
     bool done = false;
     if (graphable) {
-        if (h->sg.exec && h->sg.scan == SCAN && (SCAN || h->sg.k == k)) done = true;
-        else if (++h->sg.captures <= 16 && pf_graph_capture<SCAN>(h, u, obs3, k, angle_min) == 0) done = true;
+        if (h->sg.exec && h->sg.kind == KIND && (SCAN || h->sg.k == k)) done = true;
+        else if (++h->sg.captures <= 16 && pf_graph_capture<KIND>(h, u, obs3, k, angle_min) == 0) done = true;
         else { h->sg.off = true; pf_graph_drop(h); }
-        if (done) { rc = pf_graph_replay<SCAN>(h, u, obs3, k, angle_min); if (rc) return rc; }
+        if (done) { rc = pf_graph_replay<KIND>(h, u, obs3, k, angle_min); if (rc) return rc; }
     }
-    if (!done) { rc = pf_step_launches<SCAN>(h, u, obs3, k, angle_min); if (rc) return rc; }
+    if (!done) { rc = pf_step_launches<KIND>(h, u, obs3, k, angle_min); if (rc) return rc; }
     h->fu.last = h->fu.on;
     h->n_predict++;
     h->steps++;
@@ -822,7 +871,7 @@ extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3,
     PF_CUDA(cudaSetDevice(h->ctx.device));
     int rc = pf_stage_obs(h, obs3, k);
     if (rc) return rc;
-    return pf_step_impl<false>(h, u, obs3, k, 0.0, est);
+    return pf_step_impl<PF_KIND_LM>(h, u, obs3, k, 0.0, est);
 }
 extern "C" int pfgpu_pf_estimate(pfgpu_pf* h, double est[4], double cov_cm[16]) {
     if (!h) return PFGPU_ERR_INVALID;
@@ -978,7 +1027,7 @@ extern "C" int pfgpu_pf_update_scan(pfgpu_pf* h, const double* ranges, size_t B,
     size_t k = 0;
     int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
     if (rc) return rc;
-    rc = pf_launch_main<false, true, true>(h, nullptr, nullptr, k, angle_min);
+    rc = pf_launch_main<false, true, PF_KIND_LF>(h, nullptr, nullptr, k, angle_min);
     if (rc) return rc;
     h->rec.armed = false;                                                            // the weights are no longer uniform
     rc = pf_normalize(h);
@@ -993,7 +1042,109 @@ extern "C" int pfgpu_pf_step_scan(pfgpu_pf* h, const double u[2], const double* 
     size_t k = 0;
     int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
     if (rc) return rc;
-    return pf_step_impl<true>(h, u, nullptr, k, angle_min, est);
+    return pf_step_impl<PF_KIND_LF>(h, u, nullptr, k, angle_min, est);
+}
+
+// ---- beam model: ray-cast every particle's expected ranges in the occupancy grid (DESIGN §3.11, pf_beam.cuh) ----
+static void pf_beam_free(pfgpu_pf* h) {
+    cudaFree(h->bm.clr);
+    h->bm.clr = nullptr;
+    h->bm.on = false; h->bm.W = h->bm.H = 0; h->bm.L = 0;
+}
+extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_beam_config* c) {
+    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
+    if (W < 1 || H < 1 || W > 65536 || H > 65536 || W * H > ((size_t)1 << 28)) return PFGPU_ERR_INVALID;
+    auto positive = [](double v) { return finite_d(v) && v > 0.0; };
+    auto nonneg = [](double v) { return finite_d(v) && v >= 0.0; };
+    if (!positive(c->resolution) || !positive(c->sigma_hit) || !positive(c->z_rand) || !positive(c->max_range) ||
+        !positive(c->lambda_short) || !nonneg(c->z_hit) || !nonneg(c->z_short) || !nonneg(c->z_max) || c->max_beams < 2 ||
+        !(c->max_range / c->resolution <= 1048576.0))
+        return PFGPU_ERR_INVALID;
+    const double q_rand = c->z_rand / c->max_range;
+    const double coeff = 1.0 / sqrt(2.0 * PFC_PI * (c->sigma_hit * c->sigma_hit));
+    const double q_lo = c->z_max > 0.0 ? std::min(q_rand, c->z_max) : q_rand;
+    const double q_hi = c->z_hit * coeff + c->z_short * c->lambda_short + std::max(q_rand, c->z_max);
+    const uint64_t L = pf_lf_limit(q_lo, q_hi);
+    if (L < 1) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    pf_graph_drop(h);                          // the captured step holds the old table's address
+    pf_beam_free(h);
+    const size_t cells = W * H;
+    PF_CUDA(cudaMalloc(&h->bm.clr, cells));
+    PfScopedBuf m, g;
+    PF_CUDA(cudaMalloc(&m.p, cells));
+    PF_CUDA(cudaMalloc(&g.p, cells));
+    PF_CUDA(cudaMemcpyAsync(m.p, mask, cells, cudaMemcpyHostToDevice, h->ctx.stream));
+    PF_LAUNCH(h->ctx, pf_beam_clr_lines_kernel, cdiv_u(cells, 256), 256, 0, (const unsigned char*)m.p, (unsigned char*)g.p, (int)W, (int)H);
+    PF_LAUNCH(h->ctx, pf_beam_clr_cols_kernel, cdiv_u(cells, 256), 256, 0, (const unsigned char*)g.p, h->bm.clr, (int)W, (int)H);
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    const char* e = getenv("PFGPU_BEAM_SKIP");
+    h->bm.skip = (e && e[0] == '0') ? 0 : 1;
+    h->bm.W = W; h->bm.H = H; h->bm.L = L; h->bm.cfg = *c;
+    h->bm.on = true;
+    return 0;
+}
+extern "C" int pfgpu_pf_beam_clear(pfgpu_pf* h) {
+    if (!h) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    pf_graph_drop(h);
+    pf_beam_free(h);
+    return 0;
+}
+extern "C" int pfgpu_pf_beam_info(pfgpu_pf* h, size_t* W, size_t* H, uint64_t* L) {
+    if (!h) return PFGPU_ERR_INVALID;
+    if (W) *W = h->bm.W;
+    if (H) *H = h->bm.H;
+    if (L) *L = h->bm.L;
+    return 0;
+}
+extern "C" int pfgpu_pf_beam_download(pfgpu_pf* h, uint8_t* clearance, size_t cells) {
+    if (!h || !h->bm.on || !clearance || cells != h->bm.W * h->bm.H) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaMemcpyAsync(clearance, h->bm.clr, cells, cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_pf_update_beam(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc) {
+    if (!h) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    size_t k = 0;
+    int rc = pf_stage_beam(h, ranges, B, angle_min, angle_inc, &k);
+    if (rc) return rc;
+    rc = pf_launch_main<false, true, PF_KIND_BEAM>(h, nullptr, nullptr, k, angle_min);
+    if (rc) return rc;
+    h->rec.armed = false;                                                            // the weights are no longer uniform
+    rc = pf_normalize(h);
+    if (rc) return rc;
+    return pf_refresh_cache(h);
+}
+extern "C" int pfgpu_pf_step_beam(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
+                                  double est[4]) {
+    if (!h || !u) return PFGPU_ERR_INVALID;
+    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    size_t k = 0;
+    int rc = pf_stage_beam(h, ranges, B, angle_min, angle_inc, &k);
+    if (rc) return rc;
+    return pf_step_impl<PF_KIND_BEAM>(h, u, nullptr, k, angle_min, est);
+}
+extern "C" int pfgpu_pf_beam_raycast(pfgpu_pf* h, const double* poses3, size_t n, size_t B, double angle_min, double angle_inc,
+                                     double* out) {
+    if (!h || !h->bm.on || !finite_d(angle_min) || !finite_d(angle_inc)) return PFGPU_ERR_INVALID;
+    if (n == 0 || B == 0) return 0;
+    if (!poses3 || !out || n > ((size_t)1 << 40) / B) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PfScopedBuf dp, dout;
+    PF_CUDA(cudaMalloc(&dp.p, n * 3 * sizeof(double)));
+    PF_CUDA(cudaMalloc(&dout.p, n * B * sizeof(double)));
+    PF_CUDA(cudaMemcpyAsync(dp.p, poses3, n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+    PF_LAUNCH(h->ctx, pf_beam_raycast_kernel, cdiv_u(n * B, 256), 256, 0, pf_beam_arg(h, angle_min), (const double*)dp.p, n, B, angle_inc,
+              (double*)dout.p);
+    PF_CUDA(cudaMemcpyAsync(out, dout.p, n * B * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return 0;
 }
 
 // ---- pose hypotheses: the cloud clustered in a fixed (x, y, yaw) histogram (DESIGN §3.10, pf_cluster.cuh) ----

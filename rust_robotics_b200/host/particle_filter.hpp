@@ -114,6 +114,35 @@ public:
         dirty_ = true;
         return est;
     }
+    // beam scan model (not in the reference; DESIGN §3.11): the likelihood field's map conventions, a map of its own
+    static pfgpu_beam_config beam_defaults(double resolution) {                       // ROS AMCL's beam-model defaults
+        pfgpu_beam_config c{};
+        c.resolution = resolution; c.sigma_hit = 0.2; c.z_hit = 0.95; c.z_short = 0.1; c.z_max = 0.05; c.z_rand = 0.05;
+        c.lambda_short = 0.1; c.max_range = 30.0; c.max_beams = 60;
+        return c;
+    }
+    void set_beam_model(const std::vector<uint8_t>& mask, size_t width, size_t height, const pfgpu_beam_config& c) {
+        if (mask.size() != width * height) throw RoboticsError(RoboticsError::InvalidParameter, "beam model: mask size != width * height");
+        check(pfgpu_pf_beam_set(h_, mask.data(), width, height, &c), "beam model");
+    }
+    void clear_beam_model() { check(pfgpu_pf_beam_clear(h_), "beam model"); }
+    void try_update_with_beam_scan(const std::vector<double>& ranges, double angle_min, double angle_increment) {
+        check(pfgpu_pf_update_beam(h_, ranges.data(), ranges.size(), angle_min, angle_increment), "beam scan update"); dirty_ = true;
+    }
+    PFState try_step_beam_scan(const PFControl& u, const std::vector<double>& ranges, double angle_min, double angle_increment) {
+        PFState est{};
+        check(pfgpu_pf_step_beam(h_, u.data(), ranges.data(), ranges.size(), angle_min, angle_increment, est.data()), "beam scan step");
+        dirty_ = true;
+        return est;
+    }
+    // expected ranges of poses (x, y, yaw) x n_beams in the beam map: out[p * n_beams + b]
+    std::vector<double> expected_scan(const std::vector<std::array<double, 3>>& poses, size_t n_beams, double angle_min,
+                                      double angle_increment) {
+        std::vector<double> p, out(poses.size() * n_beams);
+        for (const auto& q : poses) p.insert(p.end(), q.begin(), q.end());
+        check(pfgpu_pf_beam_raycast(h_, p.data(), poses.size(), n_beams, angle_min, angle_increment, out.data()), "expected scan");
+        return out;
+    }
     // pose hypotheses (not in the reference; ROS AMCL's pose hypotheses; DESIGN §3.10): the max_count heaviest clusters of the
     // cloud in xy_res x xy_res x (2 pi / yaw_bins) bins, heaviest first; *total = the number of clusters; rank_of_slot (when given)
     // = each local particle's cluster rank, UINT32_MAX for a non-member

@@ -73,6 +73,21 @@ pub struct pfgpu_pf_hypothesis {
     pub bins: u64,
     pub label: u64,
 }
+/// the beam scan model's parameters (pfgpu_pf_beam_set; ROS AMCL's defaults 0.2, 0.95, 0.1, 0.05, 0.05, 0.1, 30, 60)
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct pfgpu_beam_config {
+    pub resolution: f64,
+    pub sigma_hit: f64,
+    pub z_hit: f64,
+    pub z_short: f64,
+    pub z_max: f64,
+    pub z_rand: f64,
+    pub lambda_short: f64,
+    pub max_range: f64,
+    pub max_beams: u32,
+    pub _pad: u32,
+}
 pub enum pfgpu_pf {}
 pub enum pfgpu_fs {}
 
@@ -107,6 +122,15 @@ extern "C" {
                               est: *mut f64) -> c_int;
     pub fn pfgpu_pf_hypotheses(h: *mut pfgpu_pf, xy_res: f64, yaw_bins: u32, out: *mut pfgpu_pf_hypothesis, cap: usize,
                                n_total: *mut usize, rank_of_slot: *mut u32) -> c_int;
+    pub fn pfgpu_pf_beam_set(h: *mut pfgpu_pf, mask: *const u8, width: usize, height: usize, cfg: *const pfgpu_beam_config) -> c_int;
+    pub fn pfgpu_pf_beam_clear(h: *mut pfgpu_pf) -> c_int;
+    pub fn pfgpu_pf_beam_info(h: *mut pfgpu_pf, width: *mut usize, height: *mut usize, max_used_beams: *mut u64) -> c_int;
+    pub fn pfgpu_pf_beam_download(h: *mut pfgpu_pf, clearance: *mut u8, cells: usize) -> c_int;
+    pub fn pfgpu_pf_update_beam(h: *mut pfgpu_pf, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64) -> c_int;
+    pub fn pfgpu_pf_step_beam(h: *mut pfgpu_pf, u: *const f64, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64,
+                              est: *mut f64) -> c_int;
+    pub fn pfgpu_pf_beam_raycast(h: *mut pfgpu_pf, poses3: *const f64, n: usize, n_beams: usize, angle_min: f64, angle_inc: f64,
+                                 out: *mut f64) -> c_int;
     pub fn pfgpu_fs_default_config(cfg: *mut pfgpu_fs_config);
     pub fn pfgpu_fs_create(cfg: *const pfgpu_fs_config, n_particles: usize, n_landmarks: usize, seed: u64, device: c_int,
                            out: *mut *mut pfgpu_fs) -> c_int;

@@ -120,6 +120,37 @@ impl MonteCarloLocalizer {
         out.truncate(total.min(max_count));
         Ok((out, total))
     }
+    /// Beam scan model (not in the reference; DESIGN §3.11): the likelihood field's map conventions, a map of its own.  Every
+    /// particle's expected range along every used beam is ray-cast in the map on the device and compared with the measured one.
+    pub fn set_beam_model(&mut self, obstacles: &[u8], width: usize, height: usize, cfg: &sys::pfgpu_beam_config) -> RoboticsResult<()> {
+        if obstacles.len() != width * height {
+            return Err(RoboticsError::InvalidParameter("beam model: obstacles.len() != width * height".to_string()));
+        }
+        status(unsafe { sys::pfgpu_pf_beam_set(self.h, obstacles.as_ptr(), width, height, cfg) })
+    }
+    pub fn clear_beam_model(&mut self) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_beam_clear(self.h) })
+    }
+    /// try_update_with_scan under the beam model
+    pub fn try_update_with_beam_scan(&mut self, ranges: &[f64], angle_min: f64, angle_increment: f64) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_update_beam(self.h, ranges.as_ptr(), ranges.len(), angle_min, angle_increment) })?;
+        self.refresh_cache()
+    }
+    /// try_step with a laser scan under the beam model
+    pub fn try_step_beam_scan(&mut self, control: &PFControl, ranges: &[f64], angle_min: f64, angle_increment: f64) -> RoboticsResult<PFState> {
+        let mut est = [0.0f64; 4];
+        status(unsafe { sys::pfgpu_pf_step_beam(self.h, control.as_ptr(), ranges.as_ptr(), ranges.len(), angle_min, angle_increment,
+                                                est.as_mut_ptr()) })?;
+        self.refresh_cache()?;
+        Ok(self.state_estimate)
+    }
+    /// expected ranges of poses (x, y, yaw) x n_beams in the beam map: out[p * n_beams + b]
+    pub fn expected_scan(&mut self, poses: &[[f64; 3]], n_beams: usize, angle_min: f64, angle_increment: f64) -> RoboticsResult<Vec<f64>> {
+        let mut out = vec![0.0f64; poses.len() * n_beams];
+        status(unsafe { sys::pfgpu_pf_beam_raycast(self.h, poses.as_ptr() as *const f64, poses.len(), n_beams, angle_min, angle_increment,
+                                                   out.as_mut_ptr()) })?;
+        Ok(out)
+    }
     pub fn try_predict_with_control(&mut self, control: &PFControl) -> RoboticsResult<()> {          // mcl.rs:209-257
         status(unsafe { sys::pfgpu_pf_predict(self.h, control.as_ptr()) })?;
         self.refresh_cache()
