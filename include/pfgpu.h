@@ -239,6 +239,62 @@ int  pfgpu_pf_step_beam(pfgpu_pf*, const double u[2], const double* ranges, size
                         double est[4]);
 int  pfgpu_pf_beam_raycast(pfgpu_pf*, const double* poses3, size_t n, size_t n_beams, double angle_min, double angle_inc, double* out);
 
+/* ===================================== Occupancy grid mapping ======================================= */
+
+/* OccupancyGridMap (rust_robotics_mapping/src/occupancy_grid_map.rs) on the device: laser scans fused into a log-odds grid with the
+ * reference's sequential result bit for bit, and its obstacle mask handed to the PF / MCL scan models without a host round trip
+ * (DESIGN §3.12).
+ *   grid       grid[ix * H + iy], f64 log-odds, initialised to prior_log_odds; world (0, 0) at the grid centre.  world_to_grid(x, y) =
+ *              (floor(x / res + W as f64 / 2.0), floor(y / res + H as f64 / 2.0)) with Rust's saturating `as i32` (NaN -> 0), None
+ *              when outside.
+ *   one scan   pose (x, y, yaw), ranges r_0 .. r_{B-1}, exactly update_with_scan (:78-130):
+ *              origin = world_to_grid(x, y); None: the whole scan is a no-op.  Beam i with r <= 0 or r not finite: skipped.  Else
+ *              angle = (yaw + angle_min) + i as f64 * angle_inc, end = (x + r * cos(angle), y + r * sin(angle)) (one sincos);
+ *              end_cell = world_to_grid(end) when inside, else BOTH coordinates round(end / res + W / 2) as i32 (round half away
+ *              from zero, saturating) clamped to [0, W - 1] (resp. H).  The cells of bresenham_line(origin, end_cell) (:164-193)
+ *              except the last get l = clamp(l + free_log_odds); the last gets l = clamp(l + occupied_log_odds) only when end was
+ *              inside.  clamp(l) = l < min ? min : (l > max ? max : l) (Rust's f64::clamp; NaN stays NaN).
+ *   batch      S poses x B ranges with one (angle_min, angle_inc): S single-scan updates in order.  The grid equals that bit for bit
+ *              whatever the batch size and the internal chunking, on every call.  No floating-point atomics.
+ *   obstacle   cell is an obstacle when 1.0 - 1.0 / (1.0 + exp(l)) > threshold (is_occupied, :136-159, with the contract exp).
+ * pfgpu_ogm_create: 1 <= W, H <= 65536, W * H <= 2^28, resolution positive and finite, every log-odds field finite and
+ *   min_log_odds <= max_log_odds (the prior may lie outside [min, max]); else PFGPU_ERR_INVALID.  The event workspace
+ *   (DESIGN §3.12) is allocated by the first update.
+ * pfgpu_ogm_update_scans: poses3 S x (x, y, yaw), ranges S x B row-major; S = 0 or B = 0 is a no-op.  Synchronises.
+ * pfgpu_ogm_set: uploads cells = W * H log-odds (any values).  pfgpu_ogm_read: count cells from `first` into out.
+ * pfgpu_ogm_obstacles: mask_out[c] = 1 for an obstacle cell, else 0, cells = W * H; threshold must be finite.
+ * pfgpu_ogm_info: W, H and the last update's stats (all nullable).
+ * pfgpu_pf_lfield_set_grid / pfgpu_pf_beam_set_grid: pfgpu_pf_lfield_set / pfgpu_pf_beam_set with the obstacle mask of `grid` at
+ *   `threshold`, built on the device: the same tables, the same refusals.  The grid is copied at set time; later updates of it do not
+ *   change the loaded model.  cfg->resolution must equal the grid's, and the grid must live on the handle's device; else
+ *   PFGPU_ERR_INVALID.  On a sharded engine every rank passes a grid of the same cells on its own device. */
+typedef struct {
+    double   resolution;         /* 0.5  metres per cell                                   */
+    uint64_t width, height;      /* 100, 100                                               */
+    double   prior_log_odds;     /* 0                                                      */
+    double   occupied_log_odds;  /* 0.85                                                   */
+    double   free_log_odds;      /* -0.4                                                   */
+    double   max_log_odds;       /* 5                                                      */
+    double   min_log_odds;       /* -5                                                     */
+} pfgpu_ogm_config;
+typedef struct {
+    uint64_t events;             /* cell updates of the last pfgpu_ogm_update_scans       */
+    uint64_t chunks;             /* pieces it ran in (a chunk holds at most the event cap) */
+    uint64_t longest_run;        /* the most updates one cell took in one chunk           */
+    uint64_t event_cap;          /* events per chunk at most                              */
+} pfgpu_ogm_stats;
+typedef struct pfgpu_ogm pfgpu_ogm;
+int  pfgpu_ogm_create(const pfgpu_ogm_config* cfg, int device, pfgpu_ogm** out);
+void pfgpu_ogm_destroy(pfgpu_ogm*);
+int  pfgpu_ogm_update_scans(pfgpu_ogm*, const double* poses3, size_t n_scans, const double* ranges, size_t n_ranges, double angle_min,
+                            double angle_inc);
+int  pfgpu_ogm_set(pfgpu_ogm*, const double* grid, size_t cells);
+int  pfgpu_ogm_read(pfgpu_ogm*, size_t first, size_t count, double* out);
+int  pfgpu_ogm_obstacles(pfgpu_ogm*, double threshold, uint8_t* mask_out, size_t cells);
+int  pfgpu_ogm_info(pfgpu_ogm*, size_t* width, size_t* height, pfgpu_ogm_stats* stats);
+int  pfgpu_pf_lfield_set_grid(pfgpu_pf*, const pfgpu_ogm* grid, double threshold, const pfgpu_lfield_config* cfg);
+int  pfgpu_pf_beam_set_grid(pfgpu_pf*, const pfgpu_ogm* grid, double threshold, const pfgpu_beam_config* cfg);
+
 /* ============================================ FastSLAM 1.0 ========================================== */
 
 /* Module constants of fs1.rs:13-23 as fields; pfgpu_fs_default_config() fills in the reference values. */

@@ -5,4 +5,5 @@ reference's public types (ParticleFilterLocalizer, MonteCarloLocalizer, fastslam
 ctypes.  There is no CPU fallback: constructing any filter without a CUDA device raises.
 """
 from .api import (FastSlam1, FastSlam2, FsConfig, InvalidParameter, MonteCarloLocalizationConfig, MonteCarloLocalizer,  # noqa: F401
-                  ParticleFilterConfig, ParticleFilterLocalizer, PfgpuError, PfHypothesis, load_library, obstacles_from_log_odds)
+                  OccupancyGridConfig, OccupancyGridMap, OgmStats, ParticleFilterConfig, ParticleFilterLocalizer, PfgpuError, PfHypothesis,
+                  load_library, obstacles_from_log_odds)

@@ -52,6 +52,16 @@ class _BmCfg(C.Structure):
                 ("max_beams", C.c_uint32), ("_pad", C.c_uint32)]
 
 
+class _OgmCfg(C.Structure):
+    _fields_ = [("resolution", C.c_double), ("width", C.c_uint64), ("height", C.c_uint64), ("prior_log_odds", C.c_double),
+                ("occupied_log_odds", C.c_double), ("free_log_odds", C.c_double), ("max_log_odds", C.c_double),
+                ("min_log_odds", C.c_double)]
+
+
+class _OgmStats(C.Structure):
+    _fields_ = [("events", C.c_uint64), ("chunks", C.c_uint64), ("longest_run", C.c_uint64), ("event_cap", C.c_uint64)]
+
+
 class _Hyp(C.Structure):
     _fields_ = [("mass", C.c_double), ("mean", C.c_double * 4), ("cov", C.c_double * 16), ("count", C.c_uint64),
                 ("bins", C.c_uint64), ("label", C.c_uint64)]
@@ -104,6 +114,8 @@ EXPORTS = [
     "pfgpu_pf_step_scan", "pfgpu_pf_hypotheses",
     "pfgpu_pf_beam_set", "pfgpu_pf_beam_clear", "pfgpu_pf_beam_info", "pfgpu_pf_beam_download", "pfgpu_pf_update_beam",
     "pfgpu_pf_step_beam", "pfgpu_pf_beam_raycast",
+    "pfgpu_ogm_create", "pfgpu_ogm_destroy", "pfgpu_ogm_update_scans", "pfgpu_ogm_set", "pfgpu_ogm_read", "pfgpu_ogm_obstacles",
+    "pfgpu_ogm_info", "pfgpu_pf_lfield_set_grid", "pfgpu_pf_beam_set_grid",
 ]
 
 
@@ -160,6 +172,16 @@ def load_library():
     L.pfgpu_pf_update_beam.argtypes = [vp, c_dp, C.c_size_t, C.c_double, C.c_double]
     L.pfgpu_pf_step_beam.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
     L.pfgpu_pf_beam_raycast.argtypes = [vp, c_dp, C.c_size_t, C.c_size_t, C.c_double, C.c_double, c_dp]
+    L.pfgpu_ogm_create.argtypes = [C.POINTER(_OgmCfg), C.c_int, C.POINTER(vp)]
+    L.pfgpu_ogm_destroy.argtypes = [vp]
+    L.pfgpu_ogm_destroy.restype = None
+    L.pfgpu_ogm_update_scans.argtypes = [vp, c_dp, C.c_size_t, c_dp, C.c_size_t, C.c_double, C.c_double]
+    L.pfgpu_ogm_set.argtypes = [vp, c_dp, C.c_size_t]
+    L.pfgpu_ogm_read.argtypes = [vp, C.c_size_t, C.c_size_t, c_dp]
+    L.pfgpu_ogm_obstacles.argtypes = [vp, C.c_double, C.POINTER(C.c_uint8), C.c_size_t]
+    L.pfgpu_ogm_info.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(_OgmStats)]
+    L.pfgpu_pf_lfield_set_grid.argtypes = [vp, vp, C.c_double, C.POINTER(_LfCfg)]
+    L.pfgpu_pf_beam_set_grid.argtypes = [vp, vp, C.c_double, C.POINTER(_BmCfg)]
     L.pfgpu_fs_default_config.argtypes = [C.POINTER(_FsCfg)]
     L.pfgpu_fs_create.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, C.POINTER(vp)]
     L.pfgpu_fs_create_sharded.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, vp, C.c_int,
@@ -497,6 +519,26 @@ class _PfBase:
                      float(max_range), int(max_beams), 0)
         _check(self.L, self.L.pfgpu_pf_beam_set(self.h, m.ctypes.data_as(C.POINTER(C.c_uint8)), m.shape[0], m.shape[1], C.byref(cfg)))
 
+    def set_likelihood_field_from_grid(self, grid_map, threshold=0.5, sigma_hit=0.2, z_hit=0.95, z_rand=0.05, max_range=30.0,
+                                       max_beams=60):
+        """set_likelihood_field(grid_map.obstacles(threshold), grid_map.config.resolution, ...) without leaving the device: the
+        OccupancyGridMap's obstacle mask is built on the device and the same table is loaded.  The grid is copied now: later
+        updates of grid_map do not change the loaded field.  grid_map must live on this filter's device."""
+        if not (max_beams >= 2 and max_beams < 2 ** 32):
+            raise InvalidParameter("max_beams >= 2")
+        cfg = _LfCfg(float(grid_map.config.resolution), float(sigma_hit), float(z_hit), float(z_rand), float(max_range), int(max_beams), 0)
+        _check(self.L, self.L.pfgpu_pf_lfield_set_grid(self.h, grid_map.h, float(threshold), C.byref(cfg)))
+
+    def set_beam_model_from_grid(self, grid_map, threshold=0.5, sigma_hit=0.2, z_hit=0.95, z_short=0.1, z_max=0.05, z_rand=0.05,
+                                 lambda_short=0.1, max_range=30.0, max_beams=60):
+        """set_beam_model(grid_map.obstacles(threshold), grid_map.config.resolution, ...) without leaving the device (see
+        set_likelihood_field_from_grid)"""
+        if not (max_beams >= 2 and max_beams < 2 ** 32):
+            raise InvalidParameter("max_beams >= 2")
+        cfg = _BmCfg(float(grid_map.config.resolution), float(sigma_hit), float(z_hit), float(z_short), float(z_max), float(z_rand),
+                     float(lambda_short), float(max_range), int(max_beams), 0)
+        _check(self.L, self.L.pfgpu_pf_beam_set_grid(self.h, grid_map.h, float(threshold), C.byref(cfg)))
+
     def clear_beam_model(self):
         _check(self.L, self.L.pfgpu_pf_beam_clear(self.h))
 
@@ -572,6 +614,134 @@ def obstacles_from_log_odds(grid, threshold=0.5):
     g = np.asarray(grid, dtype=np.float64)
     with np.errstate(over="ignore"):
         return (1.0 - 1.0 / (1.0 + np.exp(g))) > threshold
+
+
+# ------------------------------------------------------------------------------------------------
+class OccupancyGridConfig:
+    """occupancy_grid_map.rs:6-41"""
+
+    def __init__(self, resolution=0.5, width=100, height=100, prior_log_odds=0.0, occupied_log_odds=0.85, free_log_odds=-0.4,
+                 max_log_odds=5.0, min_log_odds=-5.0):
+        self.resolution, self.width, self.height = resolution, width, height
+        self.prior_log_odds, self.occupied_log_odds, self.free_log_odds = prior_log_odds, occupied_log_odds, free_log_odds
+        self.max_log_odds, self.min_log_odds = max_log_odds, min_log_odds
+
+    def _c(self):
+        if not (0 <= int(self.width) < 2 ** 64 and 0 <= int(self.height) < 2 ** 64):
+            raise InvalidParameter("width, height: 1 .. 65536")
+        return _OgmCfg(float(self.resolution), int(self.width), int(self.height), float(self.prior_log_odds), float(self.occupied_log_odds),
+                       float(self.free_log_odds), float(self.max_log_odds), float(self.min_log_odds))
+
+
+# OccupancyGridMap.stats(): the last update's cell updates, the chunks it ran in, the most updates one cell took in one chunk, and
+# the events a chunk holds at most
+OgmStats = collections.namedtuple("OgmStats", ["events", "chunks", "longest_run", "event_cap"])
+
+
+class OccupancyGridMap:
+    """occupancy_grid_map.rs:43-160 on the device (DESIGN §3.12): a W x H log-odds grid, grid[ix, iy], world (0, 0) at the grid centre.
+    Scans are fused on the device with update_with_scan's sequential result bit for bit; the grid stays there until read."""
+
+    def __init__(self, config=None, device=0):
+        self.config = config or OccupancyGridConfig()
+        self.L = load_library()
+        self.h = C.c_void_p()
+        self.device = device
+        _check(self.L, self.L.pfgpu_ogm_create(C.byref(self.config._c()), device, C.byref(self.h)))
+        self.W, self.H = int(self.config.width), int(self.config.height)
+
+    @classmethod
+    def new(cls, config, **kw):
+        return cls(config, **kw)
+
+    def close(self):
+        if getattr(self, "h", None) and self.h.value:
+            self.L.pfgpu_ogm_destroy(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    # -- reference API --
+    def update_with_scan(self, robot_x, robot_y, robot_yaw, scan_ranges, angle_min, angle_increment):
+        """Fuse one scan: scan_ranges[i] at robot_yaw + angle_min + i * angle_increment from the pose (:69-131)"""
+        self.update_with_scans([(robot_x, robot_y, robot_yaw)], [scan_ranges], angle_min, angle_increment)
+
+    def get_probability(self, ix, iy):
+        """1 - 1 / (1 + exp(l)) of cell (ix, iy) (:133-138)"""
+        l = self._cell(ix, iy)
+        try:
+            e = math.exp(l)
+        except OverflowError:
+            e = math.inf
+        return 1.0 - 1.0 / (1.0 + e)
+
+    def world_to_grid(self, x, y):
+        """(ix, iy), or None outside the grid (:140-153)"""
+        ix = _sat_floor_i32(float(x) / float(self.config.resolution) + self.W / 2.0)
+        iy = _sat_floor_i32(float(y) / float(self.config.resolution) + self.H / 2.0)
+        return (ix, iy) if 0 <= ix < self.W and 0 <= iy < self.H else None
+
+    def is_occupied(self, ix, iy, threshold):
+        return self.get_probability(ix, iy) > threshold
+
+    @property
+    def grid(self):
+        """the log-odds grid, (W, H) f64, downloaded"""
+        out = np.empty((self.W, self.H))
+        _check(self.L, self.L.pfgpu_ogm_read(self.h, 0, out.size, _dp(out)))
+        return out
+
+    # -- batched and device-side additions --
+    def update_with_scans(self, poses, scan_ranges, angle_min, angle_increment):
+        """Fuse S scans in order in one call: poses (S, 3) = (x, y, yaw), scan_ranges (S, B); the same bits as S update_with_scan calls"""
+        p = np.ascontiguousarray(_f64(poses).reshape(-1, 3))
+        r = _f64(scan_ranges)
+        if p.shape[0] == 0:
+            return
+        r = np.ascontiguousarray(r.reshape(p.shape[0], -1))
+        _check(self.L, self.L.pfgpu_ogm_update_scans(self.h, _dp(p), p.shape[0], _dp(r), r.shape[1], float(angle_min), float(angle_increment)))
+
+    def set_grid(self, grid):
+        """replace the log-odds grid: (W, H) values (any; they are not clamped)"""
+        g = np.ascontiguousarray(_f64(grid))
+        if g.shape != (self.W, self.H):
+            raise InvalidParameter(f"grid: shape ({self.W}, {self.H})")
+        _check(self.L, self.L.pfgpu_ogm_set(self.h, _dp(g), g.size))
+
+    def obstacles(self, threshold=0.5):
+        """is_occupied of every cell, computed on the device: (W, H) bool (obstacles_from_log_odds's rule with the contract exp)"""
+        m = np.empty((self.W, self.H), dtype=np.uint8)
+        _check(self.L, self.L.pfgpu_ogm_obstacles(self.h, float(threshold), m.ctypes.data_as(C.POINTER(C.c_uint8)), m.size))
+        return m.view(bool)
+
+    def stats(self):
+        """OgmStats of the last update"""
+        s = _OgmStats()
+        _check(self.L, self.L.pfgpu_ogm_info(self.h, None, None, C.byref(s)))
+        return OgmStats(s.events, s.chunks, s.longest_run, s.event_cap)
+
+    def _cell(self, ix, iy):
+        ix, iy = int(ix), int(iy)
+        if not (0 <= ix < self.W and 0 <= iy < self.H):
+            raise IndexError(f"cell ({ix}, {iy}) outside a {self.W} x {self.H} grid")
+        out = np.empty(1)
+        _check(self.L, self.L.pfgpu_ogm_read(self.h, ix * self.H + iy, 1, _dp(out)))
+        return float(out[0])
+
+
+def _sat_floor_i32(v):
+    """Rust's `floor() as i32`: saturating, NaN -> 0"""
+    if v != v:
+        return 0
+    if v >= 2147483647.0:
+        return 2147483647
+    if v <= -2147483648.0:
+        return -2147483648
+    return int(math.floor(v))
 
 
 class ParticleFilterLocalizer(_PfBase):

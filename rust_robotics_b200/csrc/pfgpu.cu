@@ -7,6 +7,7 @@
 #include "pf_kld.cuh"
 #include "pf_lfield.cuh"
 #include "pf_cluster.cuh"
+#include "ogm.cuh"
 #include "xsum_sharded.cuh"
 #include <cstdlib>
 #include <new>
@@ -966,37 +967,51 @@ struct PfScopedBuf {
     void* p = nullptr;
     ~PfScopedBuf() { if (p) cudaFree(p); }
 };
-extern "C" int pfgpu_pf_lfield_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_lfield_config* c) {
-    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
-    if (W < 1 || H < 1 || W > 65536 || H > 65536 || W * H > ((size_t)1 << 28)) return PFGPU_ERR_INVALID;
+static bool pf_map_shape_ok(size_t W, size_t H) { return W >= 1 && H >= 1 && W <= 65536 && H <= 65536 && W * H <= ((size_t)1 << 28); }
+// the likelihood field's config check; its beam bound L and q_out
+static int pf_lf_check(size_t W, size_t H, const pfgpu_lfield_config* c, uint64_t* L, double* q_out) {
+    if (!pf_map_shape_ok(W, H)) return PFGPU_ERR_INVALID;
     auto positive = [](double v) { return finite_d(v) && v > 0.0; };
     if (!positive(c->resolution) || !positive(c->sigma_hit) || !positive(c->z_rand) || !positive(c->max_range) || !finite_d(c->z_hit) ||
         c->z_hit < 0.0 || c->max_beams < 2)
         return PFGPU_ERR_INVALID;
-    const double q_out = c->z_rand / c->max_range;
+    *q_out = c->z_rand / c->max_range;
     const double coeff = 1.0 / sqrt(2.0 * PFC_PI * (c->sigma_hit * c->sigma_hit));
-    const uint64_t L = pf_lf_limit(q_out, c->z_hit * coeff + q_out);
-    if (L < 1) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
+    *L = pf_lf_limit(*q_out, c->z_hit * coeff + *q_out);
+    return *L < 1 ? PFGPU_ERR_INVALID : 0;
+}
+// the likelihood field from an obstacle mask on the handle's device, enqueued on its stream (a host mask or a grid's, DESIGN §3.12)
+static int pf_lf_load(pfgpu_pf* h, const unsigned char* mask_dev, size_t W, size_t H, const pfgpu_lfield_config* c, uint64_t L,
+                      double q_out) {
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     pf_graph_drop(h);                          // the captured step holds the old table's address
     pf_lf_free(h);
     const size_t cells = W * H, scratch = std::max(W * (H + 1), H * (W + 1));
     PF_CUDA(cudaMalloc(&h->lf.D, cells * sizeof(double)));
     PF_CUDA(cudaMalloc(&h->lf.q, cells * sizeof(double)));
-    PfScopedBuf m, v, z;
-    PF_CUDA(cudaMalloc(&m.p, cells));
+    PfScopedBuf v, z;
     PF_CUDA(cudaMalloc(&v.p, scratch * sizeof(int)));
     PF_CUDA(cudaMalloc(&z.p, scratch * sizeof(double)));
-    PF_CUDA(cudaMemcpyAsync(m.p, mask, cells, cudaMemcpyHostToDevice, h->ctx.stream));
     // rows into q (as scratch), columns into D, then D = sqrt and the factor table
-    PF_LAUNCH(h->ctx, pf_lf_edt_rows_kernel, cdiv_u(W, 32), 32, 0, (const unsigned char*)m.p, h->lf.q, (int)W, (int)H, (int*)v.p, (double*)z.p);
+    PF_LAUNCH(h->ctx, pf_lf_edt_rows_kernel, cdiv_u(W, 32), 32, 0, mask_dev, h->lf.q, (int)W, (int)H, (int*)v.p, (double*)z.p);
     PF_LAUNCH(h->ctx, pf_lf_edt_cols_kernel, cdiv_u(H, 32), 32, 0, h->lf.q, h->lf.D, (int)W, (int)H, (int*)v.p, (double*)z.p);
     PF_LAUNCH(h->ctx, pf_lf_table_kernel, cdiv_u(cells, 256), 256, 0, h->lf.D, h->lf.q, cells, c->resolution, c->sigma_hit, c->z_hit, q_out);
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     h->lf.W = W; h->lf.H = H; h->lf.L = L; h->lf.cfg = *c; h->lf.q_out = q_out;
     h->lf.on = true;
     return 0;
+}
+extern "C" int pfgpu_pf_lfield_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_lfield_config* c) {
+    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
+    uint64_t L = 0;
+    double q_out = 0.0;
+    int rc = pf_lf_check(W, H, c, &L, &q_out);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PfScopedBuf m;
+    PF_CUDA(cudaMalloc(&m.p, W * H));
+    PF_CUDA(cudaMemcpyAsync(m.p, mask, W * H, cudaMemcpyHostToDevice, h->ctx.stream));
+    return pf_lf_load(h, (const unsigned char*)m.p, W, H, c, L, q_out);
 }
 extern "C" int pfgpu_pf_lfield_clear(pfgpu_pf* h) {
     if (!h) return PFGPU_ERR_INVALID;
@@ -1051,9 +1066,9 @@ static void pf_beam_free(pfgpu_pf* h) {
     h->bm.clr = nullptr;
     h->bm.on = false; h->bm.W = h->bm.H = 0; h->bm.L = 0;
 }
-extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_beam_config* c) {
-    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
-    if (W < 1 || H < 1 || W > 65536 || H > 65536 || W * H > ((size_t)1 << 28)) return PFGPU_ERR_INVALID;
+// the beam model's config check; its beam bound L
+static int pf_beam_check(size_t W, size_t H, const pfgpu_beam_config* c, uint64_t* Lout) {
+    if (!pf_map_shape_ok(W, H)) return PFGPU_ERR_INVALID;
     auto positive = [](double v) { return finite_d(v) && v > 0.0; };
     auto nonneg = [](double v) { return finite_d(v) && v >= 0.0; };
     if (!positive(c->resolution) || !positive(c->sigma_hit) || !positive(c->z_rand) || !positive(c->max_range) ||
@@ -1064,19 +1079,19 @@ extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, siz
     const double coeff = 1.0 / sqrt(2.0 * PFC_PI * (c->sigma_hit * c->sigma_hit));
     const double q_lo = c->z_max > 0.0 ? std::min(q_rand, c->z_max) : q_rand;
     const double q_hi = c->z_hit * coeff + c->z_short * c->lambda_short + std::max(q_rand, c->z_max);
-    const uint64_t L = pf_lf_limit(q_lo, q_hi);
-    if (L < 1) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
+    *Lout = pf_lf_limit(q_lo, q_hi);
+    return *Lout < 1 ? PFGPU_ERR_INVALID : 0;
+}
+// the beam map from an obstacle mask on the handle's device, enqueued on its stream (a host mask or a grid's, DESIGN §3.12)
+static int pf_beam_load(pfgpu_pf* h, const unsigned char* mask_dev, size_t W, size_t H, const pfgpu_beam_config* c, uint64_t L) {
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     pf_graph_drop(h);                          // the captured step holds the old table's address
     pf_beam_free(h);
     const size_t cells = W * H;
     PF_CUDA(cudaMalloc(&h->bm.clr, cells));
-    PfScopedBuf m, g;
-    PF_CUDA(cudaMalloc(&m.p, cells));
+    PfScopedBuf g;
     PF_CUDA(cudaMalloc(&g.p, cells));
-    PF_CUDA(cudaMemcpyAsync(m.p, mask, cells, cudaMemcpyHostToDevice, h->ctx.stream));
-    PF_LAUNCH(h->ctx, pf_beam_clr_lines_kernel, cdiv_u(cells, 256), 256, 0, (const unsigned char*)m.p, (unsigned char*)g.p, (int)W, (int)H);
+    PF_LAUNCH(h->ctx, pf_beam_clr_lines_kernel, cdiv_u(cells, 256), 256, 0, mask_dev, (unsigned char*)g.p, (int)W, (int)H);
     PF_LAUNCH(h->ctx, pf_beam_clr_cols_kernel, cdiv_u(cells, 256), 256, 0, (const unsigned char*)g.p, h->bm.clr, (int)W, (int)H);
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     const char* e = getenv("PFGPU_BEAM_SKIP");
@@ -1084,6 +1099,17 @@ extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, siz
     h->bm.W = W; h->bm.H = H; h->bm.L = L; h->bm.cfg = *c;
     h->bm.on = true;
     return 0;
+}
+extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_beam_config* c) {
+    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
+    uint64_t L = 0;
+    int rc = pf_beam_check(W, H, c, &L);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PfScopedBuf m;
+    PF_CUDA(cudaMalloc(&m.p, W * H));
+    PF_CUDA(cudaMemcpyAsync(m.p, mask, W * H, cudaMemcpyHostToDevice, h->ctx.stream));
+    return pf_beam_load(h, (const unsigned char*)m.p, W, H, c, L);
 }
 extern "C" int pfgpu_pf_beam_clear(pfgpu_pf* h) {
     if (!h) return PFGPU_ERR_INVALID;
@@ -1145,6 +1171,230 @@ extern "C" int pfgpu_pf_beam_raycast(pfgpu_pf* h, const double* poses3, size_t n
     PF_CUDA(cudaMemcpyAsync(out, dout.p, n * B * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     return 0;
+}
+
+// ====================================================================================================
+// Occupancy grid mapping (DESIGN §3.12, ogm.cuh)
+// ====================================================================================================
+struct pfgpu_ogm {
+    Ctx ctx;
+    pfgpu_ogm_config cfg = {};
+    size_t W = 0, H = 0;
+    double* grid = nullptr;            // [W * H], ix * H + iy
+    unsigned long long cap = PF_OGM_EVENT_CAP;
+    // the event workspace, allocated by the first update (DESIGN §3.12 gives its size)
+    int4* geo = nullptr;               // [PF_OGM_BEAM_CAP] per beam of a window: origin, end cell
+    unsigned long long* cnt = nullptr; // [PF_OGM_BEAM_CAP] events per beam
+    unsigned long long* incl = nullptr;// [PF_OGM_BEAM_CAP] their inclusive sum
+    unsigned int* keys[2] = {nullptr, nullptr};   // [cap] each: the radix sort's double buffer
+    void* tmp = nullptr;               // CUB temporary storage
+    size_t tmp_bytes = 0;
+    unsigned long long* scal = nullptr;// [4] device: chunk end, chunk events, longest run (as u32)
+    unsigned long long* h_pin = nullptr;   // [4] pinned host
+    pfgpu_ogm_stats st = {};
+};
+
+static void pf_ogm_free(pfgpu_ogm* g) {
+    cudaFree(g->grid); cudaFree(g->geo); cudaFree(g->cnt); cudaFree(g->incl); cudaFree(g->keys[0]); cudaFree(g->keys[1]);
+    cudaFree(g->tmp); cudaFree(g->scal);
+    if (g->h_pin) cudaFreeHost(g->h_pin);
+    if (g->ctx.stream) cudaStreamDestroy(g->ctx.stream);
+}
+extern "C" void pfgpu_ogm_destroy(pfgpu_ogm* g) {
+    if (!g) return;
+    cudaSetDevice(g->ctx.device);
+    if (g->ctx.stream) cudaStreamSynchronize(g->ctx.stream);
+    pf_ogm_free(g);
+    delete g;
+}
+extern "C" int pfgpu_ogm_create(const pfgpu_ogm_config* c, int device, pfgpu_ogm** out) {
+    if (!c || !out) return PFGPU_ERR_INVALID;
+    *out = nullptr;
+    if (c->width > 65536 || c->height > 65536 || !pf_map_shape_ok((size_t)c->width, (size_t)c->height) || !finite_d(c->resolution) ||
+        !(c->resolution > 0.0) || !finite_d(c->prior_log_odds) || !finite_d(c->occupied_log_odds) || !finite_d(c->free_log_odds) ||
+        !finite_d(c->max_log_odds) || !finite_d(c->min_log_odds) || !(c->min_log_odds <= c->max_log_odds))
+        return PFGPU_ERR_INVALID;
+    pfgpu_ogm* g = new (std::nothrow) pfgpu_ogm();
+    if (!g) return PFGPU_ERR_CUDA;
+    g->cfg = *c;
+    g->W = (size_t)c->width; g->H = (size_t)c->height;
+    const char* e = getenv("PFGPU_OGM_EVENT_CAP");   // a smaller cap (at least 65536) forces chunking, for tests
+    if (e && *e) g->cap = std::max<unsigned long long>(65536ull, std::min<unsigned long long>(strtoull(e, nullptr, 10), PF_OGM_EVENT_CAP));
+    const int orc = ctx_open(g->ctx, device);
+    if (orc) { pf_ogm_free(g); delete g; return orc; }
+    auto fail = [&](cudaError_t err, int line) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "%s:%d: ogm create -> %s", __FILE__, line, cudaGetErrorString(err));
+        pf_ogm_free(g);
+        delete g;
+        return PFGPU_ERR_CUDA;
+    };
+    cudaError_t err;
+    const size_t cells = g->W * g->H;
+    if ((err = cudaMalloc(&g->grid, cells * sizeof(double))) != cudaSuccess) return fail(err, __LINE__);
+    pf_ogm_fill_kernel<<<cdiv_u(cells, 256), 256, 0, g->ctx.stream>>>(g->grid, cells, c->prior_log_odds);
+    g->ctx.launches++;
+    if ((err = cudaGetLastError()) != cudaSuccess || (err = cudaStreamSynchronize(g->ctx.stream)) != cudaSuccess) return fail(err, __LINE__);
+    *out = g;
+    return 0;
+}
+// the bits the radix sort compares for cells 0 .. cells - 1: ceil(log2 cells), at least 1
+static int pf_ogm_bits(size_t cells) {
+    int b = 1;
+    while (b < 28 && ((size_t)1 << b) < cells) ++b;
+    return b;
+}
+static int pf_ogm_alloc(pfgpu_ogm* g) {
+    PF_CUDA(cudaMalloc(&g->geo, PF_OGM_BEAM_CAP * sizeof(int4)));
+    PF_CUDA(cudaMalloc(&g->cnt, PF_OGM_BEAM_CAP * sizeof(unsigned long long)));
+    PF_CUDA(cudaMalloc(&g->incl, PF_OGM_BEAM_CAP * sizeof(unsigned long long)));
+    PF_CUDA(cudaMalloc(&g->keys[0], g->cap * sizeof(unsigned int)));
+    PF_CUDA(cudaMalloc(&g->keys[1], g->cap * sizeof(unsigned int)));
+    PF_CUDA(cudaMalloc(&g->scal, 4 * sizeof(unsigned long long)));
+    PF_CUDA(cudaMallocHost(&g->h_pin, 4 * sizeof(unsigned long long)));
+    size_t b0 = 0, b1 = 0;
+    cub::DoubleBuffer<unsigned int> db(g->keys[0], g->keys[1]);
+    PF_CUDA(cub::DeviceScan::InclusiveSum(nullptr, b0, g->cnt, g->incl, (int)PF_OGM_BEAM_CAP, g->ctx.stream));
+    PF_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, b1, db, (int)g->cap, 0, pf_ogm_bits(g->W * g->H), g->ctx.stream));
+    g->tmp_bytes = std::max(b0, b1);
+    PF_CUDA(cudaMalloc(&g->tmp, g->tmp_bytes));
+    return 0;
+}
+extern "C" int pfgpu_ogm_update_scans(pfgpu_ogm* g, const double* poses3, size_t S, const double* ranges, size_t B, double angle_min,
+                                      double angle_inc) {
+    if (!g) return PFGPU_ERR_INVALID;
+    g->st.events = g->st.chunks = g->st.longest_run = 0;
+    g->st.event_cap = g->cap;
+    if (S == 0 || B == 0) return 0;
+    if (!poses3 || !ranges || S > ((size_t)1 << 40) / B) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(g->ctx.device));
+    if (!g->keys[0]) {
+        const int rc = pf_ogm_alloc(g);
+        if (rc) {
+            cudaFree(g->geo); cudaFree(g->cnt); cudaFree(g->incl); cudaFree(g->keys[0]); cudaFree(g->keys[1]); cudaFree(g->tmp);
+            cudaFree(g->scal);
+            if (g->h_pin) cudaFreeHost(g->h_pin);
+            g->geo = nullptr; g->cnt = g->incl = g->scal = g->h_pin = nullptr; g->keys[0] = g->keys[1] = nullptr; g->tmp = nullptr;
+            return rc;
+        }
+    }
+    Ctx& ctx = g->ctx;
+    const size_t NB = S * B;
+    PfScopedBuf dp, dr;
+    PF_CUDA(cudaMalloc(&dp.p, S * 3 * sizeof(double)));
+    PF_CUDA(cudaMalloc(&dr.p, NB * sizeof(double)));
+    PF_CUDA(cudaMemcpyAsync(dp.p, poses3, S * 3 * sizeof(double), cudaMemcpyHostToDevice, ctx.stream));
+    PF_CUDA(cudaMemcpyAsync(dr.p, ranges, NB * sizeof(double), cudaMemcpyHostToDevice, ctx.stream));
+    PF_CUDA(cudaMemsetAsync(g->scal + 2, 0, sizeof(unsigned long long), ctx.stream));
+    PfOgmGeom gm;
+    gm.res = g->cfg.resolution; gm.half_w = (double)g->W / 2.0; gm.half_h = (double)g->H / 2.0; gm.W = (int)g->W; gm.H = (int)g->H;
+    const int bits = pf_ogm_bits(g->W * g->H);
+    const pfgpu_ogm_config& c = g->cfg;
+    for (size_t w0 = 0; w0 < NB; w0 += PF_OGM_BEAM_CAP) {
+        const size_t nb = std::min<size_t>(PF_OGM_BEAM_CAP, NB - w0);
+        PF_LAUNCH(ctx, pf_ogm_count_kernel, cdiv_u(nb, 256), 256, 0, gm, (const double*)dp.p, (const double*)dr.p, B, w0, nb, angle_min,
+                  angle_inc, g->geo, g->cnt);
+        size_t tb = g->tmp_bytes;
+        PF_CUDA(cub::DeviceScan::InclusiveSum(g->tmp, tb, g->cnt, g->incl, (int)nb, ctx.stream));
+        unsigned long long base = 0;
+        for (size_t b = 0; b < nb;) {
+            PF_LAUNCH(ctx, pf_ogm_chunk_kernel, 1, 1, 0, (const unsigned long long*)g->incl, b, nb, base, g->cap, g->scal);
+            PF_CUDA(cudaMemcpyAsync(g->h_pin, g->scal, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx.stream));
+            PF_CUDA(cudaStreamSynchronize(ctx.stream));
+            const size_t e = (size_t)g->h_pin[0];
+            const unsigned long long E = g->h_pin[1];
+            if (E > 0) {
+                PF_LAUNCH(ctx, pf_ogm_emit_kernel, cdiv_u((e - b) * 32, 256), 256, 0, (const int4*)g->geo, (const unsigned long long*)g->incl,
+                          b, e, base, (int)g->H, g->keys[0]);
+                cub::DoubleBuffer<unsigned int> db(g->keys[0], g->keys[1]);
+                PF_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, db, (int)E, 0, bits, ctx.stream));
+                if (tb > g->tmp_bytes) {
+                    snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "ogm: radix sort of %llu keys wants %zu temporary bytes, %zu allocated", E, tb,
+                             g->tmp_bytes);
+                    return PFGPU_ERR_CUDA;
+                }
+                PF_CUDA(cub::DeviceRadixSort::SortKeys(g->tmp, tb, db, (int)E, 0, bits, ctx.stream));
+                PF_LAUNCH(ctx, pf_ogm_fold_kernel, cdiv_u(E, 256), 256, 0, (const unsigned int*)db.Current(), (size_t)E, g->grid,
+                          c.occupied_log_odds, c.free_log_odds, c.min_log_odds, c.max_log_odds, (unsigned int*)(g->scal + 2));
+                g->st.events += E;
+                g->st.chunks += 1;
+            }
+            base += E;
+            b = e;
+        }
+    }
+    PF_CUDA(cudaMemcpyAsync(g->h_pin + 2, g->scal + 2, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(ctx.stream));
+    g->st.longest_run = g->h_pin[2];
+    return 0;
+}
+extern "C" int pfgpu_ogm_set(pfgpu_ogm* g, const double* grid, size_t cells) {
+    if (!g || !grid || cells != g->W * g->H) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(g->ctx.device));
+    PF_CUDA(cudaMemcpyAsync(g->grid, grid, cells * sizeof(double), cudaMemcpyHostToDevice, g->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(g->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_ogm_read(pfgpu_ogm* g, size_t first, size_t count, double* out) {
+    if (!g || first > g->W * g->H || count > g->W * g->H - first || (count && !out)) return PFGPU_ERR_INVALID;
+    if (count == 0) return 0;
+    PF_CUDA(cudaSetDevice(g->ctx.device));
+    PF_CUDA(cudaMemcpyAsync(out, g->grid + first, count * sizeof(double), cudaMemcpyDeviceToHost, g->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(g->ctx.stream));
+    return 0;
+}
+// the obstacle mask of g at `threshold` into mask_dev (cells bytes on g's device), enqueued on `ctx`'s stream after g's work
+static int pf_ogm_mask(const pfgpu_ogm* g, double threshold, unsigned char* mask_dev, Ctx& ctx) {
+    PF_CUDA(cudaStreamSynchronize(g->ctx.stream));
+    const size_t cells = g->W * g->H;
+    PF_LAUNCH(ctx, pf_ogm_mask_kernel, cdiv_u(cells, 256), 256, 0, (const double*)g->grid, cells, threshold, mask_dev);
+    return 0;
+}
+extern "C" int pfgpu_ogm_obstacles(pfgpu_ogm* g, double threshold, uint8_t* mask_out, size_t cells) {
+    if (!g || !mask_out || cells != g->W * g->H || !finite_d(threshold)) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(g->ctx.device));
+    PfScopedBuf m;
+    PF_CUDA(cudaMalloc(&m.p, cells));
+    int rc = pf_ogm_mask(g, threshold, (unsigned char*)m.p, g->ctx);
+    if (rc) return rc;
+    PF_CUDA(cudaMemcpyAsync(mask_out, m.p, cells, cudaMemcpyDeviceToHost, g->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(g->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_ogm_info(pfgpu_ogm* g, size_t* W, size_t* H, pfgpu_ogm_stats* st) {
+    if (!g) return PFGPU_ERR_INVALID;
+    if (W) *W = g->W;
+    if (H) *H = g->H;
+    if (st) { *st = g->st; st->event_cap = g->cap; }
+    return 0;
+}
+// a grid handed to a PF handle: on its device, at the model's resolution
+static bool pf_grid_ok(const pfgpu_pf* h, const pfgpu_ogm* g, double threshold, double resolution) {
+    return g && finite_d(threshold) && g->ctx.device == h->ctx.device && resolution == g->cfg.resolution;
+}
+extern "C" int pfgpu_pf_lfield_set_grid(pfgpu_pf* h, const pfgpu_ogm* grid, double threshold, const pfgpu_lfield_config* c) {
+    if (!h || !c || !pf_grid_ok(h, grid, threshold, c->resolution)) return PFGPU_ERR_INVALID;
+    uint64_t L = 0;
+    double q_out = 0.0;
+    int rc = pf_lf_check(grid->W, grid->H, c, &L, &q_out);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PfScopedBuf m;
+    PF_CUDA(cudaMalloc(&m.p, grid->W * grid->H));
+    rc = pf_ogm_mask(grid, threshold, (unsigned char*)m.p, h->ctx);
+    if (rc) return rc;
+    return pf_lf_load(h, (const unsigned char*)m.p, grid->W, grid->H, c, L, q_out);
+}
+extern "C" int pfgpu_pf_beam_set_grid(pfgpu_pf* h, const pfgpu_ogm* grid, double threshold, const pfgpu_beam_config* c) {
+    if (!h || !c || !pf_grid_ok(h, grid, threshold, c->resolution)) return PFGPU_ERR_INVALID;
+    uint64_t L = 0;
+    int rc = pf_beam_check(grid->W, grid->H, c, &L);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PfScopedBuf m;
+    PF_CUDA(cudaMalloc(&m.p, grid->W * grid->H));
+    rc = pf_ogm_mask(grid, threshold, (unsigned char*)m.p, h->ctx);
+    if (rc) return rc;
+    return pf_beam_load(h, (const unsigned char*)m.p, grid->W, grid->H, c, L);
 }
 
 // ---- pose hypotheses: the cloud clustered in a fixed (x, y, yaw) histogram (DESIGN §3.10, pf_cluster.cuh) ----

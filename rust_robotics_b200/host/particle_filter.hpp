@@ -125,6 +125,14 @@ public:
         if (mask.size() != width * height) throw RoboticsError(RoboticsError::InvalidParameter, "beam model: mask size != width * height");
         check(pfgpu_pf_beam_set(h_, mask.data(), width, height, &c), "beam model");
     }
+    // the obstacle mask of an occupancy grid on this handle's device (OccupancyGridMap::handle(), occupancy_grid_map.hpp), built
+    // there at `threshold`: the same table as the host-mask calls; the grid is copied now
+    void set_beam_model_from_grid(const pfgpu_ogm* grid, double threshold, const pfgpu_beam_config& c) {
+        check(pfgpu_pf_beam_set_grid(h_, grid, threshold, &c), "beam model from grid");
+    }
+    void set_likelihood_field_from_grid(const pfgpu_ogm* grid, double threshold, const pfgpu_lfield_config& c) {
+        check(pfgpu_pf_lfield_set_grid(h_, grid, threshold, &c), "likelihood field from grid");
+    }
     void clear_beam_model() { check(pfgpu_pf_beam_clear(h_), "beam model"); }
     void try_update_with_beam_scan(const std::vector<double>& ranges, double angle_min, double angle_increment) {
         check(pfgpu_pf_update_beam(h_, ranges.data(), ranges.size(), angle_min, angle_increment), "beam scan update"); dirty_ = true;

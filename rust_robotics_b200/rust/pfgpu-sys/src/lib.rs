@@ -88,8 +88,31 @@ pub struct pfgpu_beam_config {
     pub max_beams: u32,
     pub _pad: u32,
 }
+/// OccupancyGridConfig (pfgpu_ogm_create; the reference's defaults 0.5, 100, 100, 0, 0.85, -0.4, 5, -5)
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct pfgpu_ogm_config {
+    pub resolution: f64,
+    pub width: u64,
+    pub height: u64,
+    pub prior_log_odds: f64,
+    pub occupied_log_odds: f64,
+    pub free_log_odds: f64,
+    pub max_log_odds: f64,
+    pub min_log_odds: f64,
+}
+/// the last pfgpu_ogm_update_scans: cell updates, chunks, the most updates of one cell in one chunk, the chunk cap
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct pfgpu_ogm_stats {
+    pub events: u64,
+    pub chunks: u64,
+    pub longest_run: u64,
+    pub event_cap: u64,
+}
 pub enum pfgpu_pf {}
 pub enum pfgpu_fs {}
+pub enum pfgpu_ogm {}
 
 #[link(name = "pfgpu")]
 extern "C" {
@@ -131,6 +154,16 @@ extern "C" {
                               est: *mut f64) -> c_int;
     pub fn pfgpu_pf_beam_raycast(h: *mut pfgpu_pf, poses3: *const f64, n: usize, n_beams: usize, angle_min: f64, angle_inc: f64,
                                  out: *mut f64) -> c_int;
+    pub fn pfgpu_ogm_create(cfg: *const pfgpu_ogm_config, device: c_int, out: *mut *mut pfgpu_ogm) -> c_int;
+    pub fn pfgpu_ogm_destroy(h: *mut pfgpu_ogm);
+    pub fn pfgpu_ogm_update_scans(h: *mut pfgpu_ogm, poses3: *const f64, n_scans: usize, ranges: *const f64, n_ranges: usize,
+                                  angle_min: f64, angle_inc: f64) -> c_int;
+    pub fn pfgpu_ogm_set(h: *mut pfgpu_ogm, grid: *const f64, cells: usize) -> c_int;
+    pub fn pfgpu_ogm_read(h: *mut pfgpu_ogm, first: usize, count: usize, out: *mut f64) -> c_int;
+    pub fn pfgpu_ogm_obstacles(h: *mut pfgpu_ogm, threshold: f64, mask_out: *mut u8, cells: usize) -> c_int;
+    pub fn pfgpu_ogm_info(h: *mut pfgpu_ogm, width: *mut usize, height: *mut usize, stats: *mut pfgpu_ogm_stats) -> c_int;
+    pub fn pfgpu_pf_lfield_set_grid(h: *mut pfgpu_pf, grid: *const pfgpu_ogm, threshold: f64, cfg: *const pfgpu_lfield_config) -> c_int;
+    pub fn pfgpu_pf_beam_set_grid(h: *mut pfgpu_pf, grid: *const pfgpu_ogm, threshold: f64, cfg: *const pfgpu_beam_config) -> c_int;
     pub fn pfgpu_fs_default_config(cfg: *mut pfgpu_fs_config);
     pub fn pfgpu_fs_create(cfg: *const pfgpu_fs_config, n_particles: usize, n_landmarks: usize, seed: u64, device: c_int,
                            out: *mut *mut pfgpu_fs) -> c_int;

@@ -9,6 +9,8 @@
 pub mod fastslam1;
 pub mod fastslam2;
 pub mod monte_carlo_localization;
+pub mod occupancy_grid_map;
 pub mod particle_filter;
 pub use monte_carlo_localization::{MonteCarloLocalizationConfig, MonteCarloLocalizer};
+pub use occupancy_grid_map::{OccupancyGridConfig, OccupancyGridMap};
 pub use particle_filter::{ParticleFilterConfig, ParticleFilterLocalizer};

@@ -165,6 +165,16 @@ impl ParticleFilterLocalizer {
         }
         status(unsafe { sys::pfgpu_pf_beam_set(self.h, obstacles.as_ptr(), width, height, cfg) })
     }
+    /// set_beam_model with the obstacle mask of an OccupancyGridMap built on the device at `threshold`; the grid is copied now
+    pub fn set_beam_model_from_grid(&mut self, grid: &crate::occupancy_grid_map::OccupancyGridMap, threshold: f64,
+                                    cfg: &sys::pfgpu_beam_config) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_beam_set_grid(self.h, grid.handle(), threshold, cfg) })
+    }
+    /// set_likelihood_field with the obstacle mask of an OccupancyGridMap built on the device at `threshold`
+    pub fn set_likelihood_field_from_grid(&mut self, grid: &crate::occupancy_grid_map::OccupancyGridMap, threshold: f64,
+                                          cfg: &sys::pfgpu_lfield_config) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_lfield_set_grid(self.h, grid.handle(), threshold, cfg) })
+    }
     pub fn clear_beam_model(&mut self) -> RoboticsResult<()> {
         status(unsafe { sys::pfgpu_pf_beam_clear(self.h) })
     }
