@@ -295,6 +295,75 @@ int  pfgpu_ogm_info(pfgpu_ogm*, size_t* width, size_t* height, pfgpu_ogm_stats* 
 int  pfgpu_pf_lfield_set_grid(pfgpu_pf*, const pfgpu_ogm* grid, double threshold, const pfgpu_lfield_config* cfg);
 int  pfgpu_pf_beam_set_grid(pfgpu_pf*, const pfgpu_ogm* grid, double threshold, const pfgpu_beam_config* cfg);
 
+/* ====================================== Correlative scan matching ===================================== */
+
+/* correlative_scan_match (rust_robotics_slam/src/correlative_scan_matching.rs:55-197, Olson's brute-force correlative matcher) on
+ * the device, the reference's result bit for bit (DESIGN §3.13).  A handle holds reference points on one device; the lookup table
+ * for a resolution is built from them on first use and rebuilt when the resolution changes, so any config works on any reference.
+ *   invalid    an empty reference or query, linear_step <= 0, angular_step <= 0 or grid_resolution <= 0 (:63-78): the result is
+ *              (x, y, yaw) of the initial pose, yaw NOT normalised, score 0.0, converged 0.
+ *   offsets    n = round(range / step) as i32 (round half away from zero, Rust's saturating cast); the offsets are i as f64 * step for
+ *              i = -n ..= n (:122-127), none for n < 0.  No linear or no angular offset: (x, y, normalize_angle(yaw)), score -1.0,
+ *              converged 0 (:84-90).
+ *   table      sigma = res, R = ceil(3.0 * sigma / res) as i32 (R = 4 where 3 * res / res rounds above 3, as for res = 0.025, 0.05,
+ *              0.1, 0.2; R = 3 for 0.01, 0.02, 0.25, 0.5, 1.0), inv = 0.5 / (sigma * sigma).  Each reference point (x, y) has centre
+ *              cell (round(x / res), round(y / res)) as i32; every cell (ix, iy) of its (2R+1)^2 window gets
+ *              w = exp((-d2) * inv), d2 = (gx - x) * (gx - x) + (gy - y) * (gy - y), gx = ix as f64 * res, gy = iy as f64 * res,
+ *              unless w < 1e-6; a cell keeps the maximum of its weights, and a cell no point reached reads 0.0 (:129-159).
+ *   score      for a candidate (cx, cy, cyaw) with cyaw = normalize_angle(yaw + dyaw), cx = x + dx, cy = y + dy and
+ *              (c, s) = (cos cyaw, sin cyaw): per query point (px, py) in order, wx = ((c * px) - (s * py)) + cx,
+ *              wy = ((s * px) + (c * py)) + cy, cell (round(wx / res), round(wy / res)) as i32; score = 0.0 + v_0 + v_1 + ...,
+ *              one sequential sum (:161-180).
+ *   winner     candidates in the loop order dx, then dy, then dyaw (:93-117), penalty = (dx * dx + dy * dy) + dyaw * dyaw; the
+ *              loop keeps a candidate when score > best or (score == best and penalty < best penalty).  Every score is >= 0 > -1,
+ *              so that loop's answer is the lexicographic optimum: the largest score, then the smallest penalty, then the earliest
+ *              candidate.  The device reduces by exactly that total order, so no block or reduction order can change the result.
+ *              The result is (cx, cy, cyaw, score) of the winner, converged = score > 0.0.
+ *   normalize_angle is fs1.rs's loop (`-= 2.0 * PI` while > PI, `+= 2.0 * PI` while < -PI), capped at 2^22 turns (DESIGN §8
+ *   deviation 2); cos, sin and exp are the contract's (pf_contract_math.h).
+ * Refusals (DESIGN §8 deviation 16): a non-finite reference point, query point, pose or config field, or a reference cell with
+ *   |round(x / res)| or |round(y / res)| above 2^30 (the reference's i32 window arithmetic would overflow): PFGPU_ERR_INVALID.  A table
+ *   wider than PFGPU_CSM_TABLE_CAP cells, a resolution outside [2^-500, 2^500], n_linear > 2^15, n_angular > 2^22, more than
+ *   2^34 candidates per query, or one query whose cell indices for one yaw exceed the workspace (8 (2 n_linear + 1) points bytes
+ *   above 2^28): PFGPU_ERR_UNSUPPORTED, and the handle stays usable.  The table is built only for a call in which some query has
+ *   candidates.
+ * pfgpu_csm_set_reference: n points (n = 0 allowed: every match is then invalid), copied to the device.
+ * pfgpu_csm_set_reference_grid: the cell centres of `grid`'s obstacle cells at `threshold` (pfgpu_ogm_obstacles' rule), in the
+ *   grid's cell order: x = ((ix + 0.5) - W / 2.0) * res, y = ((iy + 0.5) - H / 2.0) * res (each an f64 operation in that order),
+ *   built on the device without a host round trip.  The grid must live on the matcher's device and threshold be finite, else
+ *   PFGPU_ERR_INVALID.  The points are copied now: later updates of the grid do not change the matcher until it is set again.
+ * pfgpu_csm_match: Q queries against the reference under one config; query q has the initial pose poses3[3q .. 3q + 2] and the
+ *   points qx[k], qy[k] for offsets[q] <= k < offsets[q + 1] (offsets[0] = 0, non-decreasing).  Each query's result is what
+ *   correlative_scan_match returns for it alone; an invalid query gets the invalid result and the others are still matched.
+ *   Synchronises.
+ * pfgpu_csm_table_info: builds (or keeps) the table for `resolution` and reports its extent: cell (ix, iy) with
+ *   origin_x <= ix < origin_x + width (likewise y) is at ix * height + iy relative to the origin, and every cell outside reads 0.0;
+ *   the extent is the reference cells' bounding box grown by R.  No reference point: width = height = 0.  All outputs nullable.
+ * pfgpu_csm_table_read: count f64 cells of the current table from `first`. */
+#define PFGPU_CSM_TABLE_CAP ((uint64_t)1 << 26)
+typedef struct {
+    double linear_search_range;  /* 1.0   metres                                           */
+    double angular_search_range; /* 0.2   radians                                          */
+    double linear_step;          /* 0.1                                                    */
+    double angular_step;         /* 0.02                                                   */
+    double grid_resolution;      /* 0.05  metres per lookup cell                           */
+} pfgpu_csm_config;
+typedef struct {
+    double   x, y, yaw, score;
+    uint32_t converged, _pad;
+} pfgpu_csm_result;
+typedef struct pfgpu_csm pfgpu_csm;
+int  pfgpu_csm_create(int device, pfgpu_csm** out);
+void pfgpu_csm_destroy(pfgpu_csm*);
+int  pfgpu_csm_set_reference(pfgpu_csm*, const double* x, const double* y, size_t n);
+int  pfgpu_csm_set_reference_grid(pfgpu_csm*, const pfgpu_ogm* grid, double threshold);
+int  pfgpu_csm_reference_size(pfgpu_csm*, size_t* n);
+int  pfgpu_csm_match(pfgpu_csm*, const pfgpu_csm_config* cfg, const double* poses3, size_t n_queries, const double* qx, const double* qy,
+                     const uint64_t* offsets, pfgpu_csm_result* results);
+int  pfgpu_csm_table_info(pfgpu_csm*, double resolution, int64_t* origin_x, int64_t* origin_y, uint64_t* width, uint64_t* height,
+                          int32_t* radius);
+int  pfgpu_csm_table_read(pfgpu_csm*, size_t first, size_t count, double* out);
+
 /* ============================================ FastSLAM 1.0 ========================================== */
 
 /* Module constants of fs1.rs:13-23 as fields; pfgpu_fs_default_config() fills in the reference values. */

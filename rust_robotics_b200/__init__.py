@@ -4,6 +4,7 @@ The product is the CUDA library (csrc/ -> libpfgpu.so, C ABI in include/pfgpu.h)
 reference's public types (ParticleFilterLocalizer, MonteCarloLocalizer, fastslam1) over that ABI with
 ctypes.  There is no CPU fallback: constructing any filter without a CUDA device raises.
 """
-from .api import (FastSlam1, FastSlam2, FsConfig, InvalidParameter, MonteCarloLocalizationConfig, MonteCarloLocalizer,  # noqa: F401
+from .api import (CorrelativeScanMatcher, CorrelativeScanMatcherConfig, FastSlam1, FastSlam2, FsConfig, InvalidParameter,  # noqa: F401
+                  MonteCarloLocalizationConfig, MonteCarloLocalizer,
                   OccupancyGridConfig, OccupancyGridMap, OgmStats, ParticleFilterConfig, ParticleFilterLocalizer, PfgpuError, PfHypothesis,
-                  load_library, obstacles_from_log_odds)
+                  ScanMatchResult, correlative_scan_match, load_library, obstacles_from_log_odds)

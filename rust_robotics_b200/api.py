@@ -62,6 +62,16 @@ class _OgmStats(C.Structure):
     _fields_ = [("events", C.c_uint64), ("chunks", C.c_uint64), ("longest_run", C.c_uint64), ("event_cap", C.c_uint64)]
 
 
+class _CsmCfg(C.Structure):
+    _fields_ = [("linear_search_range", C.c_double), ("angular_search_range", C.c_double), ("linear_step", C.c_double),
+                ("angular_step", C.c_double), ("grid_resolution", C.c_double)]
+
+
+class _CsmResult(C.Structure):
+    _fields_ = [("x", C.c_double), ("y", C.c_double), ("yaw", C.c_double), ("score", C.c_double), ("converged", C.c_uint32),
+                ("_pad", C.c_uint32)]
+
+
 class _Hyp(C.Structure):
     _fields_ = [("mass", C.c_double), ("mean", C.c_double * 4), ("cov", C.c_double * 16), ("count", C.c_uint64),
                 ("bins", C.c_uint64), ("label", C.c_uint64)]
@@ -116,6 +126,8 @@ EXPORTS = [
     "pfgpu_pf_step_beam", "pfgpu_pf_beam_raycast",
     "pfgpu_ogm_create", "pfgpu_ogm_destroy", "pfgpu_ogm_update_scans", "pfgpu_ogm_set", "pfgpu_ogm_read", "pfgpu_ogm_obstacles",
     "pfgpu_ogm_info", "pfgpu_pf_lfield_set_grid", "pfgpu_pf_beam_set_grid",
+    "pfgpu_csm_create", "pfgpu_csm_destroy", "pfgpu_csm_set_reference", "pfgpu_csm_set_reference_grid", "pfgpu_csm_reference_size",
+    "pfgpu_csm_match", "pfgpu_csm_table_info", "pfgpu_csm_table_read",
 ]
 
 
@@ -182,6 +194,16 @@ def load_library():
     L.pfgpu_ogm_info.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(_OgmStats)]
     L.pfgpu_pf_lfield_set_grid.argtypes = [vp, vp, C.c_double, C.POINTER(_LfCfg)]
     L.pfgpu_pf_beam_set_grid.argtypes = [vp, vp, C.c_double, C.POINTER(_BmCfg)]
+    L.pfgpu_csm_create.argtypes = [C.c_int, C.POINTER(vp)]
+    L.pfgpu_csm_destroy.argtypes = [vp]
+    L.pfgpu_csm_destroy.restype = None
+    L.pfgpu_csm_set_reference.argtypes = [vp, c_dp, c_dp, C.c_size_t]
+    L.pfgpu_csm_set_reference_grid.argtypes = [vp, vp, C.c_double]
+    L.pfgpu_csm_reference_size.argtypes = [vp, C.POINTER(C.c_size_t)]
+    L.pfgpu_csm_match.argtypes = [vp, C.POINTER(_CsmCfg), c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_uint64), C.POINTER(_CsmResult)]
+    L.pfgpu_csm_table_info.argtypes = [vp, C.c_double, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_uint64),
+                                       C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    L.pfgpu_csm_table_read.argtypes = [vp, C.c_size_t, C.c_size_t, c_dp]
     L.pfgpu_fs_default_config.argtypes = [C.POINTER(_FsCfg)]
     L.pfgpu_fs_create.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, C.POINTER(vp)]
     L.pfgpu_fs_create_sharded.argtypes = [C.POINTER(_FsCfg), C.c_size_t, C.c_size_t, C.c_uint64, C.c_int, vp, C.c_int,
@@ -731,6 +753,114 @@ class OccupancyGridMap:
         out = np.empty(1)
         _check(self.L, self.L.pfgpu_ogm_read(self.h, ix * self.H + iy, 1, _dp(out)))
         return float(out[0])
+
+
+# ------------------------------------------------------------------------------------------------
+class CorrelativeScanMatcherConfig:
+    """correlative_scan_matching.rs:17-42"""
+
+    def __init__(self, linear_search_range=1.0, angular_search_range=0.2, linear_step=0.1, angular_step=0.02, grid_resolution=0.05):
+        self.linear_search_range, self.angular_search_range = linear_search_range, angular_search_range
+        self.linear_step, self.angular_step, self.grid_resolution = linear_step, angular_step, grid_resolution
+
+    def _c(self):
+        return _CsmCfg(float(self.linear_search_range), float(self.angular_search_range), float(self.linear_step), float(self.angular_step),
+                       float(self.grid_resolution))
+
+
+# correlative_scan_matching.rs:44-52
+ScanMatchResult = collections.namedtuple("ScanMatchResult", ["x", "y", "yaw", "score", "converged"])
+
+
+class CorrelativeScanMatcher:
+    """correlative_scan_match (correlative_scan_matching.rs:55-197) on the device (DESIGN §3.13): reference points held on one device,
+    their lookup table built there for each resolution a match asks for, every candidate pose of the window scored there, the
+    reference's result bit for bit.  One call matches one query or a batch of queries against the same reference."""
+
+    def __init__(self, device=0):
+        self.L = load_library()
+        self.h = C.c_void_p()
+        self.device = device
+        _check(self.L, self.L.pfgpu_csm_create(int(device), C.byref(self.h)))
+
+    def close(self):
+        if getattr(self, "h", None) and self.h.value:
+            self.L.pfgpu_csm_destroy(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_reference(self, reference_x, reference_y):
+        """the reference scan (world points); copied to the device"""
+        x, y = _f64(reference_x).ravel(), _f64(reference_y).ravel()
+        if x.size != y.size:
+            raise InvalidParameter("reference_x and reference_y differ in length")
+        _check(self.L, self.L.pfgpu_csm_set_reference(self.h, _dp(x), _dp(y), x.size))
+
+    def set_reference_from_grid(self, grid_map, threshold=0.5):
+        """the centres of grid_map's obstacle cells at `threshold` (OccupancyGridMap.obstacles), built on the device; the grid is copied
+        now, so later updates of grid_map do not change the matcher.  grid_map must live on this matcher's device."""
+        _check(self.L, self.L.pfgpu_csm_set_reference_grid(self.h, grid_map.h, float(threshold)))
+
+    @property
+    def reference_size(self):
+        n = C.c_size_t()
+        _check(self.L, self.L.pfgpu_csm_reference_size(self.h, C.byref(n)))
+        return int(n.value)
+
+    def match(self, query_x, query_y, initial_pose, config=None):
+        """One query: query_x, query_y (sequences of floats) and initial_pose (x, y, yaw) -> ScanMatchResult.  A batch: query_x and
+        query_y lists of per-query sequences (any lengths) and initial_pose (Q, 3) -> a list of ScanMatchResult."""
+        cfg = (config or CorrelativeScanMatcherConfig())._c()
+        p = _f64(initial_pose)
+        single = p.ndim == 1
+        p = np.ascontiguousarray(p.reshape(-1, 3))
+        qxs = [query_x] if single else list(query_x)
+        qys = [query_y] if single else list(query_y)
+        if len(qxs) != p.shape[0] or len(qys) != p.shape[0]:
+            raise InvalidParameter("one point list per initial pose")
+        xs, ys = [_f64(a).ravel() for a in qxs], [_f64(a).ravel() for a in qys]
+        if any(a.size != b.size for a, b in zip(xs, ys)):
+            raise InvalidParameter("query_x and query_y differ in length")
+        off = np.zeros(len(xs) + 1, dtype=np.uint64)
+        off[1:] = np.cumsum([a.size for a in xs])
+        qx = np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros(0))
+        qy = np.ascontiguousarray(np.concatenate(ys) if ys else np.zeros(0))
+        out = (_CsmResult * max(1, p.shape[0]))()
+        _check(self.L, self.L.pfgpu_csm_match(self.h, C.byref(cfg), _dp(p), p.shape[0], _dp(qx), _dp(qy),
+                                              off.ctypes.data_as(C.POINTER(C.c_uint64)), out))
+        res = [ScanMatchResult(r.x, r.y, r.yaw, r.score, bool(r.converged)) for r in out[:p.shape[0]]]
+        return res[0] if single else res
+
+    def table_info(self, grid_resolution=0.05):
+        """(origin_x, origin_y, width, height, R) of the lookup table for grid_resolution (built now if it is not the current one)"""
+        ox, oy, W, H, R = C.c_int64(), C.c_int64(), C.c_uint64(), C.c_uint64(), C.c_int32()
+        _check(self.L, self.L.pfgpu_csm_table_info(self.h, float(grid_resolution), C.byref(ox), C.byref(oy), C.byref(W), C.byref(H),
+                                                   C.byref(R)))
+        return int(ox.value), int(oy.value), int(W.value), int(H.value), int(R.value)
+
+    def lookup_table(self, grid_resolution=0.05):
+        """the lookup table for grid_resolution: (dense (width, height) f64 array, (origin_x, origin_y), R); cell (ix, iy) is
+        table[ix - origin_x, iy - origin_y], and every cell outside reads 0.0 (build_lookup_table's HashMap, :129-159)"""
+        ox, oy, W, H, R = self.table_info(grid_resolution)
+        t = np.zeros((W, H))
+        if t.size:
+            _check(self.L, self.L.pfgpu_csm_table_read(self.h, 0, t.size, _dp(t)))
+        return t, (ox, oy), R
+
+
+def correlative_scan_match(reference_x, reference_y, query_x, query_y, initial_pose, config=None, device=0):
+    """correlative_scan_matching.rs:55-120 with its signature: a one-shot matcher on `device`"""
+    m = CorrelativeScanMatcher(device)
+    try:
+        m.set_reference(reference_x, reference_y)
+        return m.match(query_x, query_y, tuple(initial_pose), config)
+    finally:
+        m.close()
 
 
 def _sat_floor_i32(v):

@@ -8,6 +8,7 @@
 #include "pf_lfield.cuh"
 #include "pf_cluster.cuh"
 #include "ogm.cuh"
+#include "csm.cuh"
 #include "xsum_sharded.cuh"
 #include <cstdlib>
 #include <new>
@@ -1395,6 +1396,341 @@ extern "C" int pfgpu_pf_beam_set_grid(pfgpu_pf* h, const pfgpu_ogm* grid, double
     rc = pf_ogm_mask(grid, threshold, (unsigned char*)m.p, h->ctx);
     if (rc) return rc;
     return pf_beam_load(h, (const unsigned char*)m.p, grid->W, grid->H, c, L);
+}
+
+// ====================================================================================================
+// Correlative scan matching (DESIGN §3.13, csm.cuh)
+// ====================================================================================================
+#define PF_CSM_WS_CAP ((size_t)1 << 28)         // bytes of cell indices per launch (X and Y)
+#define PF_CSM_PART_CAP ((size_t)1 << 20)       // block bests per launch
+struct pfgpu_csm {
+    Ctx ctx;
+    double* rx = nullptr;               // [ncap] reference points
+    double* ry = nullptr;
+    size_t n = 0, ncap = 0;
+    unsigned long long* table = nullptr;// [tcap] f64 bits, (ix - ox) * TH + (iy - oy)
+    size_t tcap = 0;
+    bool table_ok = false;
+    double table_res = 0.0;
+    long long ox = 0, oy = 0, TW = 0, TH = 0;
+    int R = 0;
+    int* X = nullptr;                   // [ws_ints] cell indices of one launch
+    int* Y = nullptr;
+    size_t ws_ints = 0;
+    double2* cs = nullptr;              // [cs_cap] (cos, sin) per (query, yaw) of a launch
+    size_t cs_cap = 0;
+    PfCsmBest* part = nullptr;          // [PF_CSM_PART_CAP] block bests
+    PfCsmBest* best = nullptr;          // [best_cap] per query
+    size_t best_cap = 0;
+    int* ext = nullptr;                 // [5] device: extent and the out-of-range flag
+    int* h_ext = nullptr;               // [5] pinned host
+    size_t ws_cap = PF_CSM_WS_CAP;
+    // pfgpu_csm_set_reference_grid's buffers, kept between calls (a mapping loop sets the reference once per step)
+    unsigned char* gmask = nullptr;     // [gmask_cap] obstacle mask
+    size_t gmask_cap = 0;
+    unsigned int* gidx = nullptr;       // [gidx_cap] compacted obstacle cell indices
+    size_t gidx_cap = 0;
+    unsigned long long* gnum = nullptr; // [1] their count
+    size_t gnum_cap = 0;
+    unsigned char* gtmp = nullptr;      // [gtmp_cap] CUB temporary storage
+    size_t gtmp_cap = 0;
+};
+
+// Rust's `as i32` of a double: saturating, NaN -> 0
+static int csm_sat_i32(double v) {
+    if (v != v) return 0;
+    if (v >= 2147483647.0) return 2147483647;
+    if (v <= -2147483648.0) return (int)(-2147483647 - 1);
+    return (int)v;
+}
+// cudaMalloc of `need` elements unless `cap` already holds them (the old contents are dropped)
+template <class T> static int csm_grow(T** p, size_t* cap, size_t need) {
+    if (need <= *cap) return 0;
+    cudaFree(*p);
+    *p = nullptr;
+    *cap = 0;
+    PF_CUDA(cudaMalloc(p, need * sizeof(T)));
+    *cap = need;
+    return 0;
+}
+static void pf_csm_free(pfgpu_csm* h) {
+    cudaFree(h->rx); cudaFree(h->ry); cudaFree(h->table); cudaFree(h->X); cudaFree(h->Y); cudaFree(h->cs); cudaFree(h->part);
+    cudaFree(h->best); cudaFree(h->ext); cudaFree(h->gmask); cudaFree(h->gidx); cudaFree(h->gnum); cudaFree(h->gtmp);
+    if (h->h_ext) cudaFreeHost(h->h_ext);
+    if (h->ctx.stream) cudaStreamDestroy(h->ctx.stream);
+}
+extern "C" void pfgpu_csm_destroy(pfgpu_csm* h) {
+    if (!h) return;
+    cudaSetDevice(h->ctx.device);
+    if (h->ctx.stream) cudaStreamSynchronize(h->ctx.stream);
+    pf_csm_free(h);
+    delete h;
+}
+extern "C" int pfgpu_csm_create(int device, pfgpu_csm** out) {
+    if (!out) return PFGPU_ERR_INVALID;
+    *out = nullptr;
+    pfgpu_csm* h = new (std::nothrow) pfgpu_csm();
+    if (!h) return PFGPU_ERR_CUDA;
+    const char* e = getenv("PFGPU_CSM_WS_CAP");    // a smaller workspace (at least 2^16 bytes) forces chunking, for tests
+    if (e && *e) h->ws_cap = std::max<size_t>((size_t)1 << 16, std::min<size_t>(strtoull(e, nullptr, 10), PF_CSM_WS_CAP));
+    int rc = ctx_open(h->ctx, device);
+    if (!rc) {
+        auto alloc = [&]() -> int {
+            PF_CUDA(cudaMalloc(&h->ext, 5 * sizeof(int)));
+            PF_CUDA(cudaMallocHost(&h->h_ext, 5 * sizeof(int)));
+            PF_CUDA(cudaMalloc(&h->part, PF_CSM_PART_CAP * sizeof(PfCsmBest)));
+            return 0;
+        };
+        rc = alloc();
+    }
+    if (rc) { pf_csm_free(h); delete h; return rc; }
+    *out = h;
+    return 0;
+}
+extern "C" int pfgpu_csm_set_reference(pfgpu_csm* h, const double* x, const double* y, size_t n) {
+    if (!h || (n && (!x || !y)) || n > ((size_t)1 << 31)) return PFGPU_ERR_INVALID;
+    for (size_t i = 0; i < n; ++i)
+        if (!finite_d(x[i]) || !finite_d(y[i])) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    h->table_ok = false;
+    h->n = 0;
+    if (n) {
+        size_t c = h->ncap;
+        int rc = csm_grow(&h->rx, &c, n);
+        if (!rc) { c = h->ncap; rc = csm_grow(&h->ry, &c, n); }
+        if (rc) { cudaFree(h->rx); cudaFree(h->ry); h->rx = h->ry = nullptr; h->ncap = 0; return rc; }
+        h->ncap = std::max(h->ncap, n);
+        PF_CUDA(cudaMemcpyAsync(h->rx, x, n * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+        PF_CUDA(cudaMemcpyAsync(h->ry, y, n * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    }
+    h->n = n;
+    return 0;
+}
+extern "C" int pfgpu_csm_set_reference_grid(pfgpu_csm* h, const pfgpu_ogm* g, double threshold) {
+    if (!h || !g || !finite_d(threshold) || g->ctx.device != h->ctx.device) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    const size_t cells = g->W * g->H;
+    thrust::counting_iterator<unsigned int> it(0u);
+    size_t tb = 0;
+    PF_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, it, (const unsigned char*)nullptr, (unsigned int*)nullptr,
+                                       (unsigned long long*)nullptr, (long long)cells, h->ctx.stream));
+    int rc = csm_grow(&h->gmask, &h->gmask_cap, cells);
+    if (!rc) rc = csm_grow(&h->gidx, &h->gidx_cap, cells);
+    if (!rc) rc = csm_grow(&h->gnum, &h->gnum_cap, 1);
+    if (!rc) rc = csm_grow(&h->gtmp, &h->gtmp_cap, std::max<size_t>(tb, 1));
+    if (rc) return rc;
+    rc = pf_ogm_mask(g, threshold, h->gmask, h->ctx);
+    if (rc) return rc;
+    PF_CUDA(cub::DeviceSelect::Flagged(h->gtmp, tb, it, (const unsigned char*)h->gmask, h->gidx, h->gnum, (long long)cells, h->ctx.stream));
+    unsigned long long n = 0;
+    PF_CUDA(cudaMemcpyAsync(&n, h->gnum, sizeof(n), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    h->table_ok = false;
+    h->n = 0;
+    if (n) {
+        size_t c = h->ncap;
+        rc = csm_grow(&h->rx, &c, n);
+        if (!rc) { c = h->ncap; rc = csm_grow(&h->ry, &c, n); }
+        if (rc) { cudaFree(h->rx); cudaFree(h->ry); h->rx = h->ry = nullptr; h->ncap = 0; return rc; }
+        h->ncap = std::max<size_t>(h->ncap, n);
+        PF_LAUNCH(h->ctx, pf_csm_centres_kernel, cdiv_u(n, 256), 256, 0, (const unsigned int*)h->gidx, (size_t)n, (unsigned int)g->H,
+                  (double)g->W / 2.0, (double)g->H / 2.0, g->cfg.resolution, h->rx, h->ry);
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    }
+    h->n = n;
+    return 0;
+}
+extern "C" int pfgpu_csm_reference_size(pfgpu_csm* h, size_t* n) {
+    if (!h || !n) return PFGPU_ERR_INVALID;
+    *n = h->n;
+    return 0;
+}
+// the lookup table for `res` (build_lookup_table :129-159), kept until the reference or the resolution changes
+static int pf_csm_table(pfgpu_csm* h, double res) {
+    if (h->table_ok && h->table_res == res) return 0;
+    if (!(res >= 0x1p-500 && res <= 0x1p500)) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "csm: grid_resolution %g outside [2^-500, 2^500]", res);
+        return PFGPU_ERR_UNSUPPORTED;
+    }
+    h->table_ok = false;
+    const double sigma = res;
+    const int R = csm_sat_i32(ceil(3.0 * sigma / res));
+    const double inv = 0.5 / (sigma * sigma);
+    if (h->n == 0) {
+        h->ox = h->oy = h->TW = h->TH = 0; h->R = R;
+        h->table_ok = true; h->table_res = res;
+        return 0;
+    }
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    const int init[5] = {INT_MAX, INT_MIN, INT_MAX, INT_MIN, 0};
+    memcpy(h->h_ext, init, sizeof(init));
+    PF_CUDA(cudaMemcpyAsync(h->ext, h->h_ext, sizeof(init), cudaMemcpyHostToDevice, h->ctx.stream));
+    PF_LAUNCH(h->ctx, pf_csm_extent_kernel, cdiv_u(h->n, 256), 256, 0, (const double*)h->rx, (const double*)h->ry, h->n, res, h->ext,
+              h->ext + 4);
+    PF_CUDA(cudaMemcpyAsync(h->h_ext, h->ext, sizeof(init), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    if (h->h_ext[4]) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "csm: a reference cell beyond 2^30 at resolution %g", res);
+        return PFGPU_ERR_INVALID;
+    }
+    const long long ox = (long long)h->h_ext[0] - R, oy = (long long)h->h_ext[2] - R;
+    const long long TW = (long long)h->h_ext[1] + R + 1 - ox, TH = (long long)h->h_ext[3] + R + 1 - oy;
+    if (TW > (long long)PFGPU_CSM_TABLE_CAP || TH > (long long)PFGPU_CSM_TABLE_CAP || (uint64_t)(TW * TH) > PFGPU_CSM_TABLE_CAP) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "csm: a %lld x %lld table exceeds %llu cells", TW, TH,
+                 (unsigned long long)PFGPU_CSM_TABLE_CAP);
+        return PFGPU_ERR_UNSUPPORTED;
+    }
+    const size_t cells = (size_t)(TW * TH);
+    int rc = csm_grow(&h->table, &h->tcap, cells);
+    if (rc) return rc;
+    PF_CUDA(cudaMemsetAsync(h->table, 0, cells * sizeof(double), h->ctx.stream));
+    const size_t side = 2 * (size_t)R + 1;
+    PF_LAUNCH(h->ctx, pf_csm_fill_kernel, cdiv_u(h->n * side * side, 256), 256, 0, (const double*)h->rx, (const double*)h->ry, h->n, res,
+              inv, R, ox, oy, TH, h->table);
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    h->ox = ox; h->oy = oy; h->TW = TW; h->TH = TH; h->R = R;
+    h->table_ok = true; h->table_res = res;
+    return 0;
+}
+extern "C" int pfgpu_csm_table_info(pfgpu_csm* h, double res, int64_t* ox, int64_t* oy, uint64_t* W, uint64_t* H, int32_t* R) {
+    if (!h || !finite_d(res) || !(res > 0.0)) return PFGPU_ERR_INVALID;
+    const int rc = pf_csm_table(h, res);
+    if (rc) return rc;
+    if (ox) *ox = h->ox;
+    if (oy) *oy = h->oy;
+    if (W) *W = (uint64_t)h->TW;
+    if (H) *H = (uint64_t)h->TH;
+    if (R) *R = h->R;
+    return 0;
+}
+extern "C" int pfgpu_csm_table_read(pfgpu_csm* h, size_t first, size_t count, double* out) {
+    if (!h || !h->table_ok) return PFGPU_ERR_INVALID;
+    const size_t cells = (size_t)(h->TW * h->TH);
+    if (first > cells || count > cells - first || (count && !out)) return PFGPU_ERR_INVALID;
+    if (count == 0) return 0;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaMemcpyAsync(out, h->table + first, count * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    return 0;
+}
+extern "C" int pfgpu_csm_match(pfgpu_csm* h, const pfgpu_csm_config* c, const double* poses3, size_t Q, const double* qx, const double* qy,
+                               const uint64_t* offsets, pfgpu_csm_result* results) {
+    if (!h || !c) return PFGPU_ERR_INVALID;
+    if (Q == 0) return 0;
+    if (!poses3 || !offsets || !results || Q > ((size_t)1 << 32) || offsets[0] != 0) return PFGPU_ERR_INVALID;
+    if (!finite_d(c->linear_search_range) || !finite_d(c->angular_search_range) || !finite_d(c->linear_step) ||
+        !finite_d(c->angular_step) || !finite_d(c->grid_resolution))
+        return PFGPU_ERR_INVALID;
+    for (size_t q = 0; q < Q; ++q)
+        if (offsets[q + 1] < offsets[q] || !finite_d(poses3[3 * q]) || !finite_d(poses3[3 * q + 1]) || !finite_d(poses3[3 * q + 2]))
+            return PFGPU_ERR_INVALID;
+    const size_t K = (size_t)offsets[Q];
+    if (K && (!qx || !qy)) return PFGPU_ERR_INVALID;
+    for (size_t k = 0; k < K; ++k)
+        if (!finite_d(qx[k]) || !finite_d(qy[k])) return PFGPU_ERR_INVALID;
+    const double ls = c->linear_step, as = c->angular_step, res = c->grid_resolution;
+    // the reference's invalid input (:63-78)
+    const bool invalid = h->n == 0 || ls <= 0.0 || as <= 0.0 || res <= 0.0;
+    auto np = [&](size_t q) { return (size_t)(offsets[q + 1] - offsets[q]); };
+    size_t live = 0;
+    for (size_t q = 0; q < Q; ++q) {
+        if (invalid || np(q) == 0) results[q] = pfgpu_csm_result{poses3[3 * q], poses3[3 * q + 1], poses3[3 * q + 2], 0.0, 0u, 0u};
+        else ++live;
+    }
+    if (live == 0) return 0;
+    const int nl = csm_sat_i32(round(c->linear_search_range / ls)), na = csm_sat_i32(round(c->angular_search_range / as));
+    if (nl < 0 || na < 0) {                     // no candidate (:84-90)
+        for (size_t q = 0; q < Q; ++q)
+            if (np(q)) results[q] = pfgpu_csm_result{poses3[3 * q], poses3[3 * q + 1], fs_normalize_angle(poses3[3 * q + 2]), -1.0, 0u, 0u};
+        return 0;
+    }
+    const size_t NL = 2 * (size_t)nl + 1, NA = 2 * (size_t)na + 1;
+    if (nl > (1 << 15) || na > (1 << 22) || NL * NL * NA > ((size_t)1 << 34)) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "csm: %zu x %zu x %zu candidates per query exceed the caps", NL, NL, NA);
+        return PFGPU_ERR_UNSUPPORTED;
+    }
+    for (size_t q = 0; q < Q; ++q)
+        if (8 * NL * np(q) > h->ws_cap) {
+            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "csm: query %zu's cell indices for one yaw exceed %zu bytes", q, h->ws_cap);
+            return PFGPU_ERR_UNSUPPORTED;
+        }
+    int rc = pf_csm_table(h, res);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    Ctx& ctx = h->ctx;
+    const size_t ws_ints = h->ws_cap / 8;       // per array
+    size_t cap = h->ws_ints;
+    rc = csm_grow(&h->X, &cap, ws_ints);
+    if (!rc) { cap = h->ws_ints; rc = csm_grow(&h->Y, &cap, ws_ints); }
+    if (rc) { cudaFree(h->X); cudaFree(h->Y); h->X = h->Y = nullptr; h->ws_ints = 0; return rc; }
+    h->ws_ints = ws_ints;
+    if ((rc = csm_grow(&h->best, &h->best_cap, Q))) return rc;
+    // the queries with points: only they get score and reduce blocks (an empty one keeps the invalid result set above)
+    std::vector<unsigned long long> lq;
+    for (size_t q = 0; q < Q; ++q)
+        if (np(q)) lq.push_back(q);
+    PfScopedBuf dp, dx, dy, doff, dlive;
+    PF_CUDA(cudaMalloc(&dp.p, Q * 3 * sizeof(double)));
+    PF_CUDA(cudaMalloc(&doff.p, (Q + 1) * sizeof(unsigned long long)));
+    PF_CUDA(cudaMalloc(&dlive.p, lq.size() * sizeof(unsigned long long)));
+    PF_CUDA(cudaMemcpyAsync(dlive.p, lq.data(), lq.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, ctx.stream));
+    PF_CUDA(cudaMalloc(&dx.p, std::max<size_t>(K, 1) * sizeof(double)));
+    PF_CUDA(cudaMalloc(&dy.p, std::max<size_t>(K, 1) * sizeof(double)));
+    PF_CUDA(cudaMemcpyAsync(dp.p, poses3, Q * 3 * sizeof(double), cudaMemcpyHostToDevice, ctx.stream));
+    PF_CUDA(cudaMemcpyAsync(doff.p, offsets, (Q + 1) * sizeof(unsigned long long), cudaMemcpyHostToDevice, ctx.stream));
+    if (K) {
+        PF_CUDA(cudaMemcpyAsync(dx.p, qx, K * sizeof(double), cudaMemcpyHostToDevice, ctx.stream));
+        PF_CUDA(cudaMemcpyAsync(dy.p, qy, K * sizeof(double), cudaMemcpyHostToDevice, ctx.stream));
+    }
+    PF_LAUNCH(ctx, pf_csm_best_init_kernel, cdiv_u(Q, 256), 256, 0, h->best, Q);
+    PfCsmGeo g;
+    g.res = res; g.lstep = ls; g.ox = h->ox; g.oy = h->oy; g.TW = h->TW; g.TH = h->TH; g.nl = nl; g.NL = (int)NL;
+    const unsigned long long* off = (const unsigned long long*)doff.p;
+    const unsigned long long* dl = (const unsigned long long*)dlive.p;
+    size_t l0 = 0;                              // the group's first entry of lq
+    for (size_t q0 = 0; q0 < Q;) {
+        // a group of queries whose cell indices for one yaw fit the workspace
+        size_t q1 = q0, P = 0;
+        while (q1 < Q && q1 - q0 < 65535 && (8 * NL * (P + np(q1)) <= h->ws_cap)) P += np(q1++);
+        const size_t nq = q1 - q0, k0 = (size_t)offsets[q0];
+        size_t l1 = l0;
+        while (l1 < lq.size() && lq[l1] < q1) ++l1;
+        const size_t nlive = l1 - l0;
+        if (nlive == 0) { q0 = q1; continue; }
+        const size_t nac_ws = P ? std::max<size_t>(1, h->ws_cap / (8 * NL * P)) : NA;
+        const size_t nac = std::min(NA, nac_ws);
+        PfCsmBest* part = h->part;
+        for (size_t a0 = 0; a0 < NA; a0 += nac) {
+            const int n_a = (int)std::min(nac, NA - a0);
+            g.nac = n_a;
+            if ((rc = csm_grow(&h->cs, &h->cs_cap, nq * (size_t)n_a))) return rc;
+            PF_LAUNCH(ctx, pf_csm_trig_kernel, cdiv_u(nq * (size_t)n_a, 256), 256, 0, (const double*)dp.p, q0, nq, (long long)a0, n_a, na,
+                      as, h->cs);
+            if (P)
+                PF_LAUNCH(ctx, pf_csm_cells_kernel, cdiv_u(P * (size_t)n_a * NL, 256), 256, 0, g, (const double*)dp.p, (const double*)dx.p,
+                          (const double*)dy.p, off, q0, nq, k0, P, (const double2*)h->cs, h->X, h->Y);
+            const size_t per = NL * NL * (size_t)n_a;
+            const size_t nb = std::max<size_t>(1, std::min<size_t>(cdiv_u(per, PF_CSM_NT), PF_CSM_PART_CAP / nlive));
+            PF_LAUNCH(ctx, pf_csm_score_kernel, dim3((unsigned)nb, (unsigned)nlive), PF_CSM_NT, 0, g, (const double*)h->table, off, dl, l0,
+                      k0, (const int*)h->X, (const int*)h->Y, (long long)a0, na, as, part);
+            PF_LAUNCH(ctx, pf_csm_reduce_kernel, (unsigned)nlive, PF_CSM_NT, 0, (const PfCsmBest*)part, nb, dl, l0, h->best);
+        }
+        l0 = l1;
+        q0 = q1;
+    }
+    std::vector<PfCsmBest> best(Q);
+    PF_CUDA(cudaMemcpyAsync(best.data(), h->best, Q * sizeof(PfCsmBest), cudaMemcpyDeviceToHost, ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(ctx.stream));
+    for (size_t q = 0; q < Q; ++q) {
+        if (invalid || np(q) == 0) continue;
+        const unsigned long long i = best[q].idx;
+        const long long ia = (long long)(i % NA), iy = (long long)((i / NA) % NL), ix = (long long)(i / (NA * NL));
+        const double dxo = (double)(int)(ix - nl) * ls, dyo = (double)(int)(iy - nl) * ls, dyaw = (double)(int)(ia - na) * as;
+        results[q] = pfgpu_csm_result{poses3[3 * q] + dxo, poses3[3 * q + 1] + dyo, fs_normalize_angle(poses3[3 * q + 2] + dyaw),
+                                      best[q].score, best[q].score > 0.0 ? 1u : 0u, 0u};
+    }
+    return 0;
 }
 
 // ---- pose hypotheses: the cloud clustered in a fixed (x, y, yaw) histogram (DESIGN §3.10, pf_cluster.cuh) ----

@@ -113,6 +113,28 @@ pub struct pfgpu_ogm_stats {
 pub enum pfgpu_pf {}
 pub enum pfgpu_fs {}
 pub enum pfgpu_ogm {}
+/// CorrelativeScanMatcherConfig (pfgpu_csm_match; the reference's defaults 1.0, 0.2, 0.1, 0.02, 0.05)
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct pfgpu_csm_config {
+    pub linear_search_range: f64,
+    pub angular_search_range: f64,
+    pub linear_step: f64,
+    pub angular_step: f64,
+    pub grid_resolution: f64,
+}
+/// ScanMatchResult with converged as 0 / 1
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct pfgpu_csm_result {
+    pub x: f64,
+    pub y: f64,
+    pub yaw: f64,
+    pub score: f64,
+    pub converged: u32,
+    pub _pad: u32,
+}
+pub enum pfgpu_csm {}
 
 #[link(name = "pfgpu")]
 extern "C" {
@@ -164,6 +186,16 @@ extern "C" {
     pub fn pfgpu_ogm_info(h: *mut pfgpu_ogm, width: *mut usize, height: *mut usize, stats: *mut pfgpu_ogm_stats) -> c_int;
     pub fn pfgpu_pf_lfield_set_grid(h: *mut pfgpu_pf, grid: *const pfgpu_ogm, threshold: f64, cfg: *const pfgpu_lfield_config) -> c_int;
     pub fn pfgpu_pf_beam_set_grid(h: *mut pfgpu_pf, grid: *const pfgpu_ogm, threshold: f64, cfg: *const pfgpu_beam_config) -> c_int;
+    pub fn pfgpu_csm_create(device: c_int, out: *mut *mut pfgpu_csm) -> c_int;
+    pub fn pfgpu_csm_destroy(h: *mut pfgpu_csm);
+    pub fn pfgpu_csm_set_reference(h: *mut pfgpu_csm, x: *const f64, y: *const f64, n: usize) -> c_int;
+    pub fn pfgpu_csm_set_reference_grid(h: *mut pfgpu_csm, grid: *const pfgpu_ogm, threshold: f64) -> c_int;
+    pub fn pfgpu_csm_reference_size(h: *mut pfgpu_csm, n: *mut usize) -> c_int;
+    pub fn pfgpu_csm_match(h: *mut pfgpu_csm, cfg: *const pfgpu_csm_config, poses3: *const f64, n_queries: usize, qx: *const f64,
+                           qy: *const f64, offsets: *const u64, results: *mut pfgpu_csm_result) -> c_int;
+    pub fn pfgpu_csm_table_info(h: *mut pfgpu_csm, resolution: f64, origin_x: *mut i64, origin_y: *mut i64, width: *mut u64,
+                                height: *mut u64, radius: *mut i32) -> c_int;
+    pub fn pfgpu_csm_table_read(h: *mut pfgpu_csm, first: usize, count: usize, out: *mut f64) -> c_int;
     pub fn pfgpu_fs_default_config(cfg: *mut pfgpu_fs_config);
     pub fn pfgpu_fs_create(cfg: *const pfgpu_fs_config, n_particles: usize, n_landmarks: usize, seed: u64, device: c_int,
                            out: *mut *mut pfgpu_fs) -> c_int;

@@ -6,11 +6,13 @@
 //! `use rust_robotics_gpu::ParticleFilterLocalizer`.  Build: `cargo build -p rust_robotics_gpu` with libpfgpu.so built in-tree
 //! (pfgpu-sys/build.rs finds it; PFGPU_LIB_DIR overrides).  NOT COMPILED IN THIS REPOSITORY (no Rust toolchain in the build image):
 //! the identical C ABI is exercised by the C++ mirror (host/, run by tests) and the Python mirror (api.py).
+pub mod correlative_scan_matching;
 pub mod fastslam1;
 pub mod fastslam2;
 pub mod monte_carlo_localization;
 pub mod occupancy_grid_map;
 pub mod particle_filter;
+pub use correlative_scan_matching::{correlative_scan_match, CorrelativeScanMatcher, CorrelativeScanMatcherConfig, ScanMatchResult};
 pub use monte_carlo_localization::{MonteCarloLocalizationConfig, MonteCarloLocalizer};
 pub use occupancy_grid_map::{OccupancyGridConfig, OccupancyGridMap};
 pub use particle_filter::{ParticleFilterConfig, ParticleFilterLocalizer};
