@@ -11,8 +11,8 @@
 //
 // Bit-exactness: the three sums (S = sum w_raw, Q = sum w^2, the cumulative weights) are the reference's sequential f64 sums,
 // exactly (x3_core.h); the divisions are IEEE; the uniforms are the Philox stream the unfused path draws (same stream, call
-// counter and slot index); estimate / covariance are tolerance-level quantities (1e-6) summed in tree order, as in the unfused
-// path.  Fixed particle count, one GPU (the KLD-adaptive and the sharded forms keep the multi-kernel path).
+// counter and slot index); estimate / covariance are tolerance-level quantities (1e-6): central moments merged in a fixed tree
+// (include/pf_moments.h), as in the unfused path.  Fixed particle count, one GPU (the KLD-adaptive and the sharded forms keep the multi-kernel path).
 #pragma once
 #include "fs3.cuh"
 #include "pf_kernels.cuh"
@@ -24,12 +24,13 @@ struct Pf3Arg {
     uint64_t seed;
     unsigned K, m32;
     double* tsum; double* tsq;     // [tiles] tree-order tile sums of w_raw and w_raw^2 (steer the classification only)
-    double* mom;                   // [tiles][PF_MOM]
+    double* mom;                   // [tiles] PfMom
 };
 
 template <int NT>
 __global__ void __launch_bounds__(NT, 1)
 pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg a) {
+    static_assert(FS3_MAX_TILES <= NT, "the last CTA merges one tile partial per thread");
     extern __shared__ __align__(16) double vals[];            // [2][K][NT]: the tile's weights, their squares
     __shared__ Fs3Sh<NT> sh;
     const PfDev& pd = a.pd;
@@ -39,8 +40,6 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
     double* vals2 = vals + (size_t)K * NT;
     Fs3State* st = x.st;
     const int cur = *pd.cur;
-    // centre of the moment sums: the previous estimate (pf_moments_kernel)
-    const double c0 = pf_finite_or_zero(pd.scal[4]), c1 = pf_finite_or_zero(pd.scal[5]), c2 = pf_finite_or_zero(pd.scal[6]), c3 = pf_finite_or_zero(pd.scal[7]);
     // ---- this tile's raw weights; tile sums -> approximate prefixes in front of the tile ----
     double ts = 0.0, tq = 0.0;
 #pragma unroll 4
@@ -129,36 +128,21 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
             pd.w[t] = unif;                                    // w = 1/n pf.rs:468
         }
     }
-    // ---------------- estimate + covariance about the previous estimate (refresh_cache pf.rs:499-503), this tile's share ----------------
+    // ---------------- estimate + covariance (refresh_cache pf.rs:499-503): this tile's central moments ----------------
+    __shared__ PfMom smom[NT / 32];
     {
         const Pose4* pose = pf_pose(pd, gate ? cur ^ 1 : cur);
-        double acc[PF_MOM];
-#pragma unroll
-        for (int j = 0; j < PF_MOM; ++j) acc[j] = 0.0;
+        PfMom v = PF_MOM_EMPTY;
 #pragma unroll 1
         for (unsigned k = 0; k < K; ++k) {
             const size_t i = g0 + k;
             if (i >= n) break;
             Pose4 p;
             pose_load(pose, i, p);                             // (a resample step reads the clones this thread just wrote)
-            const double w = gate ? unif : vals[k * NT + tid];
-            const double e0 = p.x - c0, e1 = p.y - c1, e2 = p.yaw - c2, e3 = p.v - c3;
-            const double w0 = w * e0, w1 = w * e1, w2 = w * e2, w3 = w * e3;
-            acc[0] += w;
-            acc[1] += w0; acc[2] += w1; acc[3] += w2; acc[4] += w3;
-            acc[5] += w0 * e0; acc[6] += w0 * e1; acc[7] += w0 * e2; acc[8] += w0 * e3;
-            acc[9] += w1 * e1; acc[10] += w1 * e2; acc[11] += w1 * e3;
-            acc[12] += w2 * e2; acc[13] += w2 * e3;
-            acc[14] += w3 * e3;
+            pf_mom_add(&v, gate ? unif : vals[k * NT + tid], p.x, p.y, p.yaw, p.v);
         }
-        __syncthreads();
-#pragma unroll 1
-        for (int j = 0; j < PF_MOM; ++j) {
-            double x = fs3_warp_sum(acc[j]);
-            if ((tid & 31) == 0) sh.red[j & 1][tid >> 5] = x;
-            __syncthreads();
-            if (tid == 0) { double s = 0.0; for (int w = 0; w < NT / 32; ++w) s += sh.red[j & 1][w]; a.mom[(size_t)b * PF_MOM + j] = s; }
-        }
+        pf_mom_block_merge<NT>(v, smom);
+        if (tid == 0) pf_mom_store(a.mom + (size_t)b * PF_MOM, v);
     }
     // ---------------- completion: the last CTA reduces the moments, flips the state, resets the counters ----------------
     __syncthreads();
@@ -167,27 +151,11 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
     if (!sh.last) return;
     if (tid < FS3_SLOTS) { x.flagsg[tid] = 0; x.entCnt[tid] = 0u; }
     if (tid < FS3_ROUNDS) { x.bar[tid] = 0u; x.resflag[tid] = 0u; }
-    if (tid < PF_MOM) {
-        double s = 0.0;
-#pragma unroll 1
-        for (unsigned c = 0; c < nt; ++c) s += __ldcg(a.mom + (size_t)c * PF_MOM + tid);
-        sh.bef[tid] = s;
-    }
-    __syncthreads();
+    PfMom v = PF_MOM_EMPTY;                                    // thread t takes tile t (nt <= FS3_MAX_TILES <= NT), then the block tree
+    if ((unsigned)tid < nt) pf_mom_load(a.mom + (size_t)tid * PF_MOM, v);
+    pf_mom_block_merge<NT>(v, smom);
     if (tid == 0) {
-        // pf_moments_final_kernel: est = c + M1, cov about est from the moments about c
-        const double W = sh.bef[0];
-        const double c[4] = { c0, c1, c2, c3 };
-        const double M1[4] = { sh.bef[1], sh.bef[2], sh.bef[3], sh.bef[4] };
-        double M2[4][4];
-        int q = 5;
-        for (int i = 0; i < 4; ++i) for (int j = i; j < 4; ++j) { M2[i][j] = sh.bef[q]; M2[j][i] = sh.bef[q]; q++; }
-        for (int i = 0; i < 4; ++i) pd.scal[4 + i] = c[i] * W + M1[i];
-        for (int i = 0; i < 4; ++i)
-            for (int j = 0; j < 4; ++j) {
-                const double ea = c[i] * (W - 1.0) + M1[i], eb = c[j] * (W - 1.0) + M1[j];
-                pd.scal[8 + i * 4 + j] = M2[i][j] - M1[i] * eb - ea * M1[j] + W * ea * eb;
-            }
+        pf_mom_final(&v, pd.scal + 4, pd.scal + 8);
         pd.scal[0] = S; pd.scal[1] = Q; pd.scal[2] = ctot; pd.scal[3] = neff;
         *pd.gate = gate;
         if (gate) { *pd.cur = cur ^ 1; pd.counters[0] += 1; }      // pf_flip_kernel

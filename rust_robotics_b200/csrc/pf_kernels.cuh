@@ -12,11 +12,11 @@
 #pragma once
 #include "common.cuh"
 #include "xsum.cuh"
+#include "../../include/pf_moments.h"
 
 struct __align__(32) Pose4 { double x, y, yaw, v; };
 
 #define PF_NT 256
-#define PF_MOM 15              // sum w, 4 first moments, 10 second moments (upper triangle)
 
 struct PfDev {
     size_t n = 0, n_global = 0, offset = 0;
@@ -28,7 +28,7 @@ struct PfDev {
     uint32_t* idx = nullptr;
     double* scal = nullptr;        // [0] S=sum w_raw  [1] Q=sum w^2  [2] cum total  [3] neff  [4..7] est  [8..23] cov (row-major)
     int* gate = nullptr;           // device: 1 if this step resamples
-    double* partial = nullptr;     // [blocks][PF_MOM]
+    double* partial = nullptr;     // [blocks] PfMom
     double* obs = nullptr;         // device copy of the observation list (k x 3) when it does not fit the launch parameters
     unsigned int* counters = nullptr;   // device: [0] resamples done so far (= Philox call index of the next resample)
 };
@@ -277,65 +277,83 @@ __global__ void __launch_bounds__(PF_NT) pf_gather_kernel(PfDev d) {
 }
 __global__ void pf_flip_kernel(PfDev d) { if (*d.gate) { *d.cur ^= 1; d.counters[0] += 1; } }
 
-__device__ __forceinline__ double pf_finite_or_zero(double c) { return (c - c == 0.0) ? c : 0.0; }
-// compute_estimate + compute_covariance (pf.rs:382-413) in one pass with a shifted centre c (the previous
-// estimate): sum w, sum w(p-c), sum w(p-c)(p-c)^T; finalised by pf_moments_final_kernel.  Tolerance-level
-// quantity (1e-6): summed in tree order, not in the reference's sequential order.
+// thread 0 receives the block's PfMom values merged in a fixed tree: lanes by shuffle, then the warps in order
+template <int NT>
+__device__ __forceinline__ void pf_mom_block_merge(PfMom& v, PfMom* sm /* [NT / 32] */) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        PfMom u;
+        u.w = __shfl_down_sync(0xffffffffu, v.w, o);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) u.m[k] = __shfl_down_sync(0xffffffffu, v.m[k], o);
+#pragma unroll
+        for (int k = 0; k < 10; ++k) u.q[k] = __shfl_down_sync(0xffffffffu, v.q[k], o);
+        pf_mom_merge(&v, &u);
+    }
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int w = 1; w < NT / 32; ++w) pf_mom_merge(&v, &sm[w]);
+}
+__device__ __forceinline__ void pf_mom_store(double* dst, const PfMom& v) {
+    dst[0] = v.w;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) dst[1 + k] = v.m[k];
+#pragma unroll
+    for (int k = 0; k < 10; ++k) dst[5 + k] = v.q[k];
+}
+__device__ __forceinline__ void pf_mom_load(const double* src, PfMom& v) {
+    v.w = __ldcg(src);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) v.m[k] = __ldcg(src + 1 + k);
+#pragma unroll
+    for (int k = 0; k < 10; ++k) v.q[k] = __ldcg(src + 5 + k);
+}
+#define PF_MOM_EMPTY { 0.0, { 0.0, 0.0, 0.0, 0.0 }, { 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0 } }
+
+// compute_estimate + compute_covariance (pf.rs:382-413) as weighted central moments (include/pf_moments.h): thread t merges
+// particles t, t + nblocks * PF_NT, ... one at a time, the block merges its threads in a fixed tree, one PfMom per block.
+// Tolerance-level quantity: the merge order is fixed by (n, nblocks), not the reference's sequential order.
 __global__ void __launch_bounds__(PF_NT) pf_moments_kernel(PfDev d, int nblocks) {
-    __shared__ double sm[PF_NT / 32];
+    __shared__ PfMom sm[PF_NT / 32];
     const Pose4* pose = pf_pose(d, *d.cur);
-    // centre = previous estimate, or 0 when that is not finite (an overflowed pose must not poison every later estimate:
-    // the reference's refresh_cache recomputes from scratch, pf.rs:382-413).  pf_moments_final_kernel applies the same rule.
-    const double c0 = pf_finite_or_zero(d.scal[4]), c1 = pf_finite_or_zero(d.scal[5]), c2 = pf_finite_or_zero(d.scal[6]), c3 = pf_finite_or_zero(d.scal[7]);
-    double acc[PF_MOM];
+    PfMom v = PF_MOM_EMPTY;
+    const size_t stride = (size_t)nblocks * PF_NT;
+    constexpr int B = 4;                               // particles in flight per thread (the merges are one dependent chain)
+    for (size_t i = (size_t)blockIdx.x * PF_NT + threadIdx.x; i < d.n; i += B * stride) {
+        Pose4 p[B];
+        double w[B];
 #pragma unroll
-    for (int k = 0; k < PF_MOM; ++k) acc[k] = 0.0;
-    for (size_t i = (size_t)blockIdx.x * PF_NT + threadIdx.x; i < d.n; i += (size_t)nblocks * PF_NT) {
-        Pose4 p;
-        pose_load(pose, i, p);
-        double w = d.w[i];
-        double e0 = p.x - c0, e1 = p.y - c1, e2 = p.yaw - c2, e3 = p.v - c3;
-        double w0 = w * e0, w1 = w * e1, w2 = w * e2, w3 = w * e3;
-        acc[0] += w;
-        acc[1] += w0; acc[2] += w1; acc[3] += w2; acc[4] += w3;
-        acc[5] += w0 * e0; acc[6] += w0 * e1; acc[7] += w0 * e2; acc[8] += w0 * e3;
-        acc[9] += w1 * e1; acc[10] += w1 * e2; acc[11] += w1 * e3;
-        acc[12] += w2 * e2; acc[13] += w2 * e3;
-        acc[14] += w3 * e3;
-    }
+        for (int b = 0; b < B; ++b)
+            if (i + b * stride < d.n) { pose_load(pose, i + b * stride, p[b]); w[b] = d.w[i + b * stride]; }
 #pragma unroll
-    for (int k = 0; k < PF_MOM; ++k) {
-        double t = block_sum<PF_NT>(acc[k], sm);
-        if (threadIdx.x == 0) d.partial[(size_t)blockIdx.x * PF_MOM + k] = t;
+        for (int b = 0; b < B; ++b)
+            if (i + b * stride < d.n) pf_mom_add(&v, w[b], p[b].x, p[b].y, p[b].yaw, p[b].v);
     }
+    pf_mom_block_merge<PF_NT>(v, sm);
+    if (threadIdx.x == 0) pf_mom_store(d.partial + (size_t)blockIdx.x * PF_MOM, v);
 }
-// one CTA: reduce the per-block partials; out = moments about the centre (15 doubles)
-__global__ void __launch_bounds__(PF_NT) pf_moments_reduce_kernel(const double* partial, int nblocks, double* out15) {
-    __shared__ double sm[PF_NT / 32];
-    for (int k = 0; k < PF_MOM; ++k) {
-        double a = 0.0;
-        for (int b = threadIdx.x; b < nblocks; b += PF_NT) a += partial[(size_t)b * PF_MOM + k];
-        double t = block_sum<PF_NT>(a, sm);
-        if (threadIdx.x == 0) out15[k] = t;
+// one CTA: thread t merges block partials t, t + PF_NT, ... in order, then the block tree; out = this shard's PfMom
+__global__ void __launch_bounds__(PF_NT) pf_moments_reduce_kernel(const double* partial, int nblocks, double* out) {
+    __shared__ PfMom sm[PF_NT / 32];
+    PfMom v = PF_MOM_EMPTY;
+    for (int b = threadIdx.x; b < nblocks; b += PF_NT) {
+        PfMom u;
+        pf_mom_load(partial + (size_t)b * PF_MOM, u);
+        pf_mom_merge(&v, &u);
     }
+    pf_mom_block_merge<PF_NT>(v, sm);
+    if (threadIdx.x == 0) pf_mom_store(out, v);
 }
-// est = c + M1 (weights are normalised: sum w = 1 up to rounding; the reference does not divide either),
-// cov_ij = M2_ij - M1_i*m_j - m_i*M1_j + W*m_i*m_j  with m = est - c, which equals sum w (p-est)(p-est)^T.
-__global__ void pf_moments_final_kernel(PfDev d, const double* mom15) {
+// the shards' PfMom (one per rank, gathered) merged in rank order; est -> scal[4..7], cov -> scal[8..23] (row-major)
+__global__ void pf_moments_final_kernel(PfDev d, const double* mom, int shards) {
     if (threadIdx.x != 0) return;
-    const double W = mom15[0];
-    double c[4] = { pf_finite_or_zero(d.scal[4]), pf_finite_or_zero(d.scal[5]), pf_finite_or_zero(d.scal[6]), pf_finite_or_zero(d.scal[7]) };
-    double M1[4] = { mom15[1], mom15[2], mom15[3], mom15[4] };
-    double M2[4][4];
-    int q = 5;
-    for (int a = 0; a < 4; ++a) for (int b = a; b < 4; ++b) { M2[a][b] = mom15[q]; M2[b][a] = mom15[q]; q++; }
-    double m[4];
-    for (int a = 0; a < 4; ++a) m[a] = M1[a];            // est - c = sum w (p - c)   (exactly what sum w*p - c*W gives for W=1)
-    for (int a = 0; a < 4; ++a) d.scal[4 + a] = c[a] * W + M1[a];   // = sum w*p
-    for (int a = 0; a < 4; ++a)
-        for (int b = 0; b < 4; ++b) {
-            // deviations about est: (p - est) = (p - c) - (est - c), est - c = c*(W-1) + M1
-            double ea = c[a] * (W - 1.0) + m[a], eb = c[b] * (W - 1.0) + m[b];
-            d.scal[8 + a * 4 + b] = M2[a][b] - M1[a] * eb - ea * M1[b] + W * ea * eb;
-        }
+    PfMom v;
+    pf_mom_load(mom, v);
+    for (int r = 1; r < shards; ++r) {
+        PfMom u;
+        pf_mom_load(mom + (size_t)r * PF_MOM, u);
+        pf_mom_merge(&v, &u);
+    }
+    pf_mom_final(&v, d.scal + 4, d.scal + 8);
 }

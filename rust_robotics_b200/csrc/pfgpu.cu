@@ -124,7 +124,7 @@ struct pfgpu_pf {
     PfDev d;
     XsWork xs;
     size_t obs_cap = 0;
-    double* mom15 = nullptr;
+    double* mom = nullptr;     // [world] PfMom: every shard's estimate moments
     int mom_blocks = 0;
     uint32_t n_predict = 0, n_resample = 0;
     uint64_t steps = 0, resamples_unknown = 0;
@@ -260,11 +260,12 @@ __global__ void pf_pack_kernel(PfDev d, double* aos5) {
 }
 
 static int pf_refresh_cache(pfgpu_pf* h) {      // refresh_cache pf.rs:499-503
+    double* own = h->mom + (size_t)h->rank * PF_MOM;
     PF_LAUNCH(h->ctx, pf_moments_kernel, h->mom_blocks, PF_NT, 0, h->d, h->mom_blocks);
-    PF_LAUNCH(h->ctx, pf_moments_reduce_kernel, 1, PF_NT, 0, h->d.partial, h->mom_blocks, h->mom15);
-    if (h->world > 1)   // shard moments about the common centre (the previous, replicated estimate) add up
-        PF_NCCL(ncclAllReduce(h->mom15, h->mom15, PF_MOM, ncclDouble, ncclSum, h->sh.comm, h->ctx.stream));
-    PF_LAUNCH(h->ctx, pf_moments_final_kernel, 1, 32, 0, h->d, h->mom15);
+    PF_LAUNCH(h->ctx, pf_moments_reduce_kernel, 1, PF_NT, 0, h->d.partial, h->mom_blocks, own);
+    if (h->world > 1)   // every rank gathers every shard's moments and merges them in rank order: the same bits on every rank
+        PF_NCCL(ncclAllGather(own, h->mom, PF_MOM, ncclDouble, h->sh.comm, h->ctx.stream));
+    PF_LAUNCH(h->ctx, pf_moments_final_kernel, 1, 32, 0, h->d, h->mom, h->world);
     return 0;
 }
 // augmented MCL: w_slow = w_fast = p = 0, injection count 0, disarmed
@@ -300,7 +301,7 @@ static int pf_alloc(pfgpu_pf* h, size_t cap) {
     h->mom_blocks = (int)std::min<size_t>((size_t)h->ctx.num_sms * 4, cdiv_u(n, PF_NT));
     if (h->mom_blocks < 1) h->mom_blocks = 1;
     PF_CUDA(cudaMalloc(&d.partial, (size_t)h->mom_blocks * PF_MOM * sizeof(double)));
-    PF_CUDA(cudaMalloc(&h->mom15, PF_MOM * sizeof(double)));
+    PF_CUDA(cudaMalloc(&h->mom, (size_t)h->world * PF_MOM * sizeof(double)));
     h->obs_cap = 1024;
     PF_CUDA(cudaMalloc(&d.obs, h->obs_cap * 3 * sizeof(double)));
     PF_CUDA(cudaMallocHost(&h->h_pin, 64 * sizeof(double)));
@@ -409,7 +410,7 @@ extern "C" void pfgpu_pf_destroy(pfgpu_pf* h) {
     if (h->ctx.stream) cudaStreamSynchronize(h->ctx.stream);
     PfDev& d = h->d;
     cudaFree(d.pose[0]); cudaFree(d.pose[1]); cudaFree(d.cur); cudaFree(d.w_raw); cudaFree(d.w); cudaFree(d.cum);
-    cudaFree(d.idx); cudaFree(d.scal); cudaFree(d.gate); cudaFree(d.partial); cudaFree(d.obs); cudaFree(h->mom15); cudaFree(d.counters);
+    cudaFree(d.idx); cudaFree(d.scal); cudaFree(d.gate); cudaFree(d.partial); cudaFree(d.obs); cudaFree(h->mom); cudaFree(d.counters);
     cudaFree(h->lf.D); cudaFree(h->lf.q); cudaFree(h->bm.clr);
     if (h->h_pin) cudaFreeHost(h->h_pin);
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
