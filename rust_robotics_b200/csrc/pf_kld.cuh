@@ -33,13 +33,19 @@ __device__ __forceinline__ int pf_sat_i32(double v) {          // Rust `as i32`:
     return (int)v;
 }
 
-__global__ void __launch_bounds__(PF_NT) pf_kld_draw_kernel(PfDev d, uint64_t seed, PfKld k) {
+// `bad`: the scan of the cumulative weights saw a negative, infinite or NaN weight (xs flags[3]); then the CDF may go down or
+// hold NaN, and each draw scans linearly as the reference does (pf_search_kernel)
+__global__ void __launch_bounds__(PF_NT) pf_kld_draw_kernel(PfDev d, uint64_t seed, PfKld k, const int* bad) {
     const size_t t = (size_t)blockIdx.x * PF_NT + threadIdx.x;
     if (t >= k.cap) return;
     const uint32_t call = d.counters[0];
     const double r = pfc_u01_53(pfc_blk_u64(pfc_rng_block(seed, PFC_STREAM_PF_RESAMPLE, call, t), 0));
     const double* __restrict__ c = d.cum;
     size_t lo = 0, hi = d.n;
+    if (*bad) {
+        while (lo < d.n && !(r <= c[lo])) ++lo;
+        hi = lo;
+    }
     while (lo < hi) {
         size_t mid = lo + ((hi - lo) >> 1);
         if (c[mid] < r) lo = mid + 1; else hi = mid;

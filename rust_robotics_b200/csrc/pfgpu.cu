@@ -693,7 +693,7 @@ static int pf_resample_adaptive(pfgpu_pf* h) {
     PF_LAUNCH(ctx, pf_force_last_kernel, 1, 1, 0, d);                                             // mcl.rs:334-336
     PF_CUDA(cudaMemsetAsync(k.owner, 0xFF, (size_t)k.tcap * sizeof(int), ctx.stream));
     PF_CUDA(cudaMemsetAsync(k.mint, 0xFF, (size_t)k.tcap * sizeof(unsigned), ctx.stream));
-    PF_LAUNCH(ctx, pf_kld_draw_kernel, cdiv_u(k.cap, PF_NT), PF_NT, 0, d, h->seed, k);
+    PF_LAUNCH(ctx, pf_kld_draw_kernel, cdiv_u(k.cap, PF_NT), PF_NT, 0, d, h->seed, k, h->xs.flags + 3);
     PF_LAUNCH(ctx, pf_kld_insert_kernel, cdiv_u(k.cap, PF_NT), PF_NT, 0, k);
     PF_LAUNCH(ctx, pf_kld_stop_kernel, 1, 1024, 0, k, (unsigned long long)h->cfg.n_particles, (unsigned long long)h->cfg.max_particles,
               h->cfg.kld_epsilon, h->cfg.kld_z);
