@@ -271,6 +271,14 @@ def _dp(a):
     return a.ctypes.data_as(c_dp)
 
 
+def _obstacle_mask(obstacles):
+    """(pointer, W, H) of obstacles[ix, iy] != 0 as a uint8 mask (the pointer keeps the mask alive)"""
+    m = np.ascontiguousarray(np.asarray(obstacles) != 0, dtype=np.uint8)
+    if m.ndim != 2:
+        raise InvalidParameter("obstacles: a 2-D (W, H) mask")
+    return m.ctypes.data_as(C.POINTER(C.c_uint8)), m.shape[0], m.shape[1]
+
+
 # ------------------------------------------------------------------------------------------------
 class ParticleFilterConfig:
     """pf.rs:50-78"""
@@ -474,19 +482,33 @@ class _PfBase:
         f.init_region(region)
         return f
 
+    # -- what the two scan models share: fn is the model's C entry point --
+    def _set_map(self, fn, source, cfg_type, resolution, *params, max_beams):
+        """load a map from source = _obstacle_mask(...) or (grid handle, threshold) with the config (resolution, *params, max_beams)"""
+        if not (max_beams >= 2 and max_beams < 2 ** 32):
+            raise InvalidParameter("max_beams >= 2")
+        cfg = cfg_type(float(resolution), *(float(v) for v in params), int(max_beams), 0)
+        _check(self.L, fn(self.h, *source, C.byref(cfg)))
+
+    def _update_scan(self, fn, ranges, angle_min, angle_increment):
+        r = _f64(ranges).ravel()
+        _check(self.L, fn(self.h, _dp(r), r.size, float(angle_min), float(angle_increment)))
+
+    def _step_scan(self, fn, control, ranges, angle_min, angle_increment, want_estimate):
+        u = control if isinstance(control, np.ndarray) and control.dtype == np.float64 else _f64(control)
+        r = _f64(ranges).ravel()
+        est = np.empty(4)
+        _check(self.L, fn(self.h, _dp(u), _dp(r), r.size, float(angle_min), float(angle_increment), _dp(est) if want_estimate else None))
+        return est if want_estimate else None
+
     # -- likelihood-field scan model (not in the reference, whose MCL only ranges to known landmarks; DESIGN §3.9) --
     def set_likelihood_field(self, obstacles, resolution, sigma_hit=0.2, z_hit=0.95, z_rand=0.05, max_range=30.0, max_beams=60):
         """Load an occupancy map for scan updates: obstacles[ix, iy] (W x H, nonzero = obstacle; obstacles_from_log_odds turns an
         OccupancyGridMap's log-odds into one), `resolution` metres per cell, world (0, 0) at the grid centre.  Builds the distance
         field and the per-cell likelihood q = z_hit * N(d; 0, sigma_hit) + z_rand / max_range on the device (ROS AMCL's
         likelihood_field with its defaults).  On a sharded engine every rank makes the same call."""
-        m = np.ascontiguousarray(np.asarray(obstacles) != 0, dtype=np.uint8)
-        if m.ndim != 2:
-            raise InvalidParameter("obstacles: a 2-D (W, H) mask")
-        if not (max_beams >= 2 and max_beams < 2 ** 32):
-            raise InvalidParameter("max_beams >= 2")
-        cfg = _LfCfg(float(resolution), float(sigma_hit), float(z_hit), float(z_rand), float(max_range), int(max_beams), 0)
-        _check(self.L, self.L.pfgpu_pf_lfield_set(self.h, m.ctypes.data_as(C.POINTER(C.c_uint8)), m.shape[0], m.shape[1], C.byref(cfg)))
+        self._set_map(self.L.pfgpu_pf_lfield_set, _obstacle_mask(obstacles), _LfCfg, resolution, sigma_hit, z_hit, z_rand, max_range,
+                      max_beams=max_beams)
 
     def clear_likelihood_field(self):
         _check(self.L, self.L.pfgpu_pf_lfield_clear(self.h))
@@ -509,19 +531,13 @@ class _PfBase:
     def try_update_with_scan(self, ranges, angle_min, angle_increment):
         """The measurement update from a laser scan (ranges[i] at angle_min + i * angle_increment from the heading; the
         convention of OccupancyGridMap::update_with_scan): every particle's weight becomes the likelihood field of the used beams"""
-        r = _f64(ranges).ravel()
-        _check(self.L, self.L.pfgpu_pf_update_scan(self.h, _dp(r), r.size, float(angle_min), float(angle_increment)))
+        self._update_scan(self.L.pfgpu_pf_update_scan, ranges, angle_min, angle_increment)
 
     update_with_scan = try_update_with_scan
 
     def try_step_scan(self, control, ranges, angle_min, angle_increment, want_estimate=True):
         """try_step with a laser scan in place of the landmark observations"""
-        u = control if isinstance(control, np.ndarray) and control.dtype == np.float64 else _f64(control)
-        r = _f64(ranges).ravel()
-        est = np.empty(4)
-        _check(self.L, self.L.pfgpu_pf_step_scan(self.h, _dp(u), _dp(r), r.size, float(angle_min), float(angle_increment),
-                                                 _dp(est) if want_estimate else None))
-        return est if want_estimate else None
+        return self._step_scan(self.L.pfgpu_pf_step_scan, control, ranges, angle_min, angle_increment, want_estimate)
 
     step_scan = try_step_scan
 
@@ -532,34 +548,23 @@ class _PfBase:
         obstacle, `resolution` metres per cell, world (0, 0) at the grid centre).  Every particle's expected range along every used
         beam is ray-cast in the map and compared with the measured one (ROS AMCL's beam model with its defaults).  Builds the
         clearance table on the device.  Separate from the likelihood field; on a sharded engine every rank makes the same call."""
-        m = np.ascontiguousarray(np.asarray(obstacles) != 0, dtype=np.uint8)
-        if m.ndim != 2:
-            raise InvalidParameter("obstacles: a 2-D (W, H) mask")
-        if not (max_beams >= 2 and max_beams < 2 ** 32):
-            raise InvalidParameter("max_beams >= 2")
-        cfg = _BmCfg(float(resolution), float(sigma_hit), float(z_hit), float(z_short), float(z_max), float(z_rand), float(lambda_short),
-                     float(max_range), int(max_beams), 0)
-        _check(self.L, self.L.pfgpu_pf_beam_set(self.h, m.ctypes.data_as(C.POINTER(C.c_uint8)), m.shape[0], m.shape[1], C.byref(cfg)))
+        self._set_map(self.L.pfgpu_pf_beam_set, _obstacle_mask(obstacles), _BmCfg, resolution, sigma_hit, z_hit, z_short, z_max, z_rand,
+                      lambda_short, max_range, max_beams=max_beams)
 
     def set_likelihood_field_from_grid(self, grid_map, threshold=0.5, sigma_hit=0.2, z_hit=0.95, z_rand=0.05, max_range=30.0,
                                        max_beams=60):
         """set_likelihood_field(grid_map.obstacles(threshold), grid_map.config.resolution, ...) without leaving the device: the
         OccupancyGridMap's obstacle mask is built on the device and the same table is loaded.  The grid is copied now: later
         updates of grid_map do not change the loaded field.  grid_map must live on this filter's device."""
-        if not (max_beams >= 2 and max_beams < 2 ** 32):
-            raise InvalidParameter("max_beams >= 2")
-        cfg = _LfCfg(float(grid_map.config.resolution), float(sigma_hit), float(z_hit), float(z_rand), float(max_range), int(max_beams), 0)
-        _check(self.L, self.L.pfgpu_pf_lfield_set_grid(self.h, grid_map.h, float(threshold), C.byref(cfg)))
+        self._set_map(self.L.pfgpu_pf_lfield_set_grid, (grid_map.h, float(threshold)), _LfCfg, grid_map.config.resolution, sigma_hit, z_hit,
+                      z_rand, max_range, max_beams=max_beams)
 
     def set_beam_model_from_grid(self, grid_map, threshold=0.5, sigma_hit=0.2, z_hit=0.95, z_short=0.1, z_max=0.05, z_rand=0.05,
                                  lambda_short=0.1, max_range=30.0, max_beams=60):
         """set_beam_model(grid_map.obstacles(threshold), grid_map.config.resolution, ...) without leaving the device (see
         set_likelihood_field_from_grid)"""
-        if not (max_beams >= 2 and max_beams < 2 ** 32):
-            raise InvalidParameter("max_beams >= 2")
-        cfg = _BmCfg(float(grid_map.config.resolution), float(sigma_hit), float(z_hit), float(z_short), float(z_max), float(z_rand),
-                     float(lambda_short), float(max_range), int(max_beams), 0)
-        _check(self.L, self.L.pfgpu_pf_beam_set_grid(self.h, grid_map.h, float(threshold), C.byref(cfg)))
+        self._set_map(self.L.pfgpu_pf_beam_set_grid, (grid_map.h, float(threshold)), _BmCfg, grid_map.config.resolution, sigma_hit, z_hit,
+                      z_short, z_max, z_rand, lambda_short, max_range, max_beams=max_beams)
 
     def clear_beam_model(self):
         _check(self.L, self.L.pfgpu_pf_beam_clear(self.h))
@@ -581,19 +586,13 @@ class _PfBase:
 
     def try_update_with_beam_scan(self, ranges, angle_min, angle_increment):
         """try_update_with_scan under the beam model"""
-        r = _f64(ranges).ravel()
-        _check(self.L, self.L.pfgpu_pf_update_beam(self.h, _dp(r), r.size, float(angle_min), float(angle_increment)))
+        self._update_scan(self.L.pfgpu_pf_update_beam, ranges, angle_min, angle_increment)
 
     update_with_beam_scan = try_update_with_beam_scan
 
     def try_step_beam_scan(self, control, ranges, angle_min, angle_increment, want_estimate=True):
         """try_step with a laser scan under the beam model"""
-        u = control if isinstance(control, np.ndarray) and control.dtype == np.float64 else _f64(control)
-        r = _f64(ranges).ravel()
-        est = np.empty(4)
-        _check(self.L, self.L.pfgpu_pf_step_beam(self.h, _dp(u), _dp(r), r.size, float(angle_min), float(angle_increment),
-                                                 _dp(est) if want_estimate else None))
-        return est if want_estimate else None
+        return self._step_scan(self.L.pfgpu_pf_step_beam, control, ranges, angle_min, angle_increment, want_estimate)
 
     step_beam_scan = try_step_beam_scan
 

@@ -16,6 +16,7 @@
 #include <cmath>
 #include <algorithm>
 #include <cfloat>
+#include <type_traits>
 
 thread_local char g_pfgpu_err[512] = {0};
 
@@ -117,13 +118,19 @@ struct KernelTimer {
 // ====================================================================================================
 // ParticleFilterLocalizer / MonteCarloLocalizer
 // ====================================================================================================
+// what the map of either scan model has in common; on = a map is loaded
+struct PfMap {
+    bool on = false;
+    size_t W = 0, H = 0;
+    uint64_t L = 0;                // the most used beams a scan may have
+};
 struct pfgpu_pf {
     Ctx ctx;
     pfgpu_pf_config cfg;
     uint64_t seed = 0;
     PfDev d;
     XsWork xs;
-    size_t obs_cap = 0;
+    size_t obs_cap = 0;        // the doubles d.obs holds
     double* mom = nullptr;     // [world] PfMom: every shard's estimate moments
     int mom_blocks = 0;
     uint32_t n_predict = 0, n_resample = 0;
@@ -167,24 +174,22 @@ struct pfgpu_pf {
         double a_slow = 0.0, a_fast = 0.0;
         double region[4] = {0.0, 0.0, 0.0, 0.0};     // x0, x1, y0, y1
     } rec;
-    // likelihood-field scan model (DESIGN §3.9): the map's tables and parameters; on = a map is loaded
-    struct LField {
-        bool on = false;
-        size_t W = 0, H = 0;
-        uint64_t L = 0;            // the most used beams a scan may have
+    // likelihood-field scan model (DESIGN §3.9): the map's tables and parameters
+    struct LField : PfMap {
         double* D = nullptr;       // distance field [cells], ix * H + iy
         double* q = nullptr;       // per-cell factor
         pfgpu_lfield_config cfg = {};
         double q_out = 0.0;
+        bool keep_max() const { return false; }
+        void release() { cudaFree(D); cudaFree(q); *this = LField(); }
     } lf;
-    // beam model (DESIGN §3.11): the clearance table and parameters; on = a map is loaded.  Separate from the likelihood field's.
-    struct BeamMap {
-        bool on = false;
-        size_t W = 0, H = 0;
-        uint64_t L = 0;            // the most used beams a scan may have
+    // beam model (DESIGN §3.11): the clearance table and parameters.  Separate from the likelihood field's.
+    struct BeamMap : PfMap {
         unsigned char* clr = nullptr;   // clearance [cells], ix * H + iy
         pfgpu_beam_config cfg = {};
         int skip = 1;              // PFGPU_BEAM_SKIP=0 at set time: the caster steps one cell at a time
+        bool keep_max() const { return cfg.z_max > 0.0; }      // max readings are used beams (as r = max_range)
+        void release() { cudaFree(clr); *this = BeamMap(); }
     } bm;
     std::vector<double> pairs;     // the used beams of the current scan call (either model): (r_i, a_i)
     PfClu clu;                     // pose hypotheses' workspace (DESIGN §3.10), allocated by the first query
@@ -302,8 +307,8 @@ static int pf_alloc(pfgpu_pf* h, size_t cap) {
     if (h->mom_blocks < 1) h->mom_blocks = 1;
     PF_CUDA(cudaMalloc(&d.partial, (size_t)h->mom_blocks * PF_MOM * sizeof(double)));
     PF_CUDA(cudaMalloc(&h->mom, (size_t)h->world * PF_MOM * sizeof(double)));
-    h->obs_cap = 1024;
-    PF_CUDA(cudaMalloc(&d.obs, h->obs_cap * 3 * sizeof(double)));
+    PF_CUDA(cudaMalloc(&d.obs, 3 * 1024 * sizeof(double)));
+    h->obs_cap = 3 * 1024;
     PF_CUDA(cudaMallocHost(&h->h_pin, 64 * sizeof(double)));
     if (h->adaptive) {
         PfKld& k = h->kld;
@@ -411,7 +416,7 @@ extern "C" void pfgpu_pf_destroy(pfgpu_pf* h) {
     PfDev& d = h->d;
     cudaFree(d.pose[0]); cudaFree(d.pose[1]); cudaFree(d.cur); cudaFree(d.w_raw); cudaFree(d.w); cudaFree(d.cum);
     cudaFree(d.idx); cudaFree(d.scal); cudaFree(d.gate); cudaFree(d.partial); cudaFree(d.obs); cudaFree(h->mom); cudaFree(d.counters);
-    cudaFree(h->lf.D); cudaFree(h->lf.q); cudaFree(h->bm.clr);
+    h->lf.release(); h->bm.release();
     if (h->h_pin) cudaFreeHost(h->h_pin);
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
@@ -444,17 +449,17 @@ extern "C" int pfgpu_pf_init_state(pfgpu_pf* h, const double s[4]) {
     if (h->rec.on) { int rc = pf_recovery_reset(h); if (rc) return rc; }
     return pf_refresh_cache(h);
 }
-// device temporary of the bulk transfers: released on every exit path (PF_CUDA / PF_LAUNCH return early on errors)
-struct PfScopedDev {
-    double* p = nullptr;
-    ~PfScopedDev() { if (p) cudaFree(p); }
+// a device temporary: released on every exit path (PF_CUDA / PF_LAUNCH return early on errors)
+struct PfScopedBuf {
+    void* p = nullptr;
+    ~PfScopedBuf() { if (p) cudaFree(p); }
 };
 extern "C" int pfgpu_pf_upload(pfgpu_pf* h, const double* aos5, size_t n) {
     if (!h || !aos5 || n != h->d.n) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
-    PfScopedDev t;
+    PfScopedBuf t;
     PF_CUDA(cudaMalloc(&t.p, n * 5 * sizeof(double)));
-    double* tmp = t.p;
+    double* tmp = (double*)t.p;
     PF_CUDA(cudaMemcpyAsync(tmp, aos5, n * 5 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     PF_LAUNCH(h->ctx, pf_unpack_kernel, cdiv_u(n, PF_NT), PF_NT, 0, h->d, tmp);
     if (h->rec.on) { int rc = pf_recovery_reset(h); if (rc) return rc; }
@@ -465,9 +470,9 @@ extern "C" int pfgpu_pf_upload(pfgpu_pf* h, const double* aos5, size_t n) {
 extern "C" int pfgpu_pf_download(pfgpu_pf* h, double* aos5, size_t n) {
     if (!h || !aos5 || n != h->d.n) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
-    PfScopedDev t;
+    PfScopedBuf t;
     PF_CUDA(cudaMalloc(&t.p, n * 5 * sizeof(double)));
-    double* tmp = t.p;
+    double* tmp = (double*)t.p;
     PF_LAUNCH(h->ctx, pf_pack_kernel, cdiv_u(n, PF_NT), PF_NT, 0, h->d, tmp);
     PF_CUDA(cudaMemcpyAsync(aos5, tmp, n * 5 * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
@@ -480,35 +485,51 @@ extern "C" int pfgpu_pf_count(pfgpu_pf* h, size_t* nl, size_t* ng) {
     return 0;
 }
 
+// d.obs with room for n doubles (its contents are dropped when it grows).  A failed allocation leaves no buffer and capacity 0,
+// never a freed buffer under a capacity that claims it.
+static int pf_obs_reserve(pfgpu_pf* h, size_t n) {
+    if (n <= h->obs_cap) return 0;
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));                   // a queued launch may still read the old buffer
+    cudaFree(h->d.obs);
+    h->d.obs = nullptr; h->obs_cap = 0;
+    double* p = nullptr;
+    PF_CUDA(cudaMalloc(&p, 2 * n * sizeof(double)));
+    h->d.obs = p; h->obs_cap = 2 * n;
+    return 0;
+}
 static int pf_stage_obs(pfgpu_pf* h, const double* obs3, size_t k) {
     for (size_t j = 0; j < k; ++j)                                   // validate_observations pf.rs:538-549
         if (!finite_d(obs3[3 * j]) || !finite_d(obs3[3 * j + 1]) || !finite_d(obs3[3 * j + 2]) || obs3[3 * j] < 0.0)
             return PFGPU_ERR_INVALID;
     if (k <= PF_PARAM_OBS) return 0;                                 // short lists ride in the launch parameters
-    if (k > h->obs_cap) {
-        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-        cudaFree(h->d.obs);
-        h->obs_cap = k * 2;
-        PF_CUDA(cudaMalloc(&h->d.obs, h->obs_cap * 3 * sizeof(double)));
-    }
-    if (k > 0) PF_CUDA(cudaMemcpyAsync(h->d.obs, obs3, k * 3 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+    int rc = pf_obs_reserve(h, 3 * k);
+    if (rc) return rc;
+    PF_CUDA(cudaMemcpyAsync(h->d.obs, obs3, k * 3 * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     return 0;
 }
-// A scan's used beams -> h->pairs = (r_i, a_i); *k = their count.  Long lists go to d.obs.  Candidates i = 0, s, 2s, .. (AMCL's
-// laser_max_beams stride); NaN or r <= 0 is unused (occupancy_grid_map.rs:84); r >= max_range is a max reading: unused, or with
-// keep_max (the beam model with z_max > 0) used as r = max_range.
-static int pf_stage_pairs(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, uint32_t max_beams,
-                          double max_range, bool keep_max, uint64_t L, size_t* k) {
-    if ((B && !ranges) || !finite_d(angle_min) || !finite_d(angle_inc)) return PFGPU_ERR_INVALID;
+// the map slot of a scan model
+template <int KIND>
+static auto& pf_map(pfgpu_pf* h) {
+    if constexpr (KIND == PF_KIND_BEAM) return h->bm;
+    else return h->lf;
+}
+// A scan's used beams under the model KIND (its map must be loaded) -> h->pairs = (r_i, a_i); *k = their count.  Long lists go to
+// d.obs.  Candidates i = 0, s, 2s, .. (AMCL's laser_max_beams stride); NaN or r <= 0 is unused (occupancy_grid_map.rs:84);
+// r >= max_range is a max reading: unused, or with the model's keep_max used as r = max_range.
+template <int KIND>
+static int pf_stage_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
+    const auto& m = pf_map<KIND>(h);
+    if (!m.on || (B && !ranges) || !finite_d(angle_min) || !finite_d(angle_inc)) return PFGPU_ERR_INVALID;
+    const double max_range = m.cfg.max_range;
     std::vector<double>& pr = h->pairs;
     pr.clear();
     if (B) {
-        const size_t s = std::max<size_t>(1, (B - 1) / (size_t)(max_beams - 1));
+        const size_t s = std::max<size_t>(1, (B - 1) / (size_t)(m.cfg.max_beams - 1));
         for (size_t i = 0; i < B; i += s) {
             double r = ranges[i];
             if (r != r || r <= 0.0) continue;
             if (r >= max_range) {
-                if (!keep_max) continue;
+                if (!m.keep_max()) continue;
                 r = max_range;
             }
             pr.push_back(r);
@@ -516,27 +537,12 @@ static int pf_stage_pairs(pfgpu_pf* h, const double* ranges, size_t B, double an
         }
     }
     *k = pr.size() / 2;
-    if (*k > L) return PFGPU_ERR_INVALID;
+    if (*k > m.L) return PFGPU_ERR_INVALID;
     if (*k <= PF_PARAM_BEAMS) return 0;
-    if (3 * h->obs_cap < pr.size()) {
-        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-        cudaFree(h->d.obs);
-        h->obs_cap = *k;
-        PF_CUDA(cudaMalloc(&h->d.obs, h->obs_cap * 3 * sizeof(double)));
-    }
+    int rc = pf_obs_reserve(h, pr.size());
+    if (rc) return rc;
     PF_CUDA(cudaMemcpyAsync(h->d.obs, pr.data(), pr.size() * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
     return 0;
-}
-// the likelihood field's used beams (DESIGN §3.9)
-static int pf_stage_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
-    if (!h->lf.on) return PFGPU_ERR_INVALID;
-    return pf_stage_pairs(h, ranges, B, angle_min, angle_inc, h->lf.cfg.max_beams, h->lf.cfg.max_range, false, h->lf.L, k);
-}
-// the beam model's used beams (DESIGN §3.11): max readings count when z_max > 0
-static int pf_stage_beam(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc, size_t* k) {
-    if (!h->bm.on) return PFGPU_ERR_INVALID;
-    const pfgpu_beam_config& c = h->bm.cfg;
-    return pf_stage_pairs(h, ranges, B, angle_min, angle_inc, c.max_beams, c.max_range, c.z_max > 0.0, h->bm.L, k);
 }
 static PfScan pf_scan_arg(const pfgpu_pf* h, double angle_min) {
     PfScan s;
@@ -559,13 +565,6 @@ static PfBeam pf_beam_arg(const pfgpu_pf* h, double angle_min) {
     b.W = (int)h->bm.W; b.H = (int)h->bm.H; b.skip = h->bm.skip;
     return b;
 }
-// the launch-parameter form of k <= PF_PARAM_BEAMS used beams: the first pairs in the observation block, the rest in pb
-static void pf_fill_beams(const pfgpu_pf* h, size_t k, PfObsParam& po, PfBeamParam& pb) {
-    for (size_t j = 0; j < 2 * k; ++j) {
-        if (j < 3 * PF_PARAM_OBS) po.o[j] = h->pairs[j];
-        else pb.b[j - 3 * PF_PARAM_OBS] = h->pairs[j];
-    }
-}
 // the smem a weight pass stages: k observations (d, lx, ly), or the beams (r, a) of a scan (a fixed size up to PF_PARAM_BEAMS,
 // so that one captured scan step serves every beam count)
 template <bool SCAN>
@@ -580,32 +579,55 @@ static PfInj pf_inj(const pfgpu_pf* h) {
     if (h->rec.on) { for (int j = 0; j < 4; ++j) a.r[j] = h->rec.region[j]; a.arm = h->rec.armed ? 1 : 0; }
     return a;
 }
-// obs: k x (d, lx, ly), or for a scan (KIND != PF_KIND_LM) the k used beams (r, a) in h->pairs (angle_min: the scan's)
+// out = (&a...): the kernelParams of a kernel with parameters P..., which the arguments must match type for type
+template <class... P, class... A>
+static void** pf_kernel_params(void** out, A&... a) {
+    static_assert(sizeof...(P) == sizeof...(A) && (std::is_same<P, A>::value && ...), "arguments differ from the kernel's parameters");
+    size_t i = 0;
+    ((out[i++] = (void*)&a), ...);
+    return out;
+}
+// pf_predict_weight_kernel's arguments in its parameter order.  The plain launch and the graph replay's node patch both pass
+// params(kernel), so the two cannot diverge and the compiler checks them against the kernel.
+struct PfMainArgs {
+    PfDev d; PfObsParam po; double u0, u1, sv, sw, dt; uint64_t seed; uint32_t call; int k; double sigma; PfInj inj; PfScan sc;
+    PfBeamParam pb; PfBeam bm;
+    void* p[15];
+    template <class... P>
+    void** params(void (*)(P...)) { return pf_kernel_params<P...>(p, d, po, u0, u1, sv, sw, dt, seed, call, k, sigma, inj, sc, pb, bm); }
+};
+// obs: k x (d, lx, ly), or for a scan (KIND != PF_KIND_LM) the k used beams (r, a) in h->pairs (angle_min: the scan's); lists
+// short enough to ride in the launch parameters are copied there.  u = nullptr: no predict
+template <int KIND>
+static PfMainArgs pf_main_args(const pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+    PfMainArgs a;
+    if (KIND == PF_KIND_LM && k <= PF_PARAM_OBS) for (size_t j = 0; j < 3 * k; ++j) a.po.o[j] = obs3[j];
+    if (KIND != PF_KIND_LM && k <= PF_PARAM_BEAMS)      // the first pairs in the observation block, the rest in pb
+        for (size_t j = 0; j < 2 * k; ++j) (j < 3 * PF_PARAM_OBS ? a.po.o[j] : a.pb.b[j - 3 * PF_PARAM_OBS]) = h->pairs[j];
+    a.d = h->d;
+    a.u0 = u ? u[0] : 0.0; a.u1 = u ? u[1] : 0.0;
+    a.sv = h->cfg.velocity_noise; a.sw = h->cfg.yaw_rate_noise; a.dt = h->cfg.dt; a.sigma = h->cfg.range_noise;
+    a.seed = h->seed; a.call = h->n_predict; a.k = (int)k;
+    a.inj = pf_inj(h);
+    a.sc = KIND == PF_KIND_LF ? pf_scan_arg(h, angle_min) : PfScan{};
+    a.bm = KIND == PF_KIND_BEAM ? pf_beam_arg(h, angle_min) : PfBeam{};
+    return a;
+}
 template <bool P, bool W, bool INJ, int KIND>
 static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
     constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
     size_t smem = W ? pf_obs_smem<SCAN>(k) : 0;
     const bool param = !W || k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS);
-    PfObsParam po;
-    PfBeamParam pb;
-    if (W && param) {
-        if (SCAN) pf_fill_beams(h, k, po, pb);
-        else for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
-    }
     if (smem > 48 * 1024) {
         PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    const PfInj inj = pf_inj(h);
-    const PfScan sc = KIND == PF_KIND_LF ? pf_scan_arg(h, angle_min) : PfScan{};
-    const PfBeam bm = BEAM ? pf_beam_arg(h, angle_min) : PfBeam{};
+    const auto kernel = param ? pf_predict_weight_kernel<P, W, true, INJ, SCAN, BEAM> : pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>;
+    PfMainArgs a = pf_main_args<KIND>(h, u, obs3, k, angle_min);
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
-    if (param)
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, true, INJ, SCAN, BEAM>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb, bm);
-    else
-        PF_LAUNCH(h->ctx, (pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>), cdiv_u(h->d.n, PF_NT), PF_NT, smem, h->d, po, u ? u[0] : 0.0, u ? u[1] : 0.0,
-                  h->cfg.velocity_noise, h->cfg.yaw_rate_noise, h->cfg.dt, h->seed, h->n_predict, (int)k, h->cfg.range_noise, inj, sc, pb, bm);
+    cudaLaunchKernel((const void*)kernel, cdiv_u(h->d.n, PF_NT), PF_NT, a.params(kernel), smem, h->ctx.stream);    // checked as PF_LAUNCH does
+    h->ctx.launches++;
+    PF_CUDA(cudaGetLastError());
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     return 0;
 }
@@ -743,17 +765,22 @@ extern "C" int pfgpu_pf_predict(pfgpu_pf* h, const double u[2]) {
     h->rec.armed = false;
     return pf_refresh_cache(h);                                                      // pf.rs:299
 }
-extern "C" int pfgpu_pf_update(pfgpu_pf* h, const double* obs3, size_t k) {
-    if (!h || (k && !obs3)) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    int rc = pf_stage_obs(h, obs3, k);
-    if (rc) return rc;
-    rc = pf_launch_main<false, true>(h, nullptr, obs3, k);
+// try_update once the measurement is staged: landmarks obs3 (k x 3), or for a scan the k beams in h->pairs
+template <int KIND>
+static int pf_update_impl(pfgpu_pf* h, const double* obs3, size_t k, double angle_min) {
+    int rc = pf_launch_main<false, true, KIND>(h, nullptr, obs3, k, angle_min);
     if (rc) return rc;
     h->rec.armed = false;                                                            // the weights are no longer uniform
     rc = pf_normalize(h);                                                            // pf.rs:331
     if (rc) return rc;
     return pf_refresh_cache(h);                                                      // pf.rs:332
+}
+extern "C" int pfgpu_pf_update(pfgpu_pf* h, const double* obs3, size_t k) {
+    if (!h || (k && !obs3)) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    int rc = pf_stage_obs(h, obs3, k);
+    if (rc) return rc;
+    return pf_update_impl<PF_KIND_LM>(h, obs3, k, 0.0);
 }
 extern "C" int pfgpu_pf_resample(pfgpu_pf* h, int* did) {
     if (!h) return PFGPU_ERR_INVALID;
@@ -788,6 +815,12 @@ static void pf_graph_drop(pfgpu_pf* h) {
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
     h->sg.exec = nullptr; h->sg.graph = nullptr; h->sg.main_node = nullptr; h->sg.k = ~(size_t)0; h->sg.kind = PF_KIND_LM;
 }
+// the measurement kernel of a captured step (the injecting one while recovery is on)
+template <int KIND>
+static auto pf_graph_kernel(const pfgpu_pf* h) {
+    constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
+    return h->rec.on ? pf_predict_weight_kernel<true, true, true, true, SCAN, BEAM> : pf_predict_weight_kernel<true, true, true, false, SCAN, BEAM>;
+}
 // capture the step at observation count k, or a scan step of either model (no work is executed by the capture itself)
 template <int KIND>
 static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
@@ -805,9 +838,7 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
     if (cudaGraphGetNodes(g, nullptr, &nn) != cudaSuccess || nn == 0) { cudaGetLastError(); pf_graph_drop(h); return 1; }
     std::vector<cudaGraphNode_t> nodes(nn);
     if (cudaGraphGetNodes(g, nodes.data(), &nn) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
-    const void* want = h->rec.on ? (const void*)pf_predict_weight_kernel<true, true, true, true, SCAN, BEAM>
-                                 : (const void*)pf_predict_weight_kernel<true, true, true, false, SCAN, BEAM>;
+    const void* want = (const void*)pf_graph_kernel<KIND>(h);
     for (cudaGraphNode_t nd : nodes) {
         cudaGraphNodeType ty;
         if (cudaGraphNodeGetType(nd, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
@@ -822,18 +853,9 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
 // replay with this step's arguments patched into the first kernel
 template <int KIND>
 static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
-    PfObsParam po;
-    PfBeamParam pb;
-    if (KIND != PF_KIND_LM) pf_fill_beams(h, k, po, pb);
-    else for (size_t j = 0; j < 3 * k; ++j) po.o[j] = obs3[j];
-    double u0 = u[0], u1 = u[1], sv = h->cfg.velocity_noise, sw = h->cfg.yaw_rate_noise, dt = h->cfg.dt, sigma = h->cfg.range_noise;
-    uint64_t seed = h->seed; uint32_t call = h->n_predict; int kk = (int)k;
-    PfInj inj = pf_inj(h);
-    PfScan sc = KIND == PF_KIND_LF ? pf_scan_arg(h, angle_min) : PfScan{};
-    PfBeam bm = KIND == PF_KIND_BEAM ? pf_beam_arg(h, angle_min) : PfBeam{};
-    void* args[] = { &h->d, &po, &u0, &u1, &sv, &sw, &dt, &seed, &call, &kk, &sigma, &inj, &sc, &pb, &bm };
+    PfMainArgs a = pf_main_args<KIND>(h, u, obs3, k, angle_min);
     cudaKernelNodeParams kp = h->sg.main_params;
-    kp.kernelParams = args; kp.extra = nullptr;
+    kp.kernelParams = a.params(pf_graph_kernel<KIND>(h)); kp.extra = nullptr;
     PF_CUDA(cudaGraphExecKernelNodeSetParams(h->sg.exec, h->sg.main_node, &kp));
     PF_CUDA(cudaGraphLaunch(h->sg.exec, h->ctx.stream));
     h->ctx.launches += h->sg.launches;
@@ -946,7 +968,8 @@ extern "C" int pfgpu_pf_init_region(pfgpu_pf* h, const double region[4]) {
     return pf_refresh_cache(h);
 }
 
-// ---- likelihood-field scan model: localisation in an occupancy grid from a laser scan (DESIGN §3.9) ----
+// ---- scan models: localisation in an occupancy grid from a laser scan, under the likelihood field (DESIGN §3.9) or the beam
+// model (DESIGN §3.11, pf_beam.cuh).  Each model has its own map slot; a map is built from a host mask or a grid's (DESIGN §3.12) ----
 #define PF_LF_MAX_L 4096           // the beams a scan may use at most (their (r, a) pairs are staged in shared memory)
 // L: the largest count <= PF_LF_MAX_L with q_lo^(L+1) >= DBL_MIN and q_hi^(L+1) <= DBL_MAX, powers by repeated multiplication
 static uint64_t pf_lf_limit(double q_lo, double q_hi) {
@@ -960,15 +983,6 @@ static uint64_t pf_lf_limit(double q_lo, double q_hi) {
     }
     return L;
 }
-static void pf_lf_free(pfgpu_pf* h) {
-    cudaFree(h->lf.D); cudaFree(h->lf.q);
-    h->lf.D = h->lf.q = nullptr;
-    h->lf.on = false; h->lf.W = h->lf.H = 0; h->lf.L = 0;
-}
-struct PfScopedBuf {
-    void* p = nullptr;
-    ~PfScopedBuf() { if (p) cudaFree(p); }
-};
 static bool pf_map_shape_ok(size_t W, size_t H) { return W >= 1 && H >= 1 && W <= 65536 && H <= 65536 && W * H <= ((size_t)1 << 28); }
 // the likelihood field's config check; its beam bound L and q_out
 static int pf_lf_check(size_t W, size_t H, const pfgpu_lfield_config* c, uint64_t* L, double* q_out) {
@@ -981,92 +995,6 @@ static int pf_lf_check(size_t W, size_t H, const pfgpu_lfield_config* c, uint64_
     const double coeff = 1.0 / sqrt(2.0 * PFC_PI * (c->sigma_hit * c->sigma_hit));
     *L = pf_lf_limit(*q_out, c->z_hit * coeff + *q_out);
     return *L < 1 ? PFGPU_ERR_INVALID : 0;
-}
-// the likelihood field from an obstacle mask on the handle's device, enqueued on its stream (a host mask or a grid's, DESIGN §3.12)
-static int pf_lf_load(pfgpu_pf* h, const unsigned char* mask_dev, size_t W, size_t H, const pfgpu_lfield_config* c, uint64_t L,
-                      double q_out) {
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-    pf_graph_drop(h);                          // the captured step holds the old table's address
-    pf_lf_free(h);
-    const size_t cells = W * H, scratch = std::max(W * (H + 1), H * (W + 1));
-    PF_CUDA(cudaMalloc(&h->lf.D, cells * sizeof(double)));
-    PF_CUDA(cudaMalloc(&h->lf.q, cells * sizeof(double)));
-    PfScopedBuf v, z;
-    PF_CUDA(cudaMalloc(&v.p, scratch * sizeof(int)));
-    PF_CUDA(cudaMalloc(&z.p, scratch * sizeof(double)));
-    // rows into q (as scratch), columns into D, then D = sqrt and the factor table
-    PF_LAUNCH(h->ctx, pf_lf_edt_rows_kernel, cdiv_u(W, 32), 32, 0, mask_dev, h->lf.q, (int)W, (int)H, (int*)v.p, (double*)z.p);
-    PF_LAUNCH(h->ctx, pf_lf_edt_cols_kernel, cdiv_u(H, 32), 32, 0, h->lf.q, h->lf.D, (int)W, (int)H, (int*)v.p, (double*)z.p);
-    PF_LAUNCH(h->ctx, pf_lf_table_kernel, cdiv_u(cells, 256), 256, 0, h->lf.D, h->lf.q, cells, c->resolution, c->sigma_hit, c->z_hit, q_out);
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-    h->lf.W = W; h->lf.H = H; h->lf.L = L; h->lf.cfg = *c; h->lf.q_out = q_out;
-    h->lf.on = true;
-    return 0;
-}
-extern "C" int pfgpu_pf_lfield_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_lfield_config* c) {
-    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
-    uint64_t L = 0;
-    double q_out = 0.0;
-    int rc = pf_lf_check(W, H, c, &L, &q_out);
-    if (rc) return rc;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    PfScopedBuf m;
-    PF_CUDA(cudaMalloc(&m.p, W * H));
-    PF_CUDA(cudaMemcpyAsync(m.p, mask, W * H, cudaMemcpyHostToDevice, h->ctx.stream));
-    return pf_lf_load(h, (const unsigned char*)m.p, W, H, c, L, q_out);
-}
-extern "C" int pfgpu_pf_lfield_clear(pfgpu_pf* h) {
-    if (!h) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-    pf_graph_drop(h);
-    pf_lf_free(h);
-    return 0;
-}
-extern "C" int pfgpu_pf_lfield_info(pfgpu_pf* h, size_t* W, size_t* H, uint64_t* L) {
-    if (!h) return PFGPU_ERR_INVALID;
-    if (W) *W = h->lf.W;
-    if (H) *H = h->lf.H;
-    if (L) *L = h->lf.L;
-    return 0;
-}
-extern "C" int pfgpu_pf_lfield_download(pfgpu_pf* h, double* D, double* q, size_t cells) {
-    if (!h || !h->lf.on || cells != h->lf.W * h->lf.H) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    if (D) PF_CUDA(cudaMemcpyAsync(D, h->lf.D, cells * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
-    if (q) PF_CUDA(cudaMemcpyAsync(q, h->lf.q, cells * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-    return 0;
-}
-extern "C" int pfgpu_pf_update_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc) {
-    if (!h) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    size_t k = 0;
-    int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
-    if (rc) return rc;
-    rc = pf_launch_main<false, true, PF_KIND_LF>(h, nullptr, nullptr, k, angle_min);
-    if (rc) return rc;
-    h->rec.armed = false;                                                            // the weights are no longer uniform
-    rc = pf_normalize(h);
-    if (rc) return rc;
-    return pf_refresh_cache(h);
-}
-extern "C" int pfgpu_pf_step_scan(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
-                                  double est[4]) {
-    if (!h || !u) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    size_t k = 0;
-    int rc = pf_stage_scan(h, ranges, B, angle_min, angle_inc, &k);
-    if (rc) return rc;
-    return pf_step_impl<PF_KIND_LF>(h, u, nullptr, k, angle_min, est);
-}
-
-// ---- beam model: ray-cast every particle's expected ranges in the occupancy grid (DESIGN §3.11, pf_beam.cuh) ----
-static void pf_beam_free(pfgpu_pf* h) {
-    cudaFree(h->bm.clr);
-    h->bm.clr = nullptr;
-    h->bm.on = false; h->bm.W = h->bm.H = 0; h->bm.L = 0;
 }
 // the beam model's config check; its beam bound L
 static int pf_beam_check(size_t W, size_t H, const pfgpu_beam_config* c, uint64_t* Lout) {
@@ -1084,50 +1012,136 @@ static int pf_beam_check(size_t W, size_t H, const pfgpu_beam_config* c, uint64_
     *Lout = pf_lf_limit(q_lo, q_hi);
     return *Lout < 1 ? PFGPU_ERR_INVALID : 0;
 }
-// the beam map from an obstacle mask on the handle's device, enqueued on its stream (a host mask or a grid's, DESIGN §3.12)
-static int pf_beam_load(pfgpu_pf* h, const unsigned char* mask_dev, size_t W, size_t H, const pfgpu_beam_config* c, uint64_t L) {
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-    pf_graph_drop(h);                          // the captured step holds the old table's address
-    pf_beam_free(h);
-    const size_t cells = W * H;
-    PF_CUDA(cudaMalloc(&h->bm.clr, cells));
-    PfScopedBuf g;
-    PF_CUDA(cudaMalloc(&g.p, cells));
-    PF_LAUNCH(h->ctx, pf_beam_clr_lines_kernel, cdiv_u(cells, 256), 256, 0, mask_dev, (unsigned char*)g.p, (int)W, (int)H);
-    PF_LAUNCH(h->ctx, pf_beam_clr_cols_kernel, cdiv_u(cells, 256), 256, 0, (const unsigned char*)g.p, h->bm.clr, (int)W, (int)H);
-    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
-    const char* e = getenv("PFGPU_BEAM_SKIP");
-    h->bm.skip = (e && e[0] == '0') ? 0 : 1;
-    h->bm.W = W; h->bm.H = H; h->bm.L = L; h->bm.cfg = *c;
-    h->bm.on = true;
+static int pf_ogm_mask(const pfgpu_ogm* g, double threshold, unsigned char* mask_dev, Ctx& ctx);
+// the obstacle mask of a map being set, into m on the handle's device: the host mask uploaded, or with a grid its mask at threshold
+static int pf_map_mask(pfgpu_pf* h, const uint8_t* mask, const pfgpu_ogm* grid, double threshold, size_t cells, PfScopedBuf& m) {
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaMalloc(&m.p, cells));
+    if (grid) return pf_ogm_mask(grid, threshold, (unsigned char*)m.p, h->ctx);
+    PF_CUDA(cudaMemcpyAsync(m.p, mask, cells, cudaMemcpyHostToDevice, h->ctx.stream));
     return 0;
 }
-extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_beam_config* c) {
-    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
-    uint64_t L = 0;
-    int rc = pf_beam_check(W, H, c, &L);
-    if (rc) return rc;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    PfScopedBuf m;
-    PF_CUDA(cudaMalloc(&m.p, W * H));
-    PF_CUDA(cudaMemcpyAsync(m.p, mask, W * H, cudaMemcpyHostToDevice, h->ctx.stream));
-    return pf_beam_load(h, (const unsigned char*)m.p, W, H, c, L);
-}
-extern "C" int pfgpu_pf_beam_clear(pfgpu_pf* h) {
-    if (!h) return PFGPU_ERR_INVALID;
+// unload slot m's map, and drop the captured step, which holds its tables' addresses
+template <class M>
+static int pf_map_clear(pfgpu_pf* h, M& m) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
     PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     pf_graph_drop(h);
-    pf_beam_free(h);
+    m.release();
     return 0;
 }
-extern "C" int pfgpu_pf_beam_info(pfgpu_pf* h, size_t* W, size_t* H, uint64_t* L) {
+// Replace slot m's map by a W x H one with beam bound L and config c, from an obstacle mask (pf_map_mask's arguments): build(mask)
+// allocates the model's tables, enqueues their construction and records what else the model derives at set time
+template <class M, class Cfg, class Build>
+static int pf_map_load(pfgpu_pf* h, M& m, const uint8_t* mask, const pfgpu_ogm* grid, double threshold, size_t W, size_t H, uint64_t L,
+                       const Cfg& c, Build build) {
+    PfScopedBuf mask_dev;
+    int rc = pf_map_mask(h, mask, grid, threshold, W * H, mask_dev);
+    if (!rc) rc = pf_map_clear(h, m);
+    if (!rc) rc = build((const unsigned char*)mask_dev.p);
+    if (rc) return rc;
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+    m.W = W; m.H = H; m.L = L; m.cfg = c;
+    m.on = true;
+    return 0;
+}
+static int pf_map_info(const PfMap& m, size_t* W, size_t* H, uint64_t* L) {
+    if (W) *W = m.W;
+    if (H) *H = m.H;
+    if (L) *L = m.L;
+    return 0;
+}
+// the likelihood field: the distance field and the factor table
+static int pf_lf_set(pfgpu_pf* h, const uint8_t* mask, const pfgpu_ogm* grid, double threshold, size_t W, size_t H,
+                     const pfgpu_lfield_config* c) {
+    uint64_t L = 0;
+    double q_out = 0.0;
+    const int rc = pf_lf_check(W, H, c, &L, &q_out);
+    if (rc) return rc;
+    const size_t cells = W * H, scratch = std::max(W * (H + 1), H * (W + 1));
+    PfScopedBuf v, z;                          // freed after the load's last synchronise
+    auto& f = h->lf;
+    return pf_map_load(h, f, mask, grid, threshold, W, H, L, *c, [&](const unsigned char* mask_dev) -> int {
+        PF_CUDA(cudaMalloc(&f.D, cells * sizeof(double)));
+        PF_CUDA(cudaMalloc(&f.q, cells * sizeof(double)));
+        PF_CUDA(cudaMalloc(&v.p, scratch * sizeof(int)));
+        PF_CUDA(cudaMalloc(&z.p, scratch * sizeof(double)));
+        // rows into q (as scratch), columns into D, then D = sqrt and the factor table
+        PF_LAUNCH(h->ctx, pf_lf_edt_rows_kernel, cdiv_u(W, 32), 32, 0, mask_dev, f.q, (int)W, (int)H, (int*)v.p, (double*)z.p);
+        PF_LAUNCH(h->ctx, pf_lf_edt_cols_kernel, cdiv_u(H, 32), 32, 0, f.q, f.D, (int)W, (int)H, (int*)v.p, (double*)z.p);
+        PF_LAUNCH(h->ctx, pf_lf_table_kernel, cdiv_u(cells, 256), 256, 0, f.D, f.q, cells, c->resolution, c->sigma_hit, c->z_hit, q_out);
+        f.q_out = q_out;
+        return 0;
+    });
+}
+// the beam model: the clearance table
+static int pf_beam_set(pfgpu_pf* h, const uint8_t* mask, const pfgpu_ogm* grid, double threshold, size_t W, size_t H,
+                       const pfgpu_beam_config* c) {
+    uint64_t L = 0;
+    const int rc = pf_beam_check(W, H, c, &L);
+    if (rc) return rc;
+    const size_t cells = W * H;
+    PfScopedBuf tmp;                           // freed after the load's last synchronise
+    auto& b = h->bm;
+    return pf_map_load(h, b, mask, grid, threshold, W, H, L, *c, [&](const unsigned char* mask_dev) -> int {
+        PF_CUDA(cudaMalloc(&b.clr, cells));
+        PF_CUDA(cudaMalloc(&tmp.p, cells));
+        PF_LAUNCH(h->ctx, pf_beam_clr_lines_kernel, cdiv_u(cells, 256), 256, 0, mask_dev, (unsigned char*)tmp.p, (int)W, (int)H);
+        PF_LAUNCH(h->ctx, pf_beam_clr_cols_kernel, cdiv_u(cells, 256), 256, 0, (const unsigned char*)tmp.p, b.clr, (int)W, (int)H);
+        const char* e = getenv("PFGPU_BEAM_SKIP");
+        b.skip = (e && e[0] == '0') ? 0 : 1;
+        return 0;
+    });
+}
+// the update and the step from a laser scan under the model KIND
+template <int KIND>
+static int pf_scan_update(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc) {
     if (!h) return PFGPU_ERR_INVALID;
-    if (W) *W = h->bm.W;
-    if (H) *H = h->bm.H;
-    if (L) *L = h->bm.L;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    size_t k = 0;
+    int rc = pf_stage_scan<KIND>(h, ranges, B, angle_min, angle_inc, &k);
+    if (rc) return rc;
+    return pf_update_impl<KIND>(h, nullptr, k, angle_min);
+}
+template <int KIND>
+static int pf_scan_step(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc, double est[4]) {
+    if (!h || !u) return PFGPU_ERR_INVALID;
+    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    size_t k = 0;
+    int rc = pf_stage_scan<KIND>(h, ranges, B, angle_min, angle_inc, &k);
+    if (rc) return rc;
+    return pf_step_impl<KIND>(h, u, nullptr, k, angle_min, est);
+}
+
+extern "C" int pfgpu_pf_lfield_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_lfield_config* c) {
+    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
+    return pf_lf_set(h, mask, nullptr, 0.0, W, H, c);
+}
+extern "C" int pfgpu_pf_lfield_clear(pfgpu_pf* h) { return h ? pf_map_clear(h, h->lf) : PFGPU_ERR_INVALID; }
+extern "C" int pfgpu_pf_lfield_info(pfgpu_pf* h, size_t* W, size_t* H, uint64_t* L) { return h ? pf_map_info(h->lf, W, H, L) : PFGPU_ERR_INVALID; }
+extern "C" int pfgpu_pf_lfield_download(pfgpu_pf* h, double* D, double* q, size_t cells) {
+    if (!h || !h->lf.on || cells != h->lf.W * h->lf.H) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    if (D) PF_CUDA(cudaMemcpyAsync(D, h->lf.D, cells * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    if (q) PF_CUDA(cudaMemcpyAsync(q, h->lf.q, cells * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     return 0;
 }
+extern "C" int pfgpu_pf_update_scan(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc) {
+    return pf_scan_update<PF_KIND_LF>(h, ranges, B, angle_min, angle_inc);
+}
+extern "C" int pfgpu_pf_step_scan(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
+                                  double est[4]) {
+    return pf_scan_step<PF_KIND_LF>(h, u, ranges, B, angle_min, angle_inc, est);
+}
+
+extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_beam_config* c) {
+    if (!h || !mask || !c) return PFGPU_ERR_INVALID;
+    return pf_beam_set(h, mask, nullptr, 0.0, W, H, c);
+}
+extern "C" int pfgpu_pf_beam_clear(pfgpu_pf* h) { return h ? pf_map_clear(h, h->bm) : PFGPU_ERR_INVALID; }
+extern "C" int pfgpu_pf_beam_info(pfgpu_pf* h, size_t* W, size_t* H, uint64_t* L) { return h ? pf_map_info(h->bm, W, H, L) : PFGPU_ERR_INVALID; }
 extern "C" int pfgpu_pf_beam_download(pfgpu_pf* h, uint8_t* clearance, size_t cells) {
     if (!h || !h->bm.on || !clearance || cells != h->bm.W * h->bm.H) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
@@ -1136,27 +1150,11 @@ extern "C" int pfgpu_pf_beam_download(pfgpu_pf* h, uint8_t* clearance, size_t ce
     return 0;
 }
 extern "C" int pfgpu_pf_update_beam(pfgpu_pf* h, const double* ranges, size_t B, double angle_min, double angle_inc) {
-    if (!h) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    size_t k = 0;
-    int rc = pf_stage_beam(h, ranges, B, angle_min, angle_inc, &k);
-    if (rc) return rc;
-    rc = pf_launch_main<false, true, PF_KIND_BEAM>(h, nullptr, nullptr, k, angle_min);
-    if (rc) return rc;
-    h->rec.armed = false;                                                            // the weights are no longer uniform
-    rc = pf_normalize(h);
-    if (rc) return rc;
-    return pf_refresh_cache(h);
+    return pf_scan_update<PF_KIND_BEAM>(h, ranges, B, angle_min, angle_inc);
 }
 extern "C" int pfgpu_pf_step_beam(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
                                   double est[4]) {
-    if (!h || !u) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    size_t k = 0;
-    int rc = pf_stage_beam(h, ranges, B, angle_min, angle_inc, &k);
-    if (rc) return rc;
-    return pf_step_impl<PF_KIND_BEAM>(h, u, nullptr, k, angle_min, est);
+    return pf_scan_step<PF_KIND_BEAM>(h, u, ranges, B, angle_min, angle_inc, est);
 }
 extern "C" int pfgpu_pf_beam_raycast(pfgpu_pf* h, const double* poses3, size_t n, size_t B, double angle_min, double angle_inc,
                                      double* out) {
@@ -1375,28 +1373,11 @@ static bool pf_grid_ok(const pfgpu_pf* h, const pfgpu_ogm* g, double threshold, 
 }
 extern "C" int pfgpu_pf_lfield_set_grid(pfgpu_pf* h, const pfgpu_ogm* grid, double threshold, const pfgpu_lfield_config* c) {
     if (!h || !c || !pf_grid_ok(h, grid, threshold, c->resolution)) return PFGPU_ERR_INVALID;
-    uint64_t L = 0;
-    double q_out = 0.0;
-    int rc = pf_lf_check(grid->W, grid->H, c, &L, &q_out);
-    if (rc) return rc;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    PfScopedBuf m;
-    PF_CUDA(cudaMalloc(&m.p, grid->W * grid->H));
-    rc = pf_ogm_mask(grid, threshold, (unsigned char*)m.p, h->ctx);
-    if (rc) return rc;
-    return pf_lf_load(h, (const unsigned char*)m.p, grid->W, grid->H, c, L, q_out);
+    return pf_lf_set(h, nullptr, grid, threshold, grid->W, grid->H, c);
 }
 extern "C" int pfgpu_pf_beam_set_grid(pfgpu_pf* h, const pfgpu_ogm* grid, double threshold, const pfgpu_beam_config* c) {
     if (!h || !c || !pf_grid_ok(h, grid, threshold, c->resolution)) return PFGPU_ERR_INVALID;
-    uint64_t L = 0;
-    int rc = pf_beam_check(grid->W, grid->H, c, &L);
-    if (rc) return rc;
-    PF_CUDA(cudaSetDevice(h->ctx.device));
-    PfScopedBuf m;
-    PF_CUDA(cudaMalloc(&m.p, grid->W * grid->H));
-    rc = pf_ogm_mask(grid, threshold, (unsigned char*)m.p, h->ctx);
-    if (rc) return rc;
-    return pf_beam_load(h, (const unsigned char*)m.p, grid->W, grid->H, c, L);
+    return pf_beam_set(h, nullptr, grid, threshold, grid->W, grid->H, c);
 }
 
 // ====================================================================================================
