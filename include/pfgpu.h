@@ -238,6 +238,25 @@ int  pfgpu_pf_update_beam(pfgpu_pf*, const double* ranges, size_t n_ranges, doub
 int  pfgpu_pf_step_beam(pfgpu_pf*, const double u[2], const double* ranges, size_t n_ranges, double angle_min, double angle_inc,
                         double est[4]);
 int  pfgpu_pf_beam_raycast(pfgpu_pf*, const double* poses3, size_t n, size_t n_beams, double angle_min, double angle_inc, double* out);
+/* The odometry motion model: the predict moves every particle by the increment between two wheel-odometry poses instead of by a
+ * control (v, yaw_rate) over dt (not in the reference, whose filters only have the velocity model pf.rs:279-296; Probabilistic
+ * Robotics Table 5.6, ROS AMCL's odom_model_type diff-corrected with odom_alpha1..4; DESIGN §3.14).  The rule, its evaluation order
+ * and its draws are include/pf_odom_math.h's: odom = (x, y, yaw) of the previous odometry pose, then (x, y, yaw) of the current one.
+ * Noise grows with the motion: two equal poses move no particle.  The particle's v is left as it was.
+ * pfgpu_pf_set_odom_noise: alpha = (alpha1 .. alpha4), each finite and >= 0, else PFGPU_ERR_INVALID; a handle starts at 0.2 each.
+ *   pfgpu_pf_odom_noise returns them.
+ * pfgpu_pf_predict_odom / pfgpu_pf_step_odom / pfgpu_pf_step_scan_odom / pfgpu_pf_step_beam_odom: pfgpu_pf_predict / pfgpu_pf_step /
+ *   pfgpu_pf_step_scan / pfgpu_pf_step_beam with this motion in place of u, on every path those take (the call index, the recovery
+ *   injection before the move, KLD-adaptive MCL, sharding), with the same launches; they mix freely with the velocity calls.  A
+ *   component of odom that is not finite: PFGPU_ERR_INVALID, as a non-finite u is. */
+int  pfgpu_pf_set_odom_noise(pfgpu_pf*, const double alpha[4]);
+int  pfgpu_pf_odom_noise(pfgpu_pf*, double alpha[4]);
+int  pfgpu_pf_predict_odom(pfgpu_pf*, const double odom[6]);
+int  pfgpu_pf_step_odom(pfgpu_pf*, const double odom[6], const double* obs3, size_t k, double est[4]);
+int  pfgpu_pf_step_scan_odom(pfgpu_pf*, const double odom[6], const double* ranges, size_t n_ranges, double angle_min, double angle_inc,
+                             double est[4]);
+int  pfgpu_pf_step_beam_odom(pfgpu_pf*, const double odom[6], const double* ranges, size_t n_ranges, double angle_min, double angle_inc,
+                             double est[4]);
 
 /* ===================================== Occupancy grid mapping ======================================= */
 

@@ -124,6 +124,8 @@ EXPORTS = [
     "pfgpu_pf_step_scan", "pfgpu_pf_hypotheses",
     "pfgpu_pf_beam_set", "pfgpu_pf_beam_clear", "pfgpu_pf_beam_info", "pfgpu_pf_beam_download", "pfgpu_pf_update_beam",
     "pfgpu_pf_step_beam", "pfgpu_pf_beam_raycast",
+    "pfgpu_pf_set_odom_noise", "pfgpu_pf_odom_noise", "pfgpu_pf_predict_odom", "pfgpu_pf_step_odom", "pfgpu_pf_step_scan_odom",
+    "pfgpu_pf_step_beam_odom",
     "pfgpu_ogm_create", "pfgpu_ogm_destroy", "pfgpu_ogm_update_scans", "pfgpu_ogm_set", "pfgpu_ogm_read", "pfgpu_ogm_obstacles",
     "pfgpu_ogm_info", "pfgpu_pf_lfield_set_grid", "pfgpu_pf_beam_set_grid",
     "pfgpu_csm_create", "pfgpu_csm_destroy", "pfgpu_csm_set_reference", "pfgpu_csm_set_reference_grid", "pfgpu_csm_reference_size",
@@ -184,6 +186,12 @@ def load_library():
     L.pfgpu_pf_update_beam.argtypes = [vp, c_dp, C.c_size_t, C.c_double, C.c_double]
     L.pfgpu_pf_step_beam.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
     L.pfgpu_pf_beam_raycast.argtypes = [vp, c_dp, C.c_size_t, C.c_size_t, C.c_double, C.c_double, c_dp]
+    L.pfgpu_pf_set_odom_noise.argtypes = [vp, c_dp]
+    L.pfgpu_pf_odom_noise.argtypes = [vp, c_dp]
+    L.pfgpu_pf_predict_odom.argtypes = [vp, c_dp]
+    L.pfgpu_pf_step_odom.argtypes = [vp, c_dp, c_dp, C.c_size_t, c_dp]
+    L.pfgpu_pf_step_scan_odom.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
+    L.pfgpu_pf_step_beam_odom.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double, c_dp]
     L.pfgpu_ogm_create.argtypes = [C.POINTER(_OgmCfg), C.c_int, C.POINTER(vp)]
     L.pfgpu_ogm_destroy.argtypes = [vp]
     L.pfgpu_ogm_destroy.restype = None
@@ -608,6 +616,50 @@ class _PfBase:
         return out
 
     # -- pose hypotheses (not in the reference; ROS AMCL's pose hypotheses; DESIGN §3.10) --
+    # -- odometry motion model (not in the reference, whose filters only have the velocity model; DESIGN §3.14) --
+    def set_odometry_noise(self, alpha1=0.2, alpha2=0.2, alpha3=0.2, alpha4=0.2):
+        """ROS AMCL's odom_alpha1..4 (diff-corrected): rotation noise from rotation, rotation noise from translation, translation
+        noise from translation, translation noise from rotation.  Each finite and >= 0; a filter starts at 0.2 each."""
+        a = _f64([alpha1, alpha2, alpha3, alpha4])
+        _check(self.L, self.L.pfgpu_pf_set_odom_noise(self.h, _dp(a)))
+
+    def odometry_noise(self):
+        """(alpha1, alpha2, alpha3, alpha4)"""
+        a = np.empty(4)
+        _check(self.L, self.L.pfgpu_pf_odom_noise(self.h, _dp(a)))
+        return tuple(float(v) for v in a)
+
+    @staticmethod
+    def _odom_pair(odom_prev, odom_cur):
+        o = np.concatenate([_f64(odom_prev).ravel(), _f64(odom_cur).ravel()])
+        if o.size != 6:
+            raise InvalidParameter("odometry poses are (x, y, yaw)")
+        return o
+
+    def try_predict_with_odometry(self, odom_prev, odom_cur):
+        """move every particle by the increment from odometry pose odom_prev = (x, y, yaw) to odom_cur (Probabilistic Robotics
+        Table 5.6, include/pf_odom_math.h) instead of by a control over dt; v is left as it was"""
+        o = self._odom_pair(odom_prev, odom_cur)
+        _check(self.L, self.L.pfgpu_pf_predict_odom(self.h, _dp(o)))
+
+    def try_step_odometry(self, odom_prev, odom_cur, observations, want_estimate=True):
+        """try_step with the odometry motion model: predict_with_odometry, update with the landmark ranges, resample"""
+        o = self._odom_pair(odom_prev, odom_cur)
+        obs = _f64(observations).reshape(-1, 3)
+        est = np.empty(4)
+        _check(self.L, self.L.pfgpu_pf_step_odom(self.h, _dp(o), _dp(obs), obs.shape[0], _dp(est) if want_estimate else None))
+        return est if want_estimate else None
+
+    def try_step_scan_odometry(self, odom_prev, odom_cur, ranges, angle_min, angle_increment, want_estimate=True):
+        """try_step_scan (likelihood field) with the odometry motion model"""
+        return self._step_scan(self.L.pfgpu_pf_step_scan_odom, self._odom_pair(odom_prev, odom_cur), ranges, angle_min, angle_increment,
+                               want_estimate)
+
+    def try_step_beam_scan_odometry(self, odom_prev, odom_cur, ranges, angle_min, angle_increment, want_estimate=True):
+        """try_step_beam_scan (beam model) with the odometry motion model"""
+        return self._step_scan(self.L.pfgpu_pf_step_beam_odom, self._odom_pair(odom_prev, odom_cur), ranges, angle_min, angle_increment,
+                               want_estimate)
+
     def hypotheses(self, max_count=16, xy_res=0.5, yaw_bins=24, labels=False):
         """The particle cloud clustered in a fixed histogram of xy_res x xy_res x (2 pi / yaw_bins) bins (26-connected, cyclic in yaw):
         ([PfHypothesis] of the max_count heaviest clusters, heaviest first, total number of clusters), and with labels=True also an

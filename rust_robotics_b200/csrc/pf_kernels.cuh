@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "xsum.cuh"
 #include "../../include/pf_moments.h"
+#include "../../include/pf_odom_math.h"
 
 struct __align__(32) Pose4 { double x, y, yaw, v; };
 
@@ -90,12 +91,14 @@ __device__ __forceinline__ double pf_lf_factor(const PfScan& sc, const pfc_rcp_t
 // p = scal[PF_REC_P] by a pose drawn uniformly over the region (weight unchanged), then predicted like any other.
 // SCAN: the weight is the likelihood field of k_obs beams (r_i, a_i) instead of the landmark ranges (DESIGN §3.9).
 // SCAN and BEAM: the weight is the beam model of those beams instead (ray-cast in the clearance table bm, DESIGN §3.11).
-template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false, bool SCAN = false, bool BEAM = false>
+// ODOM: the predict moves every particle by the odometry increment od (include/pf_odom_math.h, DESIGN §3.14) instead of the
+// control (u0, u1); sv, sw and dt are then unused.
+template <bool DO_PREDICT, bool DO_WEIGHT, bool PARAM_OBS, bool INJ = false, bool SCAN = false, bool BEAM = false, bool ODOM = false>
 __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const __grid_constant__ PfObsParam po,
                                                                   double u0, double u1, double sv, double sw,
                                                                   double dt, uint64_t seed, uint32_t call,
                                                                   int k_obs, double sigma, PfInj inj, PfScan sc,
-                                                                  const __grid_constant__ PfBeamParam pb, PfBeam bm) {
+                                                                  const __grid_constant__ PfBeamParam pb, PfBeam bm, PfOdom od) {
     extern __shared__ double s_obs_pf[];     // k_obs x (d, lx, ly): the observation vector staged once per CTA; SCAN: k_obs x (r, a)
     if (DO_WEIGHT) {
         if constexpr (SCAN) {
@@ -127,7 +130,14 @@ __global__ void __launch_bounds__(PF_NT) pf_predict_weight_kernel(PfDev d, const
             if (votes && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(d.counters + PF_REC_COUNT, (unsigned)__popc(votes));
         }
     }
-    if (DO_PREDICT) {
+    if constexpr (ODOM) {
+        static_assert(DO_PREDICT, "odometry moves particles in a predict");
+        double za, zb, zc, unused;
+        pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_PF_PREDICT, call, d.offset + i), &za, &zb);
+        pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_PF_ODOM, call, d.offset + i), &zc, &unused);
+        pf_odom_move(&od, za, zb, zc, &p.x, &p.y, &p.yaw);         // v is left as it was
+        pose_store(pose, i, p);
+    } else if (DO_PREDICT) {
         double z0, z1;
         pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_PF_PREDICT, call, d.offset + i), &z0, &z1);
         double v_noise = sv > 0.0 ? 0.0 + sv * z0 : 0.0;            // Normal::sample = mean + std*z; no draw if sigma == 0

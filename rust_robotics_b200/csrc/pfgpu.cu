@@ -163,6 +163,7 @@ struct pfgpu_pf {
         cudaKernelNodeParams main_params = {};
         size_t k = ~(size_t)0;
         int kind = PF_KIND_LM;     // a scan step's graph (either model) serves every beam count up to PF_PARAM_BEAMS (k is patched like u)
+        bool odom = false;         // its predict is the odometry model's (DESIGN §3.14), whose kernel differs from the velocity model's
         uint64_t launches = 0;
         int captures = 0;          // an observation count that keeps changing would re-capture every step: give up after a few
         bool off = false;          // PFGPU_PF_GRAPH=0, capture failed, or too many re-captures: plain launches from then on
@@ -192,6 +193,7 @@ struct pfgpu_pf {
         void release() { cudaFree(clr); *this = BeamMap(); }
     } bm;
     std::vector<double> pairs;     // the used beams of the current scan call (either model): (r_i, a_i)
+    double odom_alpha[4] = { PF_ODOM_ALPHA_DEFAULT, PF_ODOM_ALPHA_DEFAULT, PF_ODOM_ALPHA_DEFAULT, PF_ODOM_ALPHA_DEFAULT };   // DESIGN §3.14
     PfClu clu;                     // pose hypotheses' workspace (DESIGN §3.10), allocated by the first query
 };
 
@@ -579,6 +581,23 @@ static PfInj pf_inj(const pfgpu_pf* h) {
     if (h->rec.on) { for (int j = 0; j < 4; ++j) a.r[j] = h->rec.region[j]; a.arm = h->rec.armed ? 1 : 0; }
     return a;
 }
+// The motion of a predict: the velocity model's control u (pf.rs:279-296, validated as validate_control pf.rs:515-523), or the
+// odometry model's increment (DESIGN §3.14), computed once per call on the host from the two odometry poses and the handle's alphas
+struct PfMotion {
+    bool odom = false;
+    double u[2] = { 0.0, 0.0 };
+    PfOdom od = {};
+};
+static int pf_motion_velocity(const double u[2], PfMotion* m) {
+    if (!u || !finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    m->odom = false; m->u[0] = u[0]; m->u[1] = u[1];
+    return 0;
+}
+static int pf_motion_odom(const pfgpu_pf* h, const double odom[6], PfMotion* m) {
+    if (!odom || pf_odom_increment(odom, h->odom_alpha, &m->od) != 0) return PFGPU_ERR_INVALID;
+    m->odom = true;
+    return 0;
+}
 // out = (&a...): the kernelParams of a kernel with parameters P..., which the arguments must match type for type
 template <class... P, class... A>
 static void** pf_kernel_params(void** out, A&... a) {
@@ -591,21 +610,22 @@ static void** pf_kernel_params(void** out, A&... a) {
 // params(kernel), so the two cannot diverge and the compiler checks them against the kernel.
 struct PfMainArgs {
     PfDev d; PfObsParam po; double u0, u1, sv, sw, dt; uint64_t seed; uint32_t call; int k; double sigma; PfInj inj; PfScan sc;
-    PfBeamParam pb; PfBeam bm;
-    void* p[15];
+    PfBeamParam pb; PfBeam bm; PfOdom od;
+    void* p[16];
     template <class... P>
-    void** params(void (*)(P...)) { return pf_kernel_params<P...>(p, d, po, u0, u1, sv, sw, dt, seed, call, k, sigma, inj, sc, pb, bm); }
+    void** params(void (*)(P...)) { return pf_kernel_params<P...>(p, d, po, u0, u1, sv, sw, dt, seed, call, k, sigma, inj, sc, pb, bm, od); }
 };
 // obs: k x (d, lx, ly), or for a scan (KIND != PF_KIND_LM) the k used beams (r, a) in h->pairs (angle_min: the scan's); lists
-// short enough to ride in the launch parameters are copied there.  u = nullptr: no predict
+// short enough to ride in the launch parameters are copied there.  m = nullptr: no predict
 template <int KIND>
-static PfMainArgs pf_main_args(const pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+static PfMainArgs pf_main_args(const pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
     PfMainArgs a;
     if (KIND == PF_KIND_LM && k <= PF_PARAM_OBS) for (size_t j = 0; j < 3 * k; ++j) a.po.o[j] = obs3[j];
     if (KIND != PF_KIND_LM && k <= PF_PARAM_BEAMS)      // the first pairs in the observation block, the rest in pb
         for (size_t j = 0; j < 2 * k; ++j) (j < 3 * PF_PARAM_OBS ? a.po.o[j] : a.pb.b[j - 3 * PF_PARAM_OBS]) = h->pairs[j];
     a.d = h->d;
-    a.u0 = u ? u[0] : 0.0; a.u1 = u ? u[1] : 0.0;
+    a.u0 = m ? m->u[0] : 0.0; a.u1 = m ? m->u[1] : 0.0;
+    a.od = m ? m->od : PfOdom{};
     a.sv = h->cfg.velocity_noise; a.sw = h->cfg.yaw_rate_noise; a.dt = h->cfg.dt; a.sigma = h->cfg.range_noise;
     a.seed = h->seed; a.call = h->n_predict; a.k = (int)k;
     a.inj = pf_inj(h);
@@ -613,16 +633,16 @@ static PfMainArgs pf_main_args(const pfgpu_pf* h, const double u[2], const doubl
     a.bm = KIND == PF_KIND_BEAM ? pf_beam_arg(h, angle_min) : PfBeam{};
     return a;
 }
-template <bool P, bool W, bool INJ, int KIND>
-static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+template <bool P, bool W, bool INJ, int KIND, bool ODOM>
+static int pf_launch_kernel(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
     constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
     size_t smem = W ? pf_obs_smem<SCAN>(k) : 0;
     const bool param = !W || k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS);
     if (smem > 48 * 1024) {
-        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PF_CUDA(cudaFuncSetAttribute((pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM, ODOM>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    const auto kernel = param ? pf_predict_weight_kernel<P, W, true, INJ, SCAN, BEAM> : pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM>;
-    PfMainArgs a = pf_main_args<KIND>(h, u, obs3, k, angle_min);
+    const auto kernel = param ? pf_predict_weight_kernel<P, W, true, INJ, SCAN, BEAM, ODOM> : pf_predict_weight_kernel<P, W, false, INJ, SCAN, BEAM, ODOM>;
+    PfMainArgs a = pf_main_args<KIND>(h, m, obs3, k, angle_min);
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
     cudaLaunchKernel((const void*)kernel, cdiv_u(h->d.n, PF_NT), PF_NT, a.params(kernel), smem, h->ctx.stream);    // checked as PF_LAUNCH does
@@ -631,15 +651,23 @@ static int pf_launch_kernel(pfgpu_pf* h, const double u[2], const double* obs3, 
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     return 0;
 }
-template <bool P, bool W, int KIND = PF_KIND_LM>
-static int pf_launch_main(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min = 0.0) {
+template <bool P, bool W, int KIND, bool ODOM>
+static int pf_launch_motion(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
     if constexpr (P) {
         if (h->rec.on) {                                             // every predict counts its injections afresh
             PF_CUDA(cudaMemsetAsync(h->d.counters + PF_REC_COUNT, 0, sizeof(unsigned int), h->ctx.stream));
-            return pf_launch_kernel<P, W, true, KIND>(h, u, obs3, k, angle_min);
+            return pf_launch_kernel<P, W, true, KIND, ODOM>(h, m, obs3, k, angle_min);
         }
     }
-    return pf_launch_kernel<P, W, false, KIND>(h, u, obs3, k, angle_min);
+    return pf_launch_kernel<P, W, false, KIND, ODOM>(h, m, obs3, k, angle_min);
+}
+// m: the predict's motion (P), nullptr without a predict
+template <bool P, bool W, int KIND = PF_KIND_LM>
+static int pf_launch_main(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min = 0.0) {
+    if constexpr (P) {
+        if (m->odom) return pf_launch_motion<P, W, KIND, true>(h, m, obs3, k, angle_min);
+    }
+    return pf_launch_motion<P, W, KIND, false>(h, m, obs3, k, angle_min);
 }
 // augmented MCL's filter, right after S = sum w_raw has landed in scal[0]
 static int pf_recovery_filter(pfgpu_pf* h) {
@@ -755,15 +783,33 @@ static int pf_read_gate(pfgpu_pf* h, int* gate) {
     return 0;
 }
 
-extern "C" int pfgpu_pf_predict(pfgpu_pf* h, const double u[2]) {
-    if (!h || !u) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;               // validate_control pf.rs:515-523
+static int pf_predict_impl(pfgpu_pf* h, const PfMotion& m) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
-    int rc = pf_launch_main<true, false>(h, u, nullptr, 0);
+    int rc = pf_launch_main<true, false>(h, &m, nullptr, 0);
     if (rc) return rc;
     h->n_predict++;
     h->rec.armed = false;
     return pf_refresh_cache(h);                                                      // pf.rs:299
+}
+extern "C" int pfgpu_pf_predict(pfgpu_pf* h, const double u[2]) {
+    PfMotion m;
+    if (!h || pf_motion_velocity(u, &m)) return PFGPU_ERR_INVALID;                  // validate_control pf.rs:515-523
+    return pf_predict_impl(h, m);
+}
+extern "C" int pfgpu_pf_predict_odom(pfgpu_pf* h, const double odom[6]) {
+    PfMotion m;
+    if (!h || pf_motion_odom(h, odom, &m)) return PFGPU_ERR_INVALID;
+    return pf_predict_impl(h, m);
+}
+extern "C" int pfgpu_pf_set_odom_noise(pfgpu_pf* h, const double alpha[4]) {
+    if (!h || !alpha || !pf_odom_alpha_ok(alpha)) return PFGPU_ERR_INVALID;
+    for (int j = 0; j < 4; ++j) h->odom_alpha[j] = alpha[j];
+    return 0;
+}
+extern "C" int pfgpu_pf_odom_noise(pfgpu_pf* h, double alpha[4]) {
+    if (!h || !alpha) return PFGPU_ERR_INVALID;
+    for (int j = 0; j < 4; ++j) alpha[j] = h->odom_alpha[j];
+    return 0;
 }
 // try_update once the measurement is staged: landmarks obs3 (k x 3), or for a scan the k beams in h->pairs
 template <int KIND>
@@ -795,8 +841,8 @@ extern "C" int pfgpu_pf_resample(pfgpu_pf* h, int* did) {
 }
 // the launches of one fused step, in stream order (what the graph captures).  A scan's used beams are in h->pairs.
 template <int KIND>
-static int pf_step_launches(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
-    int rc = pf_launch_main<true, true, KIND>(h, u, obs3, k, angle_min);            // predict + likelihood, one pass
+static int pf_step_launches(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
+    int rc = pf_launch_main<true, true, KIND>(h, m, obs3, k, angle_min);            // predict + likelihood, one pass
     if (rc) return rc;
     if (h->fu.on) {                                                                  // normalise .. refresh_cache: one launch (pf3.cuh)
         h->fu.arg.pd = h->d;
@@ -814,20 +860,24 @@ static void pf_graph_drop(pfgpu_pf* h) {
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
     if (h->sg.graph) cudaGraphDestroy(h->sg.graph);
     h->sg.exec = nullptr; h->sg.graph = nullptr; h->sg.main_node = nullptr; h->sg.k = ~(size_t)0; h->sg.kind = PF_KIND_LM;
+    h->sg.odom = false;
 }
-// the measurement kernel of a captured step (the injecting one while recovery is on)
+// the measurement kernel of a captured step (the injecting one while recovery is on; the odometry model's for an odometry step)
 template <int KIND>
-static auto pf_graph_kernel(const pfgpu_pf* h) {
+static auto pf_graph_kernel(const pfgpu_pf* h, bool odom) {
     constexpr bool SCAN = KIND != PF_KIND_LM, BEAM = KIND == PF_KIND_BEAM;
+    if (odom)
+        return h->rec.on ? pf_predict_weight_kernel<true, true, true, true, SCAN, BEAM, true>
+                         : pf_predict_weight_kernel<true, true, true, false, SCAN, BEAM, true>;
     return h->rec.on ? pf_predict_weight_kernel<true, true, true, true, SCAN, BEAM> : pf_predict_weight_kernel<true, true, true, false, SCAN, BEAM>;
 }
 // capture the step at observation count k, or a scan step of either model (no work is executed by the capture itself)
 template <int KIND>
-static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
+static int pf_graph_capture(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
     pf_graph_drop(h);
     const uint64_t l0 = h->ctx.launches;
     if (cudaStreamBeginCapture(h->ctx.stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); return 1; }
-    const int rc = pf_step_launches<KIND>(h, u, obs3, k, angle_min);
+    const int rc = pf_step_launches<KIND>(h, m, obs3, k, angle_min);
     cudaGraph_t g = nullptr;
     const cudaError_t e = cudaStreamEndCapture(h->ctx.stream, &g);
     h->sg.launches = h->ctx.launches - l0;
@@ -838,7 +888,7 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
     if (cudaGraphGetNodes(g, nullptr, &nn) != cudaSuccess || nn == 0) { cudaGetLastError(); pf_graph_drop(h); return 1; }
     std::vector<cudaGraphNode_t> nodes(nn);
     if (cudaGraphGetNodes(g, nodes.data(), &nn) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    const void* want = (const void*)pf_graph_kernel<KIND>(h);
+    const void* want = (const void*)pf_graph_kernel<KIND>(h, m->odom);
     for (cudaGraphNode_t nd : nodes) {
         cudaGraphNodeType ty;
         if (cudaGraphNodeGetType(nd, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel) continue;
@@ -847,15 +897,15 @@ static int pf_graph_capture(pfgpu_pf* h, const double u[2], const double* obs3, 
         if (kp.func == want) { h->sg.main_node = nd; h->sg.main_params = kp; break; }
     }
     if (!h->sg.main_node || cudaGraphInstantiate(&h->sg.exec, g, 0) != cudaSuccess) { cudaGetLastError(); pf_graph_drop(h); return 1; }
-    h->sg.k = k; h->sg.kind = KIND;
+    h->sg.k = k; h->sg.kind = KIND; h->sg.odom = m->odom;
     return 0;
 }
 // replay with this step's arguments patched into the first kernel
 template <int KIND>
-static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min) {
-    PfMainArgs a = pf_main_args<KIND>(h, u, obs3, k, angle_min);
+static int pf_graph_replay(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
+    PfMainArgs a = pf_main_args<KIND>(h, m, obs3, k, angle_min);
     cudaKernelNodeParams kp = h->sg.main_params;
-    kp.kernelParams = a.params(pf_graph_kernel<KIND>(h)); kp.extra = nullptr;
+    kp.kernelParams = a.params(pf_graph_kernel<KIND>(h, m->odom)); kp.extra = nullptr;
     PF_CUDA(cudaGraphExecKernelNodeSetParams(h->sg.exec, h->sg.main_node, &kp));
     PF_CUDA(cudaGraphLaunch(h->sg.exec, h->ctx.stream));
     h->ctx.launches += h->sg.launches;
@@ -863,22 +913,23 @@ static int pf_graph_replay(pfgpu_pf* h, const double u[2], const double* obs3, s
 }
 // try_step once the measurement is staged: landmarks obs3 (k x 3), or for a scan the k beams in h->pairs
 template <int KIND>
-static int pf_step_impl(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double angle_min, double est[4]) {
+static int pf_step_impl(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min, double est[4]) {
     int rc = 0;
     // graph replay: fixed particle count, one GPU, observations short enough to ride in the launch parameters, no per-kernel
     // timing events; the first step of a handle runs plainly (lazy set-up such as function attributes happens there).  The graph
-    // is keyed by the kind of step (landmark / likelihood field / beam) and, for landmark steps, the observation count
+    // is keyed by the kind of step (landmark / likelihood field / beam), the motion model (velocity / odometry) and, for landmark
+    // steps, the observation count
     constexpr bool SCAN = KIND != PF_KIND_LM;
     const bool graphable = !h->sg.off && h->world == 1 && !h->adaptive && k <= (SCAN ? PF_PARAM_BEAMS : PF_PARAM_OBS) && !h->timer.on &&
                            h->steps > 0;
     bool done = false;
     if (graphable) {
-        if (h->sg.exec && h->sg.kind == KIND && (SCAN || h->sg.k == k)) done = true;
-        else if (++h->sg.captures <= 16 && pf_graph_capture<KIND>(h, u, obs3, k, angle_min) == 0) done = true;
+        if (h->sg.exec && h->sg.kind == KIND && h->sg.odom == m->odom && (SCAN || h->sg.k == k)) done = true;
+        else if (++h->sg.captures <= 16 && pf_graph_capture<KIND>(h, m, obs3, k, angle_min) == 0) done = true;
         else { h->sg.off = true; pf_graph_drop(h); }
-        if (done) { rc = pf_graph_replay<KIND>(h, u, obs3, k, angle_min); if (rc) return rc; }
+        if (done) { rc = pf_graph_replay<KIND>(h, m, obs3, k, angle_min); if (rc) return rc; }
     }
-    if (!done) { rc = pf_step_launches<KIND>(h, u, obs3, k, angle_min); if (rc) return rc; }
+    if (!done) { rc = pf_step_launches<KIND>(h, m, obs3, k, angle_min); if (rc) return rc; }
     h->fu.last = h->fu.on;
     h->n_predict++;
     h->steps++;
@@ -890,13 +941,22 @@ static int pf_step_impl(pfgpu_pf* h, const double u[2], const double* obs3, size
     }
     return 0;
 }
-extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double est[4]) {
-    if (!h || !u || (k && !obs3)) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+static int pf_lm_step(pfgpu_pf* h, const PfMotion& m, const double* obs3, size_t k, double est[4]) {
+    if (k && !obs3) return PFGPU_ERR_INVALID;
     PF_CUDA(cudaSetDevice(h->ctx.device));
     int rc = pf_stage_obs(h, obs3, k);
     if (rc) return rc;
-    return pf_step_impl<PF_KIND_LM>(h, u, obs3, k, 0.0, est);
+    return pf_step_impl<PF_KIND_LM>(h, &m, obs3, k, 0.0, est);
+}
+extern "C" int pfgpu_pf_step(pfgpu_pf* h, const double u[2], const double* obs3, size_t k, double est[4]) {
+    PfMotion m;
+    if (!h || pf_motion_velocity(u, &m)) return PFGPU_ERR_INVALID;
+    return pf_lm_step(h, m, obs3, k, est);
+}
+extern "C" int pfgpu_pf_step_odom(pfgpu_pf* h, const double odom[6], const double* obs3, size_t k, double est[4]) {
+    PfMotion m;
+    if (!h || pf_motion_odom(h, odom, &m)) return PFGPU_ERR_INVALID;
+    return pf_lm_step(h, m, obs3, k, est);
 }
 extern "C" int pfgpu_pf_estimate(pfgpu_pf* h, double est[4], double cov_cm[16]) {
     if (!h) return PFGPU_ERR_INVALID;
@@ -1104,14 +1164,26 @@ static int pf_scan_update(pfgpu_pf* h, const double* ranges, size_t B, double an
     return pf_update_impl<KIND>(h, nullptr, k, angle_min);
 }
 template <int KIND>
-static int pf_scan_step(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc, double est[4]) {
-    if (!h || !u) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+static int pf_scan_step(pfgpu_pf* h, const PfMotion& m, const double* ranges, size_t B, double angle_min, double angle_inc, double est[4]) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
     size_t k = 0;
     int rc = pf_stage_scan<KIND>(h, ranges, B, angle_min, angle_inc, &k);
     if (rc) return rc;
-    return pf_step_impl<KIND>(h, u, nullptr, k, angle_min, est);
+    return pf_step_impl<KIND>(h, &m, nullptr, k, angle_min, est);
+}
+// the step from a laser scan under the model KIND with the velocity model's control u, or with the odometry pair odom
+template <int KIND>
+static int pf_scan_step_u(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc, double est[4]) {
+    PfMotion m;
+    if (!h || pf_motion_velocity(u, &m)) return PFGPU_ERR_INVALID;
+    return pf_scan_step<KIND>(h, m, ranges, B, angle_min, angle_inc, est);
+}
+template <int KIND>
+static int pf_scan_step_odom(pfgpu_pf* h, const double odom[6], const double* ranges, size_t B, double angle_min, double angle_inc,
+                             double est[4]) {
+    PfMotion m;
+    if (!h || pf_motion_odom(h, odom, &m)) return PFGPU_ERR_INVALID;
+    return pf_scan_step<KIND>(h, m, ranges, B, angle_min, angle_inc, est);
 }
 
 extern "C" int pfgpu_pf_lfield_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_lfield_config* c) {
@@ -1133,7 +1205,11 @@ extern "C" int pfgpu_pf_update_scan(pfgpu_pf* h, const double* ranges, size_t B,
 }
 extern "C" int pfgpu_pf_step_scan(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
                                   double est[4]) {
-    return pf_scan_step<PF_KIND_LF>(h, u, ranges, B, angle_min, angle_inc, est);
+    return pf_scan_step_u<PF_KIND_LF>(h, u, ranges, B, angle_min, angle_inc, est);
+}
+extern "C" int pfgpu_pf_step_scan_odom(pfgpu_pf* h, const double odom[6], const double* ranges, size_t B, double angle_min,
+                                       double angle_inc, double est[4]) {
+    return pf_scan_step_odom<PF_KIND_LF>(h, odom, ranges, B, angle_min, angle_inc, est);
 }
 
 extern "C" int pfgpu_pf_beam_set(pfgpu_pf* h, const uint8_t* mask, size_t W, size_t H, const pfgpu_beam_config* c) {
@@ -1154,7 +1230,11 @@ extern "C" int pfgpu_pf_update_beam(pfgpu_pf* h, const double* ranges, size_t B,
 }
 extern "C" int pfgpu_pf_step_beam(pfgpu_pf* h, const double u[2], const double* ranges, size_t B, double angle_min, double angle_inc,
                                   double est[4]) {
-    return pf_scan_step<PF_KIND_BEAM>(h, u, ranges, B, angle_min, angle_inc, est);
+    return pf_scan_step_u<PF_KIND_BEAM>(h, u, ranges, B, angle_min, angle_inc, est);
+}
+extern "C" int pfgpu_pf_step_beam_odom(pfgpu_pf* h, const double odom[6], const double* ranges, size_t B, double angle_min,
+                                       double angle_inc, double est[4]) {
+    return pf_scan_step_odom<PF_KIND_BEAM>(h, odom, ranges, B, angle_min, angle_inc, est);
 }
 extern "C" int pfgpu_pf_beam_raycast(pfgpu_pf* h, const double* poses3, size_t n, size_t B, double angle_min, double angle_inc,
                                      double* out) {

@@ -143,6 +143,36 @@ public:
         dirty_ = true;
         return est;
     }
+    // the odometry motion model (DESIGN §3.14): alpha = AMCL's odom_alpha1..4; each motion is the previous then the current
+    // odometry pose (x, y, yaw)
+    using OdomPose = std::array<double, 3>;
+    static std::array<double, 6> odom_pair(const OdomPose& prev, const OdomPose& cur) {
+        return {prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]};
+    }
+    void set_odometry_noise(const std::array<double, 4>& alpha) { check(pfgpu_pf_set_odom_noise(h_, alpha.data()), "odometry noise"); }
+    std::array<double, 4> odometry_noise() const { std::array<double, 4> a{}; check(pfgpu_pf_odom_noise(h_, a.data()), "odometry noise"); return a; }
+    void try_predict_with_odometry(const OdomPose& prev, const OdomPose& cur) {
+        const auto o = odom_pair(prev, cur); check(pfgpu_pf_predict_odom(h_, o.data()), "odometry predict"); dirty_ = true;
+    }
+    PFState try_step_odometry(const OdomPose& prev, const OdomPose& cur, const PFMeasurement& z) {
+        const auto o = odom_pair(prev, cur); auto f = flat(z); PFState est{};
+        check(pfgpu_pf_step_odom(h_, o.data(), f.data(), z.size(), est.data()), "odometry step"); dirty_ = true; return est;
+    }
+    PFState try_step_scan_odometry(const OdomPose& prev, const OdomPose& cur, const std::vector<double>& ranges, double angle_min,
+                                   double angle_increment) {
+        const auto o = odom_pair(prev, cur); PFState est{};
+        check(pfgpu_pf_step_scan_odom(h_, o.data(), ranges.data(), ranges.size(), angle_min, angle_increment, est.data()), "odometry scan step");
+        dirty_ = true;
+        return est;
+    }
+    PFState try_step_beam_scan_odometry(const OdomPose& prev, const OdomPose& cur, const std::vector<double>& ranges, double angle_min,
+                                        double angle_increment) {
+        const auto o = odom_pair(prev, cur); PFState est{};
+        check(pfgpu_pf_step_beam_odom(h_, o.data(), ranges.data(), ranges.size(), angle_min, angle_increment, est.data()),
+              "odometry beam scan step");
+        dirty_ = true;
+        return est;
+    }
     // expected ranges of poses (x, y, yaw) x n_beams in the beam map: out[p * n_beams + b]
     std::vector<double> expected_scan(const std::vector<std::array<double, 3>>& poses, size_t n_beams, double angle_min,
                                       double angle_increment) {

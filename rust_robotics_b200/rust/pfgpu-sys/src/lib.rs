@@ -176,6 +176,14 @@ extern "C" {
                               est: *mut f64) -> c_int;
     pub fn pfgpu_pf_beam_raycast(h: *mut pfgpu_pf, poses3: *const f64, n: usize, n_beams: usize, angle_min: f64, angle_inc: f64,
                                  out: *mut f64) -> c_int;
+    pub fn pfgpu_pf_set_odom_noise(h: *mut pfgpu_pf, alpha: *const f64) -> c_int;
+    pub fn pfgpu_pf_odom_noise(h: *mut pfgpu_pf, alpha: *mut f64) -> c_int;
+    pub fn pfgpu_pf_predict_odom(h: *mut pfgpu_pf, odom: *const f64) -> c_int;
+    pub fn pfgpu_pf_step_odom(h: *mut pfgpu_pf, odom: *const f64, obs3: *const f64, k: usize, est: *mut f64) -> c_int;
+    pub fn pfgpu_pf_step_scan_odom(h: *mut pfgpu_pf, odom: *const f64, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64,
+                                   est: *mut f64) -> c_int;
+    pub fn pfgpu_pf_step_beam_odom(h: *mut pfgpu_pf, odom: *const f64, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64,
+                                   est: *mut f64) -> c_int;
     pub fn pfgpu_ogm_create(cfg: *const pfgpu_ogm_config, device: c_int, out: *mut *mut pfgpu_ogm) -> c_int;
     pub fn pfgpu_ogm_destroy(h: *mut pfgpu_ogm);
     pub fn pfgpu_ogm_update_scans(h: *mut pfgpu_ogm, poses3: *const f64, n_scans: usize, ranges: *const f64, n_ranges: usize,

@@ -191,6 +191,50 @@ impl ParticleFilterLocalizer {
         self.refresh_cache()?;
         Ok(self.state_estimate)
     }
+    /// the odometry motion model (DESIGN §3.14): alpha = ROS AMCL's odom_alpha1..4, each finite and >= 0 (0.2 each at creation)
+    pub fn set_odometry_noise(&mut self, alpha: [f64; 4]) -> RoboticsResult<()> {
+        status(unsafe { sys::pfgpu_pf_set_odom_noise(self.h, alpha.as_ptr()) })
+    }
+    pub fn odometry_noise(&self) -> RoboticsResult<[f64; 4]> {
+        let mut a = [0.0f64; 4];
+        status(unsafe { sys::pfgpu_pf_odom_noise(self.h, a.as_mut_ptr()) })?;
+        Ok(a)
+    }
+    /// move every particle by the increment from odometry pose `prev` = (x, y, yaw) to `cur` instead of by a control over dt
+    pub fn try_predict_with_odometry(&mut self, prev: [f64; 3], cur: [f64; 3]) -> RoboticsResult<()> {
+        let o = [prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]];
+        status(unsafe { sys::pfgpu_pf_predict_odom(self.h, o.as_ptr()) })?;
+        self.refresh_cache()
+    }
+    /// try_step with the odometry motion model
+    pub fn try_step_odometry(&mut self, prev: [f64; 3], cur: [f64; 3], observations: &PFMeasurement) -> RoboticsResult<PFState> {
+        let o = [prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]];
+        let flat: Vec<f64> = observations.iter().flat_map(|&(d, x, y)| [d, x, y]).collect();
+        let mut est = [0.0f64; 4];
+        status(unsafe { sys::pfgpu_pf_step_odom(self.h, o.as_ptr(), flat.as_ptr(), observations.len(), est.as_mut_ptr()) })?;
+        self.refresh_cache()?;
+        Ok(self.state_estimate)
+    }
+    /// try_step_scan (likelihood field) with the odometry motion model
+    pub fn try_step_scan_odometry(&mut self, prev: [f64; 3], cur: [f64; 3], ranges: &[f64], angle_min: f64, angle_increment: f64)
+                                  -> RoboticsResult<PFState> {
+        let o = [prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]];
+        let mut est = [0.0f64; 4];
+        status(unsafe { sys::pfgpu_pf_step_scan_odom(self.h, o.as_ptr(), ranges.as_ptr(), ranges.len(), angle_min, angle_increment,
+                                                     est.as_mut_ptr()) })?;
+        self.refresh_cache()?;
+        Ok(self.state_estimate)
+    }
+    /// try_step_beam_scan (beam model) with the odometry motion model
+    pub fn try_step_beam_scan_odometry(&mut self, prev: [f64; 3], cur: [f64; 3], ranges: &[f64], angle_min: f64, angle_increment: f64)
+                                       -> RoboticsResult<PFState> {
+        let o = [prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]];
+        let mut est = [0.0f64; 4];
+        status(unsafe { sys::pfgpu_pf_step_beam_odom(self.h, o.as_ptr(), ranges.as_ptr(), ranges.len(), angle_min, angle_increment,
+                                                     est.as_mut_ptr()) })?;
+        self.refresh_cache()?;
+        Ok(self.state_estimate)
+    }
     /// expected ranges of poses (x, y, yaw) x n_beams in the beam map: out[p * n_beams + b]
     pub fn expected_scan(&mut self, poses: &[[f64; 3]], n_beams: usize, angle_min: f64, angle_increment: f64) -> RoboticsResult<Vec<f64>> {
         let mut out = vec![0.0f64; poses.len() * n_beams];

@@ -205,25 +205,31 @@ class ScanScenario:
         rng = np.random.default_rng(seed)
         t = list(start)
         self.controls, self.truth, self.scans = [], [], []
-        ang = self.ANGLE_MIN + np.arange(self.B) * self.ANGLE_INC
-        ds = np.arange(1, int(self.MAX_RANGE / (self.RES / 4.0)) + 1) * (self.RES / 4.0)
         W, H = base.shape
         for _ in range(steps):
             t[0] += control[0] * math.cos(t[2]) * self.dt
             t[1] += control[0] * math.sin(t[2]) * self.dt
             t[2] += control[1] * self.dt
-            ex = t[0] + np.cos(t[2] + ang)[:, None] * ds[None, :]
-            ey = t[1] + np.sin(t[2] + ang)[:, None] * ds[None, :]
-            ix, iy = np.floor(ex / self.RES + W / 2.0).astype(np.int64), np.floor(ey / self.RES + H / 2.0).astype(np.int64)
-            inside = (ix >= 0) & (ix < W) & (iy >= 0) & (iy < H)
-            hit = inside & base[np.clip(ix, 0, W - 1), np.clip(iy, 0, H - 1)]
-            first = np.where(hit.any(axis=1), hit.argmax(axis=1), -1)
-            r = np.where(first >= 0, ds[first] + rng.normal(0.0, range_noise, self.B), np.inf)
+            r = self._cast(base, t, rng, range_noise)
             self.controls.append(tuple(control))
             self.truth.append(list(t))
             self.scans.append(np.ascontiguousarray(r))
         assert not any(base[int(math.floor(x / self.RES + W / 2.0)), int(math.floor(y / self.RES + H / 2.0))] for x, y, _ in self.truth)
         self.region = self.REGION if not cells else (-cells * self.RES / 2.0, cells * self.RES / 2.0) * 2
+
+    @classmethod
+    def _cast(cls, base, t, rng, range_noise):
+        """the B ranges seen from pose t in the plan `base`, ray-cast every res / 4, with N(0, range_noise) from rng; no hit: inf"""
+        ang = cls.ANGLE_MIN + np.arange(cls.B) * cls.ANGLE_INC
+        ds = np.arange(1, int(cls.MAX_RANGE / (cls.RES / 4.0)) + 1) * (cls.RES / 4.0)
+        W, H = base.shape
+        ex = t[0] + np.cos(t[2] + ang)[:, None] * ds[None, :]
+        ey = t[1] + np.sin(t[2] + ang)[:, None] * ds[None, :]
+        ix, iy = np.floor(ex / cls.RES + W / 2.0).astype(np.int64), np.floor(ey / cls.RES + H / 2.0).astype(np.int64)
+        inside = (ix >= 0) & (ix < W) & (iy >= 0) & (iy < H)
+        hit = inside & base[np.clip(ix, 0, W - 1), np.clip(iy, 0, H - 1)]
+        first = np.where(hit.any(axis=1), hit.argmax(axis=1), -1)
+        return np.where(first >= 0, ds[first] + rng.normal(0.0, range_noise, cls.B), np.inf)
 
     @staticmethod
     def tiled(base, cells):
@@ -252,3 +258,57 @@ class ScanScenario:
         return (math.hypot(est[0] - self.truth[k][0], est[1] - self.truth[k][1]),
                 abs(normalize_angle(est[2] - self.truth[k][2])))
 
+
+
+class OdomScenario(ScanScenario):
+    """ScanScenario's plan and laser with wheel odometry (the odometry motion model, DESIGN §3.14).  The robot starts at `start`
+    and drives a plan of (steps, v, yaw_rate) legs at dt 0.1: drive, stop for several scans, turn in place, reverse, drive.
+    truth[t] and scans[t] are the pose and scan after step t (as in ScanScenario).  odom[0 .. steps] are wheel-odometry poses in
+    their own frame (odom[0] = (0, 0, 0)): each step's true body-frame increment (dx, dy, dtheta), with dx and dy scaled by
+    1 + N(0, trans_drift) and dtheta by 1 + N(0, rot_drift) plus N(0, rot_bias), composed onto the previous odometry pose
+    (numpy PCG64 `seed`, drawn before the step's scan noise).  A robot that stands still reads exactly the same odometry.
+    controls[t] = the (v, yaw_rate) that reproduces odometry step t over dt: what a caller of the velocity model would invent."""
+    LEGS = ((25, 1.0, 0.05), (10, 0.0, 0.0), (15, 0.0, 1.0), (12, -0.5, 0.0), (20, 1.0, -0.05))
+
+    def __init__(self, legs=LEGS, start=(-3.0, -4.0, 0.3), seed=13, range_noise=0.05, trans_drift=0.02, rot_drift=0.05, rot_bias=0.002):
+        base = self.plan(self.RES)
+        self.obstacles = base
+        self.dt = 0.1
+        self.start = tuple(start)
+        self.region = self.REGION
+        rng = np.random.default_rng(seed)
+        t = list(start)
+        o = [0.0, 0.0, 0.0]
+        self.truth, self.scans, self.odom, self.controls = [], [], [list(o)], []
+        for n, v, w in legs:
+            for _ in range(n):
+                p = list(t)
+                t[0] += v * math.cos(t[2]) * self.dt
+                t[1] += v * math.sin(t[2]) * self.dt
+                t[2] += w * self.dt
+                c, s = math.cos(p[2]), math.sin(p[2])
+                gx, gy = t[0] - p[0], t[1] - p[1]
+                bx, by, bt = c * gx + s * gy, -s * gx + c * gy, t[2] - p[2]
+                if bx != 0.0 or by != 0.0 or bt != 0.0:
+                    k = 1.0 + rng.normal(0.0, trans_drift)
+                    bx, by = bx * k, by * k
+                    bt = bt * (1.0 + rng.normal(0.0, rot_drift)) + rng.normal(0.0, rot_bias)
+                co, so = math.cos(o[2]), math.sin(o[2])
+                o = [o[0] + co * bx - so * by, o[1] + so * bx + co * by, o[2] + bt]
+                self.odom.append(list(o))
+                self.controls.append((math.copysign(math.hypot(bx, by), bx) / self.dt, bt / self.dt))
+                self.truth.append(list(t))
+                self.scans.append(np.ascontiguousarray(self._cast(base, t, rng, range_noise)))
+        W, H = base.shape
+        assert not any(base[int(math.floor(x / self.RES + W / 2.0)), int(math.floor(y / self.RES + H / 2.0))] for x, y, _ in self.truth)
+        ends = np.cumsum([n for n, _, _ in legs])
+        self.phases = {"drive": (0, ends[0]), "stop": (ends[0], ends[1]), "turn": (ends[1], ends[2]), "reverse": (ends[2], ends[3]),
+                       "drive_again": (ends[3], ends[4])}
+
+    @property
+    def steps(self):
+        return len(self.truth)
+
+    def odom_pair(self, t):
+        """(previous, current) odometry pose of step t"""
+        return self.odom[t], self.odom[t + 1]
