@@ -258,6 +258,7 @@ def load_library():
     L.pfgpu_fs_existence_removed.argtypes = [vp, C.POINTER(C.c_uint64)]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
+    L.pfgpu_test_pf_tail.argtypes = [vp, c_dp, C.c_size_t, c_dp, C.POINTER(C.c_int)]
     _LIB = L
     return L
 

@@ -81,6 +81,9 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
         const bool scale_ok = !(S > 0.0) || (S >= 1e-120 && S <= 1e120);
         if (!scale_ok || !(fabs(neff - thr) > slack * fmax(fabs(thr), fabs(neff)))) {     // rare; the same decision in every CTA
             const double toffq = S > 0.0 ? fs3_div(fs3_div(qoff, S), S) : (double)((size_t)b * T) * unif * unif;
+            // the steer of the exact sum must be finite: when the w_raw^2 in front of this tile overflowed (S > ~1e154), this
+            // CTA flags the sum as bad and it takes the serial walk, exact by construction
+            if (tid == 0 && !(fabs(toffq) <= 1.7976931348623157e308)) x.flagsg[FS3_Q] = 1;
             __syncthreads();
             Q = fs3_xsum<NT>(x, sh, vals2, K, nt, toffq, FS3_Q, PF3_R_Q, a.m32, nullptr, 0, 0.0, 0.0, 0.0, 0.0, 0, nullptr);
             neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
@@ -91,6 +94,7 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
     if (gate) {
         // ---------------- cumulative weights (pf.rs:448-453 / mcl.rs:328-336), exact inclusive prefix of every weight ----------------
         const double toffc = S > 0.0 ? fs3_div(toff, S) : (double)((size_t)b * T) * unif;
+        if (tid == 0 && !(fabs(toffc) <= 1.7976931348623157e308)) x.flagsg[FS3_CDF] = 1;     // (the same for the CDF's steer)
         __syncthreads();                                       // (without the Q sum, the S sum used the same scratch half)
         Fs3Run run;
         ctot = fs3_xsum<NT>(x, sh, vals, K, nt, toffc, FS3_CDF, PF3_R_CDF, a.m32, pd.cum, 0, 0.0, 0.0, 0.0, 0.0, 1, &run);
@@ -99,6 +103,11 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
         if (a.mode == 1 && b == (unsigned)((n - 1) / T) && tid == 0) { pd.cum[n - 1] = 1.0; x.tileEnd[b] = 1.0; }   // *last = 1.0 mcl.rs:334-336
         fs3_grid_sync<NT>(x, PF3_R_CDF_DONE, nt);              // the whole CDF is visible
         if ((unsigned)tid < nt) sh.tend[tid] = __ldcg(x.tileEnd + tid);
+        // A CDF with a bad value was stored by the serial walk as its running maximum, NaN sticky: non-decreasing up to the
+        // first NaN, NaN from there on (MCL: but for the last entry, 1).  The lower bound below (NaN counts as >= r) then finds
+        // the reference's first i with r <= c_i whenever one lies before the first NaN; when it lands on a NaN instead, the
+        // reference's linear scan matches nothing up to n - 1 and takes its fallback (PF 0; MCL n - 1, the forced last entry).
+        const bool cdf_bad = __ldcg(x.flagsg + FS3_CDF) != 0;
         __syncthreads();
         // ---------------- one uniform per output slot, first index with r <= c_i, clone (pf.rs:456-470, mcl.rs:344-361) ----------------
         const uint32_t call = pd.counters[0];
@@ -120,6 +129,7 @@ pf3_post_kernel(const __grid_constant__ Fs3Sum x, const __grid_constant__ Pf3Arg
 #pragma unroll 1
                 while (jl < jh) { const size_t mid = jl + ((jh - jl) >> 1); if (__ldcg(c + mid) < r) jl = mid + 1; else jh = mid; }
                 index = jl < n ? jl : (a.mode == 1 ? n - 1 : 0);
+                if (cdf_bad && jl < n) { const double cj = __ldcg(c + jl); if (cj != cj) index = a.mode == 1 ? n - 1 : 0; }
             }
             pd.idx[t] = (uint32_t)index;
             Pose4 p;

@@ -839,22 +839,26 @@ extern "C" int pfgpu_pf_resample(pfgpu_pf* h, int* did) {
     if (did) { int g = 0; rc = pf_read_gate(h, &g); if (rc) return rc; *did = g; }
     return 0;
 }
-// the launches of one fused step, in stream order (what the graph captures).  A scan's used beams are in h->pairs.
-template <int KIND>
-static int pf_step_launches(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
-    int rc = pf_launch_main<true, true, KIND>(h, m, obs3, k, angle_min);            // predict + likelihood, one pass
-    if (rc) return rc;
+// a step's tail, from the raw weights in d.w_raw: normalise, gate, resample, refresh_cache (and augmented MCL's filter)
+static int pf_step_tail(pfgpu_pf* h) {
     if (h->fu.on) {                                                                  // normalise .. refresh_cache: one launch (pf3.cuh)
         h->fu.arg.pd = h->d;
         h->fu.arg.threshold = h->cfg.resample_threshold;
         PF_LAUNCH(h->ctx, pf3_post_kernel<256>, h->fu.tiles, 256, h->fu.smem, h->fu.x, h->fu.arg);
         return pf_recovery_filter(h);                                                // S is in scal[0] once the launch ends
     }
-    rc = pf_normalize(h);
+    int rc = pf_normalize(h);
     if (rc) return rc;
     rc = pf_resample_impl(h);
     if (rc) return rc;
     return pf_refresh_cache(h);
+}
+// the launches of one fused step, in stream order (what the graph captures).  A scan's used beams are in h->pairs.
+template <int KIND>
+static int pf_step_launches(pfgpu_pf* h, const PfMotion* m, const double* obs3, size_t k, double angle_min) {
+    int rc = pf_launch_main<true, true, KIND>(h, m, obs3, k, angle_min);            // predict + likelihood, one pass
+    if (rc) return rc;
+    return pf_step_tail(h);
 }
 static void pf_graph_drop(pfgpu_pf* h) {
     if (h->sg.exec) cudaGraphExecDestroy(h->sg.exec);
@@ -1973,5 +1977,25 @@ extern "C" int pfgpu_test_xsum(const double* host_v, size_t n, double* host_scan
     cudaFree(dv); cudaFree(dc); cudaFree(dt);
     xs_work_free(xs);
     cudaStreamDestroy(ctx.stream);
+    return 0;
+}
+
+// ====================================================================================================
+// test hook: a step's tail on arbitrary raw weights (used by tests/test_gpu_pf_tail_edges.py).  w_raw[n] replaces the raw
+// weights, then exactly what a step issues after its predict + likelihood kernel runs (the fused tail, or the separate kernels
+// of a PFGPU_PF_FUSED=0 handle).  scal4 (optional): S = sum w_raw, Q = sum w^2, the last cumulative weight, N_eff, as the tail
+// left them; gate (optional): 1 when it resampled.
+// ====================================================================================================
+extern "C" int pfgpu_test_pf_tail(pfgpu_pf* h, const double* w_raw, size_t n, double* scal4, int* gate) {
+    if (!h || !w_raw || n != h->d.n) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    PF_CUDA(cudaMemcpyAsync(h->d.w_raw, w_raw, n * sizeof(double), cudaMemcpyHostToDevice, h->ctx.stream));
+    int rc = pf_step_tail(h);
+    if (rc) return rc;
+    h->fu.last = h->fu.on;
+    h->rec.armed = true;
+    if (scal4) PF_CUDA(cudaMemcpyAsync(scal4, h->d.scal, 4 * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    if (gate) PF_CUDA(cudaMemcpyAsync(gate, h->d.gate, sizeof(int), cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     return 0;
 }
