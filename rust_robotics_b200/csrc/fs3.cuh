@@ -507,9 +507,13 @@ __global__ void fs3_mark_kernel(const __grid_constant__ Fs3Dev d, const __grid_c
 // post kernel
 // =====================================================================================================================
 // Written for LATENCY: it moves ~1 MB, so what it costs is instruction fetch (every instruction runs once per warp), waits
-// at barriers and dependent memory round trips.  Hence: one small out-of-line routine (fs3_xsum) serves every exact sum; four
-// block barriers and one grid barrier per sum; the chain over the dirty values is evaluated by warp 0 with warp primitives
-// while the other warps sleep at a block barrier; grid barriers are per-round arrival counters (no generation juggling).
+// at barriers and dependent memory round trips.  The L2 holds none of its code when a step starts (the EKF launch streams
+// more than the L2 through it), so the code every step runs — the S sum, the gate, the certified CDF, normalisation — is laid
+// out as one straight run inside the kernel (fs3_xsum_body, fs3_xsum_emit_body, inline divisions), where sequential fetch
+// covers it, and what a config-3 step rarely runs stays out of line (fs3_xsum / fs3_xsum_emit for the exact S2, CDF and comb
+// sums, fs3_chain_wide, fs3_serial_walk, fs3_classify, fs3_div).  Four block barriers and one grid barrier per sum; the chain
+// over the dirty values is evaluated by warp 0 with warp primitives while the other warps sleep at a block barrier; grid
+// barriers are per-round arrival counters (no generation juggling).
 template <int NT>
 struct Fs3Sh {
     double wd[2][NT / 32]; unsigned long long wu[2][NT / 32]; int wi[2][NT / 32];   // warp totals (double-buffered by round)
@@ -595,7 +599,7 @@ __device__ __forceinline__ void fs3_block_sum2(double& x, double& y, double* smx
     x = a; y = b;
 }
 
-__device__ __noinline__ double fs3_div(double a, double b) { return a / b; }      // one copy of the IEEE division sequence
+__device__ __noinline__ double fs3_div(double a, double b) { return a / b; }      // one copy of the IEEE division sequence for the rare paths
 // value i of the sum `slot`, recomputed from global memory (serial walks only)
 __device__ __forceinline__ double fs3_value(const Fs3Sum& x, int slot, size_t i, int par, double S2, double r0, double inv) {
     if (slot == FS3_S) return __ldcg(x.raw[par] + i);
@@ -759,15 +763,61 @@ __device__ __forceinline__ void fs3_row_fill(const Fs3Dev& d, Fs3Sh<NT>& sh, int
             if (p >= base && p < base + FS3_ROW_CHUNK) sh.rowl[p - base] = (unsigned short)(w * 32u + (unsigned)__ffs(x) - 1u);
 }
 
+// The chain of an exact sum over more than 32 dirty values (rare), by warp 0 of the leader CTA behind sh.tPoff: the entries
+// ranked by index into shared memory, the serial walk by lane 0 (its total is returned there), the certificates in parallel.
+// Any failure sets *fail.  Out of line, so that the usual chain stays one straight run of code.
+template <int NT>
+__device__ __noinline__ double fs3_chain_wide(const Fs3Sum& x, Fs3Sh<NT>& sh, size_t eb, int D, unsigned long long Ptot, int* fail) {
+    const int lane = threadIdx.x & 31;
+    double total = 0.0;
+#pragma unroll 1
+    for (int e = lane; e < D; e += 32) sh.ukey[e] = __ldcg(x.entKey + eb + e);
+    __syncwarp();
+#pragma unroll 1
+    for (int e = lane; e < D; e += 32) {               // rank = position in index order (keys are distinct)
+        const unsigned key = sh.ukey[e];
+        int rank = 0;
+#pragma unroll 1
+        for (int j = 0; j < D; ++j) rank += sh.ukey[j] < key ? 1 : 0;
+        sh.skey[rank] = key; sh.sP[rank] = sh.tPoff[__ldcg(x.entTile + eb + e)] + __ldcg(x.entP + eb + e);
+        sh.sV[rank] = __ldcg(x.entV + eb + e); sh.sL[rank] = __ldcg(x.entL + eb + e);
+    }
+    __syncwarp();
+    if (lane == 0) {                                   // the serial part: one integer add + one FP add per dirty value
+        double sq = 0.0; unsigned long long prev = 0;
+#pragma unroll 1
+        for (int o = 0; o < D; ++o) {
+            const unsigned long long p = sh.sP[o];
+            sh.bef[o] = sq;
+            sq = pfc_u2d(pfc_d2u(sq) + (p - prev)) + sh.sV[o];
+            sh.aft[o] = sq; prev = p;
+        }
+        int ok = 1;
+        total = x3_apply(sq, Ptot - prev, -1, &ok);
+        if (!ok) *fail = 1;
+    }
+    __syncwarp();
+#pragma unroll 1
+    for (int o = lane; o < D; o += 32) {               // certificates of the clean runs, in parallel
+        const unsigned long long dp = sh.sP[o] - (o ? sh.sP[o - 1] : 0ull);
+        int ok = 1;
+        (void)x3_apply(sh.bef[o], dp, sh.sL[o], &ok);
+        if (!ok) *fail = 1;
+    }
+    return total;
+}
+
 // One exact sequential sum over the n_glob values held tile-wise in shared memory (thread t owns values t*K .. t*K+K-1 of its
 // tile, stored at vals[k*NT + t]).  toff = approximate sum of everything in front of this tile.  Returns the exact total
 // (identical in every CTA).  pub = 1: the chain's leader also publishes the tile prefixes and the sorted dirty values, and *run
 // keeps this thread's state, so that fs3_xsum_emit can store the exact inclusive prefixes afterwards (sh.fail = 0; with
 // sh.fail = 1 the serial walk has already stored them to `out`).  Contains ONE grid barrier (`round`).
+// fs3_xsum_body is the sum inlined where it is on every step's path (the post kernel's S sum); fs3_xsum is its one out-of-line
+// copy for every other sum.
 template <int NT, bool GT = false>
-__device__ __noinline__ double fs3_xsum(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
-                                        unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run,
-                                        const Fs3Hook* hook = nullptr) {
+__device__ __forceinline__ double fs3_xsum_body(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
+                                                unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run,
+                                                const Fs3Hook* hook) {
     const int tid = threadIdx.x, lane = tid & 31, pp = round & 1;
     const unsigned b = blockIdx.x;
     const size_t T = (size_t)NT * K;
@@ -919,40 +969,7 @@ __device__ __noinline__ double fs3_xsum(const Fs3Sum& x, Fs3Sh<NT>& sh, const do
                 }
                 if (!ok) fail = 1;
             } else {
-#pragma unroll 1
-                for (int e = lane; e < D; e += 32) sh.ukey[e] = __ldcg(x.entKey + eb + e);
-                __syncwarp();
-#pragma unroll 1
-                for (int e = lane; e < D; e += 32) {               // rank = position in index order (keys are distinct)
-                    const unsigned key = sh.ukey[e];
-                    int rank = 0;
-#pragma unroll 1
-                    for (int j = 0; j < D; ++j) rank += sh.ukey[j] < key ? 1 : 0;
-                    sh.skey[rank] = key; sh.sP[rank] = sh.tPoff[__ldcg(x.entTile + eb + e)] + __ldcg(x.entP + eb + e);
-                    sh.sV[rank] = __ldcg(x.entV + eb + e); sh.sL[rank] = __ldcg(x.entL + eb + e);
-                }
-                __syncwarp();
-                if (lane == 0) {                                   // the serial part: one integer add + one FP add per dirty value
-                    double sq = 0.0; unsigned long long prev = 0;
-#pragma unroll 1
-                    for (int o = 0; o < D; ++o) {
-                        const unsigned long long p = sh.sP[o];
-                        sh.bef[o] = sq;
-                        sq = pfc_u2d(pfc_d2u(sq) + (p - prev)) + sh.sV[o];
-                        sh.aft[o] = sq; prev = p;
-                    }
-                    int ok = 1;
-                    total = x3_apply(sq, Ptot - prev, -1, &ok);
-                    if (!ok) fail = 1;
-                }
-                __syncwarp();
-#pragma unroll 1
-                for (int o = lane; o < D; o += 32) {               // certificates of the clean runs, in parallel
-                    const unsigned long long dp = sh.sP[o] - (o ? sh.sP[o - 1] : 0ull);
-                    int ok = 1;
-                    (void)x3_apply(sh.bef[o], dp, sh.sL[o], &ok);
-                    if (!ok) fail = 1;
-                }
+                total = fs3_chain_wide<NT>(x, sh, eb, D, Ptot, &fail);
             }
             __syncwarp();
             fail = __any_sync(0xffffffffu, fail);
@@ -991,15 +1008,21 @@ __device__ __noinline__ double fs3_xsum(const Fs3Sum& x, Fs3Sh<NT>& sh, const do
     if (run) { run->a_first = a_first; run->Pex = Pex; run->e_run = e_run; }
     return sh.total;
 }
+template <int NT, bool GT = false>
+__device__ __noinline__ double fs3_xsum(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
+                                        unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run) {
+    return fs3_xsum_body<NT, GT>(x, sh, vals, K, nt, toff, slot, round, m32, out, par, S2, r0, inv, extraQ, pub, run, nullptr);
+}
 
 // The exact inclusive prefix c_j of every value of this tile after fs3_xsum(pub = 1) of round `round` (nothing when that sum took
 // the serial walk: it has stored them already).  cert == nullptr: c_j goes to out[j].  Otherwise fl(c_j / cert->S) goes to
 // out[j], and the return value is 1 when some comb value may lie on the other side of it than of the CDF the reference computes
 // (x3_cdf_near_comb), or a clean run failed its certificate.  tend: the tile's last stored value goes to tileEnd[tile].
-// vals must still hold the values the sum saw.  Contains one block barrier.
+// vals must still hold the values the sum saw.  Contains one block barrier.  Inlined as fs3_xsum_emit_body where it is on the
+// path of a config-3 resample (the certified CDF); fs3_xsum_emit is the out-of-line copy for the exact CDF and comb.
 template <int NT, bool GT = false>
-__device__ __noinline__ int fs3_xsum_emit(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
-                                          double* out, int tend, const Fs3Cert* cert, int tslot) {
+__device__ __forceinline__ int fs3_xsum_emit_body(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
+                                                  double* out, int tend, const Fs3Cert* cert, int tslot) {
     const int tid = threadIdx.x, lane = tid & 31;
     const unsigned b = blockIdx.x;
     const size_t T = (size_t)NT * K;
@@ -1044,7 +1067,7 @@ __device__ __noinline__ int fs3_xsum_emit(const Fs3Sum& x, Fs3Sh<NT>& sh, const 
             else { Pc += inc; c = x3_apply(base, Pc - Pb, inc ? lvl : -1, &ok); }
             o = c;
             if (cert) {
-                o = fs3_div(c, cert->S);
+                o = c / cert->S;
                 if (g0 + k < x.n) near |= x3_cdf_near_comb(o, cert->r0, cert->inv, cert->ninv, cert->n, cert->dl, cert->ab);
             }
             if (g0 + k < x.n) out[g0 + k] = o;
@@ -1055,6 +1078,11 @@ __device__ __noinline__ int fs3_xsum_emit(const Fs3Sum& x, Fs3Sh<NT>& sh, const 
     if (!ok) { atomicAdd(&x.st->cert_fail, 1); near = 1; }
     if (tslot >= 0) FS3_TRACE(tslot);
     return near;
+}
+template <int NT, bool GT = false>
+__device__ __noinline__ int fs3_xsum_emit(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned m32, const Fs3Run* run, int round,
+                                          double* out, int tend, const Fs3Cert* cert, int tslot) {
+    return fs3_xsum_emit_body<NT, GT>(x, sh, vals, K, m32, run, round, out, tend, cert, tslot);
 }
 
 // warp-cooperative 32-way search of one r over c[0 .. n): returns the lower bound (all lanes)
@@ -1134,7 +1162,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     FS3_TRACE(0);
     // the comb of a resample this step might need: r = Uniform::new(0, 1/n).sample(rng) (fs1.rs:219-220), one draw per resample, and
     // (n a power of two) its closed-form table, built by an otherwise idle warp inside the first exact sum
-    const double inv = fs3_div(1.0, (double)ng);
+    const double inv = 1.0 / (double)ng;
     const double r0 = pfc_u01_52(pfc_blk_u64(pfc_rng_block(seed, PFC_STREAM_FS_RESAMPLE, st->resamples, 0), 0)) * (inv - 0.0) + 0.0;
     // ---------------- S = sum w_raw (normalize_weights fs1.rs:196-203) ----------------
     // With n = 2^p, p <= FS3_CERT_MAX_LOG2N, the leader also publishes what every CTA needs to emit the exact prefixes P_j of w_raw:
@@ -1143,7 +1171,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     Fs3Hook hook;
     hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.step = step; hook.k_last = k_last; hook.po = &po;
     Fs3Run run;
-    const double S = fs3_xsum<NT, GTILE>(x, sh, vals, K, nt, toff, FS3_S, FS3_R_S, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
+    const double S = fs3_xsum_body<NT, GTILE>(x, sh, vals, K, nt, toff, FS3_S, FS3_R_S, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
     const int S_walked = sh.fail;
     FS3_TRACE(1);
     // ---------------- gate: neff = 1 / sum w^2 < NTH (compute_neff fs1.rs:186-193, fs1.rs:262-263) ----------------
@@ -1152,8 +1180,8 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     // (n + 64) 2^-51 relatively; only when neff lands that close to NTH is the exact sequential sum walked (below, once wn_all is written).
     double Q = (unsigned)tid < nt ? __ldcg(x.tileQ + tid) : 0.0, dummy = 0.0;
     fs3_block_sum2<NT>(Q, dummy, sh.red[1], sh.wd[1]);
-    if (S > 0.0) Q = fs3_div(fs3_div(Q, S), S);
-    double neff = Q > 0.0 ? fs3_div(1.0, Q) : 0.0;
+    if (S > 0.0) Q = Q / S / S;
+    double neff = Q > 0.0 ? 1.0 / Q : 0.0;
     const double slack = 16.0 * (double)(ng + 64) * 2.220446049250313e-16;
     // The error bound of the shortcut assumes that no w_raw^2 that matters under- or overflows: with S inside [1e-120, 1e120] the
     // squares of all weights within 1e-34 of the largest are normal numbers.  Outside (e.g. an outlier observation that drives
@@ -1172,7 +1200,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         cp.S = S; cp.r0 = r0; cp.inv = inv; cp.ninv = (double)ng; cp.n = ng;
         cp.dl = g / (1.0 - g) * (1.0 + 9.5367431640625e-07);             // gamma_4n (1 + 2^-20)
         cp.ab = (4.0 * (double)ng + 4.0) * 4.9406564584124654e-324 + (double)(log2n + 4) * 1.1102230246251565e-16;
-        const int near = fs3_xsum_emit<NT, GTILE>(x, sh, vals, K, m32, &run, FS3_R_S, d.cum_all, 1, &cp, -1);
+        const int near = fs3_xsum_emit_body<NT, GTILE>(x, sh, vals, K, m32, &run, FS3_R_S, d.cum_all, 1, &cp, -1);
         if (__syncthreads_or(near) && tid == 0) x.flagsg[FS3_CERT_FLAG] = 1;
         FS3_TRACE(4);
     }
@@ -1181,7 +1209,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
 #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) {
         double v = vals[k * NT + tid];
-        if (S > 0.0) v = fs3_div(v, S);
+        if (S > 0.0) v = v / S;
         vals[k * NT + tid] = v;
         const size_t i = g0 + k;
         if (i < ng) {
