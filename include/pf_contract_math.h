@@ -132,7 +132,9 @@ enum {
     PFC_STREAM_REGION_A    = 10, /* init_region, call 0: (x fraction, y fraction) of particle i         */
     PFC_STREAM_REGION_B    = 11, /* init_region, call 0: (yaw fraction, unused) of particle i           */
     /* odometry motion model (not in the reference; DESIGN §3.14, include/pf_odom_math.h), call and index as PF_PREDICT's */
-    PFC_STREAM_PF_ODOM     = 12  /* (zc = the third normal, unused) of particle i                       */
+    PFC_STREAM_PF_ODOM     = 12, /* (zc = the third normal, unused) of particle i                       */
+    /* FastSLAM's odometry motion model (DESIGN §3.15, include/fs_odom_math.h), call and index as FS_PREDICT's */
+    PFC_STREAM_FS_ODOM     = 13  /* (zc = the third normal of the odometry move, unused) of particle i  */
 };
 /* A pose drawn uniformly over the box [x0, x1] x [y0, y1] from three 53-bit fractions (augmented MCL's injection and init_region):
  * x = x0 + fx * (x1 - x0), y = y0 + fy * (y1 - y0), yaw = fyaw * 2 pi - pi. */

@@ -466,6 +466,25 @@ int  pfgpu_fs_set_variant(pfgpu_fs*, int variant);
 int  pfgpu_fs_step_unknown(pfgpu_fs*, const double u[2], const double* z2, size_t k, double gate_d2, int* did_resample);
 /* (matched, born, dropped) observation counts of the last pfgpu_fs_step_unknown, summed over this handle's particles; synchronises */
 int  pfgpu_fs_assoc_counts(pfgpu_fs*, uint64_t counts[3]);
+/* The odometry motion model for FastSLAM (not in the reference, whose fastslam1 / fastslam2 only have the velocity model
+ * fs1.rs:123-137, fs2.rs:95-120; DESIGN §3.15): every particle moves by the increment between two wheel-odometry poses instead of
+ * by a control over dt.  odom = (x, y, yaw) of the previous odometry pose, then of the current one.  The rule, its evaluation order
+ * and its draws are include/fs_odom_math.h's: include/pf_odom_math.h's increment and move (yaw wrapped), and for FastSLAM 2.0 with
+ * observations the proposal of the first observation fused with the prior the increment induces (covariance floored by 1e-8 on
+ * the diagonal).  Standing still (odom' == odom) moves no particle; weights and maps still update from the observations.  Two rules
+ * of FastSLAM 2.0 differ from its velocity proposal: a particle whose increment has no noise (every sigma 0) takes the noise-free
+ * move without a draw; a particle with nothing to fuse (the first observation's landmark not initialised, cov00 >= 100, or with
+ * unknown association no slot matched) takes FastSLAM 1.0's odometry move, not a sample of the linearised prior.
+ * pfgpu_fs_set_odom_noise: alpha = (alpha1 .. alpha4) as pfgpu_pf_set_odom_noise, each finite and >= 0, else PFGPU_ERR_INVALID; a
+ *   handle starts at 0.2 each.  pfgpu_fs_odom_noise returns them.  Every rank of a sharded engine makes the same calls.
+ * pfgpu_fs_step_odom / pfgpu_fs_step_unknown_odom: pfgpu_fs_step / pfgpu_fs_step_unknown with this motion in place of u, with the
+ *   same refusals (a non-finite component of odom: PFGPU_ERR_INVALID, as a non-finite u is; known ids while existence counters are
+ *   on, unknown association on FastSLAM 1.0: PFGPU_ERR_UNSUPPORTED); k = 0 without existence counters is pfgpu_fs_step_odom with
+ *   k = 0.  They mix freely with the velocity steps on one handle. */
+int  pfgpu_fs_set_odom_noise(pfgpu_fs*, const double alpha[4]);
+int  pfgpu_fs_odom_noise(pfgpu_fs*, double alpha[4]);
+int  pfgpu_fs_step_odom(pfgpu_fs*, const double odom[6], const pfgpu_fs_obs* z, size_t k, int* did_resample);
+int  pfgpu_fs_step_unknown_odom(pfgpu_fs*, const double odom[6], const double* z2, size_t k, double gate_d2, int* did_resample);
 int  pfgpu_fs_count(pfgpu_fs*, size_t* n_local, size_t* n_global, size_t* n_landmarks);
 /* Estimate (not in the reference, whose callers read the best particle's map, keeping landmarks with cov00 < 100).  With W the sum
  * of the stored weights (never assumed to be 1):

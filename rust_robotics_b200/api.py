@@ -117,6 +117,7 @@ EXPORTS = [
     "pfgpu_fs_time_main_kernel", "pfgpu_pf_mark", "pfgpu_pf_elapsed_ms", "pfgpu_fs_mark", "pfgpu_fs_elapsed_ms",
     "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
     "pfgpu_fs_moments", "pfgpu_fs_estimate_merge", "pfgpu_fs_step_unknown", "pfgpu_fs_assoc_counts",
+    "pfgpu_fs_set_odom_noise", "pfgpu_fs_odom_noise", "pfgpu_fs_step_odom", "pfgpu_fs_step_unknown_odom",
     "pfgpu_fs_history_enable", "pfgpu_fs_history_window", "pfgpu_fs_path", "pfgpu_fs_path_moments",
     "pfgpu_fs_existence_enable", "pfgpu_fs_existence_counts", "pfgpu_fs_existence_removed",
     "pfgpu_pf_recovery_enable", "pfgpu_pf_recovery_state", "pfgpu_pf_init_region",
@@ -249,6 +250,10 @@ def load_library():
     L.pfgpu_fs_estimate_merge.argtypes = [C.POINTER(_FsPoseMoments), C.POINTER(c_dp), C.c_int, C.c_size_t, c_dp, c_dp, c_dp, c_dp, c_dp]
     L.pfgpu_fs_step_unknown.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.POINTER(C.c_int)]
     L.pfgpu_fs_assoc_counts.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.pfgpu_fs_set_odom_noise.argtypes = [vp, c_dp]
+    L.pfgpu_fs_odom_noise.argtypes = [vp, c_dp]
+    L.pfgpu_fs_step_odom.argtypes = [vp, c_dp, C.POINTER(_FsObs), C.c_size_t, C.POINTER(C.c_int)]
+    L.pfgpu_fs_step_unknown_odom.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.POINTER(C.c_int)]
     L.pfgpu_fs_history_enable.argtypes = [vp, C.c_size_t]
     L.pfgpu_fs_history_window.argtypes = [vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.pfgpu_fs_path.argtypes = [vp, C.c_size_t, C.c_size_t, C.POINTER(C.c_uint64), c_u32p, c_dp, C.POINTER(C.c_size_t)]
@@ -1087,6 +1092,37 @@ class FastSlam1:
 
     step = fastslam_update
 
+    # -- odometry motion model (not in fs1.rs / fs2.rs, whose steps take a velocity command; DESIGN §3.15) --
+    def set_odometry_noise(self, alpha1=0.2, alpha2=0.2, alpha3=0.2, alpha4=0.2):
+        """ROS AMCL's odom_alpha1..4 (diff-corrected), as ParticleFilterLocalizer.set_odometry_noise: each finite and >= 0; a handle
+        starts at 0.2 each.  On a sharded engine every rank makes the same call."""
+        a = _f64([alpha1, alpha2, alpha3, alpha4])
+        _check(self.L, self.L.pfgpu_fs_set_odom_noise(self.h, _dp(a)))
+
+    def odometry_noise(self):
+        """(alpha1, alpha2, alpha3, alpha4)"""
+        a = np.empty(4)
+        _check(self.L, self.L.pfgpu_fs_odom_noise(self.h, _dp(a)))
+        return tuple(float(v) for v in a)
+
+    def fastslam_update_odometry(self, odom_prev, odom_cur, z, want_flag=True):
+        """fastslam_update with the odometry motion model: every particle moves by the increment from odometry pose odom_prev =
+        (x, y, yaw) to odom_cur (include/fs_odom_math.h) instead of by a control over dt.  Returns whether the step resampled
+        (None when want_flag is False: no host sync)."""
+        o = _PfBase._odom_pair(odom_prev, odom_cur)
+        did = C.c_int()
+        _check(self.L, self.L.pfgpu_fs_step_odom(self.h, _dp(o), self._obs(z), len(z), C.byref(did) if want_flag else None))
+        return bool(did.value) if want_flag else None
+
+    @staticmethod
+    def step_all_odometry(ranks, odom_prev, odom_cur, z):
+        """one fastslam_update_odometry on every in-process rank: enqueue everywhere first, then synchronise; returns did_resample"""
+        for g in ranks:
+            g.fastslam_update_odometry(odom_prev, odom_cur, z, want_flag=False)
+        for g in ranks:
+            g.sync()
+        return ranks[0].did_resample()
+
     def get_observations(self, x_true, landmarks_xy, call):
         """fs1.rs:277-299 on the device (Philox stream OBS keyed by the handle's seed, `call` and the landmark id)"""
         xt, lm = _f64(x_true), _f64(landmarks_xy)
@@ -1283,6 +1319,11 @@ class FastSlam2(FastSlam1):
     def fastslam2_update(self, u, z, **kw):
         return self.fastslam_update(u, z, **kw)
 
+    def fastslam2_update_odometry(self, odom_prev, odom_cur, z, **kw):
+        """fastslam2_update with the odometry motion model: the proposal fuses the first observation with the prior the odometry
+        increment induces (include/fs_odom_math.h)"""
+        return self.fastslam_update_odometry(odom_prev, odom_cur, z, **kw)
+
     # -- unknown data association (not in fs2.rs; the rule of ekf_slam.rs:284-308 per particle, DESIGN §3.5) --
     def fastslam2_update_unknown(self, u, z, gate_d2=16.0, want_flag=True):
         """One step from observations WITHOUT landmark ids: z = k (d, angle) pairs.  Every particle associates each observation with
@@ -1296,6 +1337,24 @@ class FastSlam2(FastSlam1):
         _check(self.L, self.L.pfgpu_fs_step_unknown(self.h, _dp(uu), _dp(zz) if zz.size else None, zz.shape[0], float(gate_d2),
                                                     C.byref(did) if want_flag else None))
         return bool(did.value) if want_flag else None
+
+    def fastslam2_update_unknown_odometry(self, odom_prev, odom_cur, z, gate_d2=16.0, want_flag=True):
+        """fastslam2_update_unknown with the odometry motion model (see fastslam2_update_odometry)"""
+        o = _PfBase._odom_pair(odom_prev, odom_cur)
+        zz = _f64(z).reshape(-1, 2) if len(z) else np.zeros((0, 2))
+        did = C.c_int()
+        _check(self.L, self.L.pfgpu_fs_step_unknown_odom(self.h, _dp(o), _dp(zz) if zz.size else None, zz.shape[0], float(gate_d2),
+                                                         C.byref(did) if want_flag else None))
+        return bool(did.value) if want_flag else None
+
+    @staticmethod
+    def step_all_unknown_odometry(ranks, odom_prev, odom_cur, z, gate_d2=16.0):
+        """one fastslam2_update_unknown_odometry on every in-process rank: enqueue everywhere, then synchronise"""
+        for g in ranks:
+            g.fastslam2_update_unknown_odometry(odom_prev, odom_cur, z, gate_d2, want_flag=False)
+        for g in ranks:
+            g.sync()
+        return ranks[0].did_resample()
 
     @staticmethod
     def step_all_unknown(ranks, u, z, gate_d2=16.0):

@@ -39,6 +39,7 @@
 #include "x3_core.h"
 #include "../../include/fs_ekf_math.h"
 #include "../../include/fs2_math.h"
+#include "../../include/fs_odom_math.h"
 
 #define FS3_MAXG 8
 #define FS3_MAX_OBS 31            // observations per EKF launch (one warp each, plus the helper warp)
@@ -478,6 +479,72 @@ fs2_propose_kernel(const __grid_constant__ Fs3Dev d, Fs3Obs ob, double u0, doubl
     const double mc[9] = { 0.1, 0.0, 0.0, 0.0, 0.1, 0.0, 0.0, 0.0, 0.01 };          // MOTION_COV fs2.rs:31
     double x = d.px[cur][i], y = d.py[cur][i], a = d.pyaw[cur][i];
     fs2_propose_pose(&x, &y, &a, &L, u0, u1, dt, ob.d, ob.angle, r00, r11, mc, n0, n1, n2);
+    d.px[cur][i] = x; d.py[cur][i] = y; d.pyaw[cur][i] = a;
+}
+
+// The odometry motion model (DESIGN §3.15, include/fs_odom_math.h).  FastSLAM 1.0, and FastSLAM 2.0 without observations: every
+// pose moved by the increment m in place, one thread per slot, ahead of the EKF launch (which then runs with flags bit 1, so its
+// helper warps only gather the weights).  (za, zb) are the velocity model's pair, taken from nz[] when the previous post kernel
+// drew it; zc is PFC_STREAM_FS_ODOM's.
+__global__ void __launch_bounds__(128)
+fs3_odom_predict_kernel(const __grid_constant__ Fs3Dev d, PfOdom m, uint64_t seed, uint32_t call, unsigned step) {
+    pf_grid_dep_sync();
+    if (d.G > 1 && d.wait_inline) {             // peers read this rank's poses until their previous post kernel is over
+        if (threadIdx.x == 0) fs3_wait_peers(d, 1, step);
+        __syncthreads();
+    }
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= d.n) return;
+    const int cur = d.st->cur;
+    double za, zb, zc, unused;
+    if (d.st->noise_call == call + 1u) { za = d.nz[0][i]; zb = d.nz[1][i]; }
+    else pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_PREDICT, call, (uint64_t)d.off + i), &za, &zb);
+    pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_ODOM, call, (uint64_t)d.off + i), &zc, &unused);
+    double x = d.px[cur][i], y = d.py[cur][i], a = d.pyaw[cur][i];
+    fs_odom_move(&m, za, zb, zc, &x, &y, &a);
+    d.px[cur][i] = x; d.py[cur][i] = y; d.pyaw[cur][i] = a;
+}
+
+// (fs2_propose_kernel's read, for its odometry twin) slot i's copy of landmark l as it stands before this step's updates: own column, or the ancestor's through the landmark's row
+__device__ __forceinline__ FsLm fs3_read_lm(const Fs3Dev& d, int rcur, int l, unsigned i) {
+    const size_t ld = d.ld;
+    const int sl = d.lmst[l];
+    const int buf = sl & 1;
+    const size_t lbase = (size_t)l * 6 * ld;
+    const double* p = d.lm[buf] + lbase + i;
+    if (sl >> 1) {
+        const unsigned ref = d.rows[rcur][(size_t)((sl >> 1) - 1) * ld + i];
+        const double* base = d.G > 1 ? reinterpret_cast<const double*>(d.peer[ref >> 28] + d.o_lm[buf]) : d.lm[buf];
+        p = base + lbase + (ref & 0x0FFFFFFFu);
+    }
+    FsLm L;
+    L.x = p[0]; L.y = p[ld]; L.c00 = p[2 * ld]; L.c01 = p[3 * ld]; L.c10 = p[4 * ld]; L.c11 = p[5 * ld];
+    return L;
+}
+// FastSLAM 2.0 with odometry and observations: fs2_propose_kernel's twin, the proposal's prior from the increment m
+// (fs2_odom_case / fs2_odom_pose: standing still takes the noise-free move, an uninitialised landmark the odometry move)
+__global__ void __launch_bounds__(128)
+fs2_propose_odom_kernel(const __grid_constant__ Fs3Dev d, Fs3Obs ob, PfOdom m, double r00, double r11, uint64_t seed, uint32_t call,
+                        unsigned step) {
+    pf_grid_dep_sync();
+    Fs3State* st = d.st;
+    if (d.G > 1 && d.wait_inline) {             // peers' rows / maps are stable once their previous post kernel is over
+        if (threadIdx.x == 0) fs3_wait_peers(d, 1, step);
+        __syncthreads();
+    }
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= d.n) return;
+    const int cur = st->cur, rcur = st->rcur;
+    const FsLm L = fs3_read_lm(d, rcur, ob.lm_id, i);
+    const int kase = fs2_odom_case(&m, &L);
+    double n0 = 0.0, n1 = 0.0, n2 = 0.0, unused;
+    if (kase != FS_ODOM_STILL) {
+        if (st->noise_call == call + 1u) { n0 = d.nz[0][i]; n1 = d.nz[1][i]; }
+        else pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_PREDICT, call, (uint64_t)d.off + i), &n0, &n1);
+        pfc_normal_pair(pfc_rng_block(seed, kase == FS_ODOM_MOVE ? PFC_STREAM_FS_ODOM : PFC_STREAM_FS2_POSE3, call, (uint64_t)d.off + i), &n2, &unused);
+    }
+    double x = d.px[cur][i], y = d.py[cur][i], a = d.pyaw[cur][i];
+    fs2_odom_pose(kase, &m, &x, &y, &a, &L, ob.d, ob.angle, r00, r11, n0, n1, n2);
     d.px[cur][i] = x; d.py[cur][i] = y; d.pyaw[cur][i] = a;
 }
 

@@ -19,11 +19,11 @@
 
 // out-of-line pieces with their own copies (a routine shared with the existing kernels would be register-allocated for all
 // callers); one copy per instantiation of fs3_assoc_kernel, so the untracked kernel's allocation does not depend on the tracked one
-template <bool EX>
+template <bool EX, bool ODOM = false>
 __device__ __noinline__ int fs3a_d2(const FsLm* L, double px, double py, double pyaw, double z0, double z1, double r00, double r11, double* q) {
     return fs_assoc_d2(L, px, py, pyaw, z0, z1, r00, r11, q);
 }
-template <bool EX>
+template <bool EX, bool ODOM = false>
 __device__ __noinline__ double fs3a_update(FsLm* L, double px, double py, double pyaw, double z0, double z1, double r00, double r11) {
     int wrote;
     return fs_update_landmark_v(L, px, py, pyaw, z0, z1, r00, r11, &wrote, 2);    // update_landmark_and_weight fs2.rs:242-280
@@ -33,6 +33,11 @@ __device__ __noinline__ void fs3a_propose(double* x, double* y, double* a, const
                                           double r00, double r11, double n0, double n1, double n2) {
     const double mc[9] = { 0.1, 0.0, 0.0, 0.0, 0.1, 0.0, 0.0, 0.0, 0.01 };           // MOTION_COV fs2.rs:31
     fs2_propose_pose(x, y, a, L, u0, u1, dt, z0, z1, r00, r11, mc, n0, n1, n2);
+}
+template <bool EX>
+__device__ __noinline__ void fs3a_odom_pose(int kase, const PfOdom* m, double* x, double* y, double* a, const FsLm* L, double z0, double z1,
+                                            double r00, double r11, double n0, double n1, double n2) {
+    fs2_odom_pose(kase, m, x, y, a, L, z0, z1, r00, r11, n0, n1, n2);
 }
 __device__ __forceinline__ FsLm fs3a_load(const double* p, size_t ld) {
     FsLm L;
@@ -46,7 +51,7 @@ __device__ __forceinline__ void fs3a_store(double* p, size_t ld, const FsLm& L) 
 __device__ __forceinline__ int fs3a_tbuf(int s) { return (s & 1) ^ ((s >> 1) ? 1 : 0); }
 
 // A(pose, z) over slot i's map (every landmark materialised): the matching slot or -1, and the lowest empty slot or -1
-template <bool EX>
+template <bool EX, bool ODOM = false>
 __device__ __forceinline__ void fs3a_scan(const Fs3Dev& d, unsigned i, double px, double py, double pyaw, double z0, double z1, double r00,
                                           double r11, double gate_d2, int* match, int* empty) {
     const size_t ld = d.ld;
@@ -59,7 +64,7 @@ __device__ __forceinline__ void fs3a_scan(const Fs3Dev& d, unsigned i, double px
         if (!(c00 < 100.0)) { if (e < 0) e = (int)l; continue; }       // is_initialized fs2.rs:49-51
         FsLm L = fs3a_load(p, ld);
         double q;
-        if (fs3a_d2<EX>(&L, px, py, pyaw, z0, z1, r00, r11, &q) && q < best) { best = q; bl = (int)l; }
+        if (fs3a_d2<EX, ODOM>(&L, px, py, pyaw, z0, z1, r00, r11, &q) && q < best) { best = q; bl = (int)l; }
     }
     *match = bl >= 0 && best < gate_d2 ? bl : -1;
     *empty = e;
@@ -149,6 +154,136 @@ fs3_assoc_kernel(const __grid_constant__ Fs3Dev d, const double* __restrict__ z2
             double* p = d.lm[tb] + (size_t)l * 6 * ld + i;
             FsLm L = fs3a_load(p, ld);
             w = w * fs3a_update<EX>(&L, x, y, a, zj0, zj1, r00, r11);
+            fs3a_store(p, ld, L);
+            if constexpr (EX) {
+                int* t = ex + (size_t)tb * plane + (size_t)l * ld + i;
+                *t = born ? (1 | FS3_EX_SEEN) : (((*t & ~FS3_EX_SEEN) + 1) | FS3_EX_SEEN);
+            }
+        }
+        // ---- negative evidence at the sampled pose: every initialised copy in range that no observation went to ----
+        if constexpr (EX) {
+#pragma unroll 1
+            for (unsigned l = 0; l < d.m; ++l) {
+                const int tb = fs3a_tbuf(d.lmst[l]);
+                int* t = ex + (size_t)tb * plane + (size_t)l * ld + i;
+                const int v = *t;
+                if (v & FS3_EX_SEEN) { *t = v & ~FS3_EX_SEEN; continue; }
+                double* p = d.lm[tb] + (size_t)l * 6 * ld + i;
+                if (!(p[2 * ld] < 100.0)) continue;
+                const double dx = p[0] - x, dy = p[ld] - y;
+                if (!(sqrt(dx * dx + dy * dy) <= X.range)) continue;
+                *t = v - 1;
+                if (v - 1 < 0) {                                       // removed: create_particles' fresh landmark, the slot is empty
+                    const FsLm F = { 0.0, 0.0, 1000.0, 0.0, 0.0, 1000.0 };
+                    fs3a_store(p, ld, F);
+                    cr++;
+                }
+            }
+        }
+        d.px[cur][i] = x; d.py[cur][i] = y; d.pyaw[cur][i] = a;
+    }
+    // ---- weights and 64-particle partials to every rank; the counters ----
+    const unsigned lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    const double ws = warp_sum(w);                                     // honest (tree-order) sum: steers x3_classify only
+    if (lane == 0) s_part[wid] = ws;
+    const unsigned long long c3[3] = { __reduce_add_sync(0xffffffffu, cm), __reduce_add_sync(0xffffffffu, cb), __reduce_add_sync(0xffffffffu, cd) };
+    if (lane < 3 && c3[lane]) atomicAdd(counts + lane, c3[lane]);
+    if constexpr (EX) {
+        const unsigned long long c = __reduce_add_sync(0xffffffffu, cr);
+        if (lane == 3 && c) atomicAdd(removed, c);
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int gg = 0; gg < d.G; ++gg) {
+        double* wr = (d.G > 1 ? reinterpret_cast<double*>(d.peer[gg] + d.o_wraw[par]) : d.wraw[par]) + d.off;
+        if (i < d.n) wr[i] = w;
+        const unsigned ge = blockIdx.x * (FS3_ASSOC_NT / 64) + threadIdx.x;
+        if (threadIdx.x < FS3_ASSOC_NT / 64 && ge < d.npart) {
+            double* pp = d.G > 1 ? reinterpret_cast<double*>(d.peer[gg] + d.o_part[par]) : d.part[par];
+            pp[(size_t)d.rank * d.npart + ge] = s_part[2 * threadIdx.x] + s_part[2 * threadIdx.x + 1];
+        }
+    }
+}
+
+// fs3_assoc_kernel with the odometry motion model (DESIGN §3.15, include/fs_odom_math.h): the increment m replaces (u, dt) and
+// sqrt(Q).  The proposal's landmark is the association at the noise-free move mu; the pose comes from fs2_odom_pose (no match: the
+// odometry move); without observations (EX, k = 0) it is the odometry move of FastSLAM 1.0.  Everything after the pose is
+// fs3_assoc_kernel's.  A kernel of its own, so that the velocity kernel's code stays as it was.
+template <bool EX>
+__global__ void __launch_bounds__(FS3_ASSOC_NT)
+fs3_assoc_odom_kernel(const __grid_constant__ Fs3Dev d, const double* __restrict__ z2, int k, double gate_d2, PfOdom m, double r00, double r11,
+                      uint64_t seed, uint32_t call, unsigned step, unsigned long long* counts, const __grid_constant__ Fs3Ex X,
+                      unsigned long long* removed) {
+    pf_grid_dep_sync();
+    __shared__ double s_part[FS3_ASSOC_NT / 32];
+    if (d.G > 1 && d.wait_inline) {             // peers' rows / poses / maps / tau are stable once their previous post kernel is over
+        if (threadIdx.x == 0) fs3_wait_peers(d, 1, step);
+        __syncthreads();
+    }
+    const Fs3State* st = d.st;
+    const int cur = st->cur, rcur = st->rcur, par = (int)(step & 1u);
+    const size_t ld = d.ld, plane = (size_t)d.m * ld;
+    int* const ex = X.base[d.rank];
+    const bool obs = !EX || k > 0;
+    const unsigned i = blockIdx.x * FS3_ASSOC_NT + threadIdx.x;
+    double w = 0.0;
+    unsigned cm = 0, cb = 0, cd = 0, cr = 0;
+    if (i < d.n) {
+        double x = d.px[cur][i], y = d.py[cur][i], a = d.pyaw[cur][i];
+        w = d.w[i];                                                    // Particle::weight
+        double n0, n1, n2, unused;
+        if (st->noise_call == call + 1u) { n0 = d.nz[0][i]; n1 = d.nz[1][i]; }      // drawn by the previous post kernel's idle warps
+        else pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_PREDICT, call, (uint64_t)d.off + i), &n0, &n1);
+        // ---- proposal scan at the noise-free move mu, materialising every landmark (and its tau) read through a row into
+        //      column i of the other buffer ----
+        const double z0 = obs ? z2[0] : 0.0, z1 = obs ? z2[1] : 0.0;
+        double xp0 = x, xp1 = y, xp2 = a;
+        fs_odom_move(&m, 0.0, 0.0, 0.0, &xp0, &xp1, &xp2);
+        double best = 1.7976931348623157e308;
+        int bl = -1;
+#pragma unroll 1
+        for (unsigned l = 0; l < d.m; ++l) {
+            const int s = d.lmst[l], buf = s & 1;
+            const size_t lbase = (size_t)l * 6 * ld;
+            FsLm L;
+            if (s >> 1) {
+                const unsigned ref = d.rows[rcur][(size_t)((s >> 1) - 1) * ld + i];
+                const double* base = d.G > 1 ? reinterpret_cast<const double*>(d.peer[ref >> 28] + d.o_lm[buf]) : d.lm[buf];
+                L = fs3a_load(base + lbase + (ref & 0x0FFFFFFFu), ld);
+                fs3a_store(d.lm[buf ^ 1] + lbase + i, ld, L);
+                if constexpr (EX)
+                    ex[(size_t)(buf ^ 1) * plane + (size_t)l * ld + i] = X.base[ref >> 28][(size_t)buf * plane + (size_t)l * ld + (ref & 0x0FFFFFFFu)];
+            } else L = fs3a_load(d.lm[buf] + lbase + i, ld);
+            double q;
+            if (obs && L.c00 < 100.0 && fs3a_d2<EX, true>(&L, xp0, xp1, xp2, z0, z1, r00, r11, &q) && q < best) { best = q; bl = (int)l; }
+        }
+        FsLm P = { 0.0, 0.0, 1000.0, 0.0, 0.0, 1000.0 };               // no match: compute_proposal's uninitialised branch (fs2.rs:188-191)
+        if (obs) {
+            if (bl >= 0 && best < gate_d2) P = fs3a_load(d.lm[fs3a_tbuf(d.lmst[bl])] + (size_t)bl * 6 * ld + i, ld);
+            const int kase = fs2_odom_case(&m, &P);                    // no match: P is fresh, the odometry move
+            if (kase != FS_ODOM_STILL)
+                pfc_normal_pair(pfc_rng_block(seed, kase == FS_ODOM_MOVE ? PFC_STREAM_FS_ODOM : PFC_STREAM_FS2_POSE3, call, (uint64_t)d.off + i),
+                                &n2, &unused);
+            fs3a_odom_pose<EX>(kase, &m, &x, &y, &a, &P, z0, z1, r00, r11, n0, n1, n2);
+        } else {                                                       // the known-id k = 0 step's odometry move
+            pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_ODOM, call, (uint64_t)d.off + i), &n2, &unused);
+            fs_odom_move(&m, n0, n1, n2, &x, &y, &a);
+        }
+        // ---- the observations in order: scan at the sampled pose, then update the match, or a birth, or drop; a match or a
+        //      birth marks its slot as seen ----
+#pragma unroll 1
+        for (int j = 0; j < k; ++j) {
+            const double zj0 = z2[2 * j], zj1 = z2[2 * j + 1];
+            int l, e;
+            fs3a_scan<EX, true>(d, i, x, y, a, zj0, zj1, r00, r11, gate_d2, &l, &e);
+            const bool born = l < 0;
+            if (l >= 0) cm++;
+            else if (e >= 0) { l = e; cb++; }
+            else { cd++; continue; }                                   // the map is full: the observation is dropped
+            const int tb = fs3a_tbuf(d.lmst[l]);
+            double* p = d.lm[tb] + (size_t)l * 6 * ld + i;
+            FsLm L = fs3a_load(p, ld);
+            w = w * fs3a_update<EX, true>(&L, x, y, a, zj0, zj1, r00, r11);
             fs3a_store(p, ld, L);
             if constexpr (EX) {
                 int* t = ex + (size_t)tb * plane + (size_t)l * ld + i;

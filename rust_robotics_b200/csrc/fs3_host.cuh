@@ -42,6 +42,7 @@ struct pfgpu_fs {
     char* hs = nullptr; size_t hs_bytes = 0;    // path / path-moments scratch, grows on demand
     int* ex = nullptr; double ex_range = 0.0;   // landmark existence counters [2][m][ld] and their range (fs3_exist.cuh), pfgpu_fs_existence_enable
     void* ex_peer[FS3_MAXG] = {};               // peers' counters mapped through cudaIpc (one process per GPU)
+    double odom_alpha[4] = { PF_ODOM_ALPHA_DEFAULT, PF_ODOM_ALPHA_DEFAULT, PF_ODOM_ALPHA_DEFAULT, PF_ODOM_ALPHA_DEFAULT };   // DESIGN §3.15
 };
 static int fs_hist_record(pfgpu_fs* h, int root);
 static int fs_ex_fill(pfgpu_fs* h);
@@ -448,9 +449,10 @@ static int fs_step_end(pfgpu_fs* h, const Fs3ObsParam& po, int k_last, bool host
     return 0;
 }
 
-extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs* z, size_t k, int* did) {
-    if (!h || !u || (k && !z)) return PFGPU_ERR_INVALID;
-    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+// One known-id step.  om == nullptr: the velocity model with control u; otherwise the odometry increment om (DESIGN §3.15), whose
+// predict (fs3_odom_predict_kernel) or proposal (fs2_propose_odom_kernel) runs ahead of the EKF launch, which then runs with flags
+// bit 1 (poses already this step's).
+static int fs_step_impl(pfgpu_fs* h, const double u[2], const PfOdom* om, const pfgpu_fs_obs* z, size_t k, int* did) {
     if (h->ex) {
         snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "landmark existence counters are enabled: known-id steps are not supported (the EKF launch "
                  "moves landmarks without their counters); disable them with pfgpu_fs_existence_enable(h, 0) first");
@@ -487,14 +489,20 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
     const bool proposed = h->variant == 2 && k > 0;
     if (proposed) {        // FastSLAM 2.0: sample every pose from the proposal of the first observation (fs2.rs:341-346)
         Fs3Obs ob0; ob0.d = z[0].d; ob0.angle = z[0].angle; ob0.lm_id = (int)z[0].lm_id;
-        PF_LAUNCH_PDL(h->ctx, h->pdl, fs2_propose_kernel, cdiv_u(d.n, 128), 128, 0, d, ob0, u[0], u[1], h->cfg.dt, h->cfg.r00, h->cfg.r11,
-                      h->seed, (uint32_t)h->n_step, (unsigned)h->n_step);
-    }
+        if (om)
+            PF_LAUNCH_PDL(h->ctx, h->pdl, fs2_propose_odom_kernel, cdiv_u(d.n, 128), 128, 0, d, ob0, *om, h->cfg.r00, h->cfg.r11,
+                          h->seed, (uint32_t)h->n_step, (unsigned)h->n_step);
+        else
+            PF_LAUNCH_PDL(h->ctx, h->pdl, fs2_propose_kernel, cdiv_u(d.n, 128), 128, 0, d, ob0, u[0], u[1], h->cfg.dt, h->cfg.r00, h->cfg.r11,
+                          h->seed, (uint32_t)h->n_step, (unsigned)h->n_step);
+    } else if (om)
+        PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_odom_predict_kernel, cdiv_u(d.n, 128), 128, 0, d, *om, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step);
+    const bool moved = proposed || om;
     for (size_t seg = 0; seg < nseg; ++seg) {
         const size_t j0 = cuts[seg], kk = cuts[seg + 1] - cuts[seg];
         // (ranks that share a GPU take turns on its SMs through the wait / signal launches: parked early CTAs of one rank could keep
         // another rank's persistent CTAs from ever being scheduled, so nothing is released early there)
-        const int flags = (seg == 0 ? 1 : 0) | (proposed ? 2 : 0) | (h->variant == 2 ? 4 : 0) | (h->early && h->pdl && !host_waits ? 8 : 0);
+        const int flags = (seg == 0 ? 1 : 0) | (moved ? 2 : 0) | (h->variant == 2 ? 4 : 0) | (h->early && h->pdl && !host_waits ? 8 : 0);
         memset(&po, 0, sizeof(po));
         for (size_t j = 0; j < kk; ++j) { po.o[j].d = z[j0 + j].d; po.o[j].angle = z[j0 + j].angle; po.o[j].lm_id = (int)z[j0 + j].lm_id; }
         int rc = kk <= 15 ? fs3_launch_ekf<512>(h, po, u, (int)kk, flags) : fs3_launch_ekf<1024>(h, po, u, (int)kk, flags);
@@ -505,6 +513,28 @@ extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs*
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     return fs_step_end(h, po, k_last, host_waits, did);
 }
+extern "C" int pfgpu_fs_step(pfgpu_fs* h, const double u[2], const pfgpu_fs_obs* z, size_t k, int* did) {
+    if (!h || !u || (k && !z)) return PFGPU_ERR_INVALID;
+    if (!finite_d(u[0]) || !finite_d(u[1])) return PFGPU_ERR_INVALID;
+    return fs_step_impl(h, u, nullptr, z, k, did);
+}
+extern "C" int pfgpu_fs_step_odom(pfgpu_fs* h, const double odom[6], const pfgpu_fs_obs* z, size_t k, int* did) {
+    if (!h || !odom || (k && !z)) return PFGPU_ERR_INVALID;
+    PfOdom om;
+    if (pf_odom_increment(odom, h->odom_alpha, &om) != 0) return PFGPU_ERR_INVALID;
+    const double u0[2] = { 0.0, 0.0 };            // unused: the EKF launch runs no motion model after the odometry move
+    return fs_step_impl(h, u0, &om, z, k, did);
+}
+extern "C" int pfgpu_fs_set_odom_noise(pfgpu_fs* h, const double alpha[4]) {
+    if (!h || !alpha || !pf_odom_alpha_ok(alpha)) return PFGPU_ERR_INVALID;
+    for (int j = 0; j < 4; ++j) h->odom_alpha[j] = alpha[j];
+    return 0;
+}
+extern "C" int pfgpu_fs_odom_noise(pfgpu_fs* h, double alpha[4]) {
+    if (!h || !alpha) return PFGPU_ERR_INVALID;
+    for (int j = 0; j < 4; ++j) alpha[j] = h->odom_alpha[j];
+    return 0;
+}
 // the association counters [8] (fs3_assoc.cuh), allocated and cleared on the handle's stream by the first call that needs them
 static int fs_acnt(pfgpu_fs* h) {
     if (h->acnt) return 0;
@@ -513,15 +543,8 @@ static int fs_acnt(pfgpu_fs* h) {
     return 0;
 }
 // FastSLAM 2.0 with unknown data association (DESIGN §3.5): fs3_assoc_kernel, the lazy-clone bookkeeping, then the post kernel
-extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const double* z2, size_t k, double gate_d2, int* did) {
-    if (!h || !u || (k && !z2)) return PFGPU_ERR_INVALID;
-    if (h->variant != 2) {
-        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "unknown data association needs FastSLAM 2.0 (pfgpu_fs_set_variant(h, 2)): FastSLAM 1.0 "
-                 "never initialises a fresh landmark's covariance, so a landmark it adds could never be matched");
-        return PFGPU_ERR_UNSUPPORTED;
-    }
-    if (!finite_d(u[0]) || !finite_d(u[1]) || !(gate_d2 > 0.0)) return PFGPU_ERR_INVALID;      // gate_d2 = +inf is allowed
-    for (size_t j = 0; j < 2 * k; ++j) if (!finite_d(z2[j])) return PFGPU_ERR_INVALID;
+// (om: the odometry increment in place of u, as in fs_step_impl; the caller has checked h, the variant and the motion)
+static int fs_step_unknown_impl(pfgpu_fs* h, const double u[2], const PfOdom* om, const double* z2, size_t k, double gate_d2, int* did) {
     PF_CUDA(cudaSetDevice(h->ctx.device));
     Fs3Dev& d = h->d;
     int rc = fs_acnt(h);
@@ -530,7 +553,7 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
     if (h->ex) { rc = fs_ex_param(h, &X); if (rc) return rc; }
     if (k == 0 && !h->ex) {  // no observation: the known-id step with k = 0, bit for bit; nothing was associated
         PF_CUDA(cudaMemsetAsync(h->acnt + 3, 0, 3 * sizeof(unsigned long long), h->ctx.stream));
-        return pfgpu_fs_step(h, u, nullptr, 0, did);
+        return fs_step_impl(h, u, om, nullptr, 0, did);
     }
     if (k && 2 * k > h->zcap) {  // (the previous step may still read the old list: wait for it before the buffer goes)
         PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
@@ -547,14 +570,41 @@ extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const doubl
     if (h->timer.on) { PF_CUDA(cudaEventCreate(&e0)); PF_CUDA(cudaEventCreate(&e1)); PF_CUDA(cudaEventRecord(e0, h->ctx.stream)); }
     // with existence counters (DESIGN §3.7), acnt[6] collects this step's removals
     if (h->ex) PF_CUDA(cudaMemsetAsync(h->acnt + 6, 0, sizeof(unsigned long long), h->ctx.stream));
-    PF_LAUNCH(h->ctx, (h->ex ? fs3_assoc_kernel<true> : fs3_assoc_kernel<false>), cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d,
-              (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1], h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step,
-              h->acnt, X, sqrt(h->cfg.q00), sqrt(h->cfg.q11), h->ex ? h->acnt + 6 : nullptr);
+    if (om)
+        PF_LAUNCH(h->ctx, (h->ex ? fs3_assoc_odom_kernel<true> : fs3_assoc_odom_kernel<false>), cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d,
+                  (const double*)h->zbuf, (int)k, gate_d2, *om, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step,
+                  h->acnt, X, h->ex ? h->acnt + 6 : nullptr);
+    else
+        PF_LAUNCH(h->ctx, (h->ex ? fs3_assoc_kernel<true> : fs3_assoc_kernel<false>), cdiv_u(d.ld, FS3_ASSOC_NT), FS3_ASSOC_NT, 0, d,
+                  (const double*)h->zbuf, (int)k, gate_d2, u[0], u[1], h->cfg.dt, h->cfg.r00, h->cfg.r11, h->seed, (uint32_t)h->n_step, (unsigned)h->n_step,
+                  h->acnt, X, sqrt(h->cfg.q00), sqrt(h->cfg.q11), h->ex ? h->acnt + 6 : nullptr);
     if (h->timer.on) { PF_CUDA(cudaEventRecord(e1, h->ctx.stream)); h->timer.pending.push_back({e0, e1}); }
     PF_LAUNCH_PDL(h->ctx, h->pdl, fs3_assoc_mark_kernel, std::max(1u, std::min(cdiv_u(d.m, 256), 64u)), 256, 0, d, h->acnt);
     Fs3ObsParam po;
     memset(&po, 0, sizeof(po));
     return fs_step_end(h, po, 0, host_waits, did);
+}
+static int fs_unknown_variant_ok(pfgpu_fs* h) {
+    if (h->variant == 2) return 1;
+    snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "unknown data association needs FastSLAM 2.0 (pfgpu_fs_set_variant(h, 2)): FastSLAM 1.0 "
+             "never initialises a fresh landmark's covariance, so a landmark it adds could never be matched");
+    return 0;
+}
+extern "C" int pfgpu_fs_step_unknown(pfgpu_fs* h, const double u[2], const double* z2, size_t k, double gate_d2, int* did) {
+    if (!h || !u || (k && !z2)) return PFGPU_ERR_INVALID;
+    if (!fs_unknown_variant_ok(h)) return PFGPU_ERR_UNSUPPORTED;
+    if (!finite_d(u[0]) || !finite_d(u[1]) || !(gate_d2 > 0.0)) return PFGPU_ERR_INVALID;      // gate_d2 = +inf is allowed
+    for (size_t j = 0; j < 2 * k; ++j) if (!finite_d(z2[j])) return PFGPU_ERR_INVALID;
+    return fs_step_unknown_impl(h, u, nullptr, z2, k, gate_d2, did);
+}
+extern "C" int pfgpu_fs_step_unknown_odom(pfgpu_fs* h, const double odom[6], const double* z2, size_t k, double gate_d2, int* did) {
+    if (!h || !odom || (k && !z2)) return PFGPU_ERR_INVALID;
+    if (!fs_unknown_variant_ok(h)) return PFGPU_ERR_UNSUPPORTED;
+    PfOdom om;
+    if (pf_odom_increment(odom, h->odom_alpha, &om) != 0 || !(gate_d2 > 0.0)) return PFGPU_ERR_INVALID;
+    for (size_t j = 0; j < 2 * k; ++j) if (!finite_d(z2[j])) return PFGPU_ERR_INVALID;
+    const double u0[2] = { 0.0, 0.0 };
+    return fs_step_unknown_impl(h, u0, &om, z2, k, gate_d2, did);
 }
 extern "C" int pfgpu_fs_assoc_counts(pfgpu_fs* h, uint64_t counts[3]) {
     if (!h || !counts) return PFGPU_ERR_INVALID;

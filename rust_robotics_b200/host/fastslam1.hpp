@@ -43,6 +43,23 @@ public:
         check(pfgpu_fs_step(h_, u.data(), o.data(), o.size(), &did), "fastslam_update");
         return did != 0;
     }
+    // the odometry motion model (no reference counterpart; DESIGN §3.15): ROS AMCL's odom_alpha1..4, each finite and >= 0 (0.2 each
+    // at creation)
+    void set_odometry_noise(const std::array<double, 4>& alpha) { check(pfgpu_fs_set_odom_noise(h_, alpha.data()), "set_odometry_noise"); }
+    std::array<double, 4> odometry_noise() const {
+        std::array<double, 4> a{};
+        check(pfgpu_fs_odom_noise(h_, a.data()), "odometry_noise");
+        return a;
+    }
+    // step with the odometry motion model: every particle moves by the increment from odometry pose prev = (x, y, yaw) to cur
+    bool step_odometry(const std::array<double, 3>& prev, const std::array<double, 3>& cur, const std::vector<Observation>& z) {
+        std::vector<pfgpu_fs_obs> o(z.size());
+        for (size_t i = 0; i < z.size(); ++i) { o[i].d = std::get<0>(z[i]); o[i].angle = std::get<1>(z[i]); o[i].lm_id = std::get<2>(z[i]); }
+        const std::array<double, 6> od = { prev[0], prev[1], prev[2], cur[0], cur[1], cur[2] };
+        int did = 0;
+        check(pfgpu_fs_step_odom(h_, od.data(), o.data(), o.size(), &did), "fastslam_update_odometry");
+        return did != 0;
+    }
     // get_best_particle fs1.rs:269-274 (pose + weight + that particle's landmarks, what render_gif_slam.rs:183-191 reads)
     Particle best() const {
         size_t idx = 0; double pw[4];
@@ -106,6 +123,8 @@ protected:
 inline FastSlam create_particles(size_t n_particles, size_t n_landmarks) = delete;   // engines are not copyable: construct FastSlam directly
 inline bool fastslam_update(FastSlam& particles, const std::array<double, 2>& u, const std::vector<Observation>& z) { return particles.step(u, z); }
 inline Particle get_best_particle(const FastSlam& particles) { return particles.best(); }
+inline bool fastslam_update_odometry(FastSlam& particles, const std::array<double, 3>& prev, const std::array<double, 3>& cur,
+                                     const std::vector<Observation>& z) { return particles.step_odometry(prev, cur, z); }
 
 }  // namespace fastslam1
 
@@ -121,6 +140,16 @@ struct FastSlam : fastslam1::FastSlam {
         for (size_t i = 0; i < z.size(); ++i) { z2[2 * i] = z[i].first; z2[2 * i + 1] = z[i].second; }
         int did = 0;
         check(pfgpu_fs_step_unknown(handle(), u.data(), z2.data(), z.size(), gate_d2, &did), "fastslam2_update_unknown");
+        return did != 0;
+    }
+    // update_unknown with the odometry motion model (DESIGN §3.15)
+    bool update_unknown_odometry(const std::array<double, 3>& prev, const std::array<double, 3>& cur,
+                                 const std::vector<std::pair<double, double>>& z, double gate_d2 = 16.0) {
+        std::vector<double> z2(2 * z.size());
+        for (size_t i = 0; i < z.size(); ++i) { z2[2 * i] = z[i].first; z2[2 * i + 1] = z[i].second; }
+        const std::array<double, 6> od = { prev[0], prev[1], prev[2], cur[0], cur[1], cur[2] };
+        int did = 0;
+        check(pfgpu_fs_step_unknown_odom(handle(), od.data(), z2.data(), z.size(), gate_d2, &did), "fastslam2_update_unknown_odometry");
         return did != 0;
     }
     // (matched, born, dropped) observations of the last update_unknown over all particles

@@ -219,6 +219,12 @@ extern "C" {
     // FastSLAM 2.0 with unknown data association (no reference counterpart in fastslam2; ekf_slam.rs:284-308's rule per particle)
     pub fn pfgpu_fs_step_unknown(h: *mut pfgpu_fs, u: *const f64, z2: *const f64, k: usize, gate_d2: f64, did_resample: *mut c_int) -> c_int;
     pub fn pfgpu_fs_assoc_counts(h: *mut pfgpu_fs, counts: *mut u64) -> c_int;
+    // FastSLAM's odometry motion model (no reference counterpart; DESIGN §3.15)
+    pub fn pfgpu_fs_set_odom_noise(h: *mut pfgpu_fs, alpha: *const f64) -> c_int;
+    pub fn pfgpu_fs_odom_noise(h: *mut pfgpu_fs, alpha: *mut f64) -> c_int;
+    pub fn pfgpu_fs_step_odom(h: *mut pfgpu_fs, odom: *const f64, z: *const pfgpu_fs_obs, k: usize, did_resample: *mut c_int) -> c_int;
+    pub fn pfgpu_fs_step_unknown_odom(h: *mut pfgpu_fs, odom: *const f64, z2: *const f64, k: usize, gate_d2: f64,
+                                      did_resample: *mut c_int) -> c_int;
     pub fn pfgpu_fs_last_neff(h: *mut pfgpu_fs, neff: *mut f64) -> c_int;
     pub fn pfgpu_fs_particle_landmarks(h: *mut pfgpu_fs, index_local: usize, lm6: *mut f64) -> c_int;
     pub fn pfgpu_fs_count(h: *mut pfgpu_fs, n_local: *mut usize, n_global: *mut usize, n_landmarks: *mut usize) -> c_int;

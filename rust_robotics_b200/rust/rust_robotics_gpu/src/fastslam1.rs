@@ -47,6 +47,27 @@ pub fn fastslam_update(particles: &mut FastSlam, u: Vector2<f64>, z: &[(f64, f64
     let rc = unsafe { sys::pfgpu_fs_step(particles.h, u.as_ptr(), obs.as_ptr(), obs.len(), std::ptr::null_mut()) };
     assert_eq!(rc, 0, "pfgpu_fs_step failed");       // lm_id out of range panics in the reference too (Vec index, fs1.rs:141)
 }
+/// The odometry motion model (not in fs1.rs; DESIGN §3.15): alpha = ROS AMCL's odom_alpha1..4, each finite and >= 0 (0.2 each at
+/// creation).  Panics on a refused value, as the other wrappers here do.
+pub fn set_odometry_noise(particles: &mut FastSlam, alpha: [f64; 4]) {
+    let rc = unsafe { sys::pfgpu_fs_set_odom_noise(particles.h, alpha.as_ptr()) };
+    assert_eq!(rc, 0, "pfgpu_fs_set_odom_noise failed");
+}
+/// (alpha1, alpha2, alpha3, alpha4)
+pub fn odometry_noise(particles: &FastSlam) -> [f64; 4] {
+    let mut a = [0.0f64; 4];
+    let rc = unsafe { sys::pfgpu_fs_odom_noise(particles.h, a.as_mut_ptr()) };
+    assert_eq!(rc, 0, "pfgpu_fs_odom_noise failed");
+    a
+}
+/// fastslam_update with the odometry motion model: every particle moves by the increment from odometry pose `prev` = (x, y, yaw)
+/// to `cur` instead of by a control over dt
+pub fn fastslam_update_odometry(particles: &mut FastSlam, prev: [f64; 3], cur: [f64; 3], z: &[(f64, f64, usize)]) {
+    let o = [prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]];
+    let obs: Vec<sys::pfgpu_fs_obs> = z.iter().map(|&(d, angle, id)| sys::pfgpu_fs_obs { d, angle, lm_id: id as u64 }).collect();
+    let rc = unsafe { sys::pfgpu_fs_step_odom(particles.h, o.as_ptr(), obs.as_ptr(), obs.len(), std::ptr::null_mut()) };
+    assert_eq!(rc, 0, "pfgpu_fs_step_odom failed");
+}
 /// get_best_particle fs1.rs:269-274
 pub fn get_best_particle(particles: &FastSlam) -> Particle {
     let (mut idx, mut pw) = (0usize, [0.0f64; 4]);

@@ -5,7 +5,7 @@
 use nalgebra::Vector2;
 use pfgpu_sys as sys;
 
-pub use crate::fastslam1::{get_best_particle, get_observations, Estimate, FastSlam, Landmark, Particle};
+pub use crate::fastslam1::{get_best_particle, get_observations, odometry_noise, set_odometry_noise, Estimate, FastSlam, Landmark, Particle};
 
 /// create_particles fs2.rs:418-422
 pub fn create_particles(n_particles: usize, n_landmarks: usize) -> FastSlam {
@@ -27,6 +27,18 @@ pub fn fastslam2_update_unknown(particles: &mut FastSlam, u: Vector2<f64>, z: &[
     let z2: Vec<f64> = z.iter().flat_map(|&(d, a)| [d, a]).collect();
     let rc = unsafe { sys::pfgpu_fs_step_unknown(particles.raw(), uu.as_ptr(), z2.as_ptr(), z.len(), 16.0, std::ptr::null_mut()) };
     assert_eq!(rc, 0, "pfgpu_fs_step_unknown failed");
+}
+/// fastslam2_update with the odometry motion model (DESIGN §3.15): the proposal fuses the first observation with the prior the
+/// odometry increment from `prev` to `cur` induces
+pub fn fastslam2_update_odometry(particles: &mut FastSlam, prev: [f64; 3], cur: [f64; 3], z: &[(f64, f64, usize)]) {
+    crate::fastslam1::fastslam_update_odometry(particles, prev, cur, z)      // the handle carries the variant
+}
+/// fastslam2_update_unknown with the odometry motion model
+pub fn fastslam2_update_unknown_odometry(particles: &mut FastSlam, prev: [f64; 3], cur: [f64; 3], z: &[(f64, f64)]) {
+    let o = [prev[0], prev[1], prev[2], cur[0], cur[1], cur[2]];
+    let z2: Vec<f64> = z.iter().flat_map(|&(d, a)| [d, a]).collect();
+    let rc = unsafe { sys::pfgpu_fs_step_unknown_odom(particles.raw(), o.as_ptr(), z2.as_ptr(), z.len(), 16.0, std::ptr::null_mut()) };
+    assert_eq!(rc, 0, "pfgpu_fs_step_unknown_odom failed");
 }
 /// (matched, born, dropped) observations of the last `fastslam2_update_unknown`, summed over the particles
 pub fn assoc_counts(particles: &FastSlam) -> [u64; 3] {

@@ -260,6 +260,38 @@ class ScanScenario:
 
 
 
+def drive_odometry(legs, start, dt, rng, trans_drift, rot_drift, rot_bias):
+    """The drive of a plan of (steps, v, yaw_rate) legs from `start` at `dt`, with wheel odometry in its own frame (starting at
+    (0, 0, 0)): each step's true body-frame increment (dx, dy, dtheta), with dx and dy scaled by 1 + N(0, trans_drift) and dtheta by
+    1 + N(0, rot_drift) plus N(0, rot_bias) (drawn from rng, nothing for a step that does not move), composed onto the previous
+    odometry pose.  Yields, per step, the true pose, the odometry pose and the (v, yaw_rate) that reproduces the odometry step over dt."""
+    t = list(start)
+    o = [0.0, 0.0, 0.0]
+    for n, v, w in legs:
+        for _ in range(n):
+            p = list(t)
+            t[0] += v * math.cos(t[2]) * dt
+            t[1] += v * math.sin(t[2]) * dt
+            t[2] += w * dt
+            c, s = math.cos(p[2]), math.sin(p[2])
+            gx, gy = t[0] - p[0], t[1] - p[1]
+            bx, by, bt = c * gx + s * gy, -s * gx + c * gy, t[2] - p[2]
+            if bx != 0.0 or by != 0.0 or bt != 0.0:
+                k = 1.0 + rng.normal(0.0, trans_drift)
+                bx, by = bx * k, by * k
+                bt = bt * (1.0 + rng.normal(0.0, rot_drift)) + rng.normal(0.0, rot_bias)
+            co, so = math.cos(o[2]), math.sin(o[2])
+            o = [o[0] + co * bx - so * by, o[1] + so * bx + co * by, o[2] + bt]
+            yield list(t), list(o), (math.copysign(math.hypot(bx, by), bx) / dt, bt / dt)
+
+
+def leg_phases(legs):
+    """{phase: (first step, end step)} of a drive, stop, turn, reverse, drive plan"""
+    ends = np.cumsum([n for n, _, _ in legs])
+    return {"drive": (0, ends[0]), "stop": (ends[0], ends[1]), "turn": (ends[1], ends[2]), "reverse": (ends[2], ends[3]),
+            "drive_again": (ends[3], ends[4])}
+
+
 class OdomScenario(ScanScenario):
     """ScanScenario's plan and laser with wheel odometry (the odometry motion model, DESIGN §3.14).  The robot starts at `start`
     and drives a plan of (steps, v, yaw_rate) legs at dt 0.1: drive, stop for several scans, turn in place, reverse, drive.
@@ -277,33 +309,47 @@ class OdomScenario(ScanScenario):
         self.start = tuple(start)
         self.region = self.REGION
         rng = np.random.default_rng(seed)
-        t = list(start)
-        o = [0.0, 0.0, 0.0]
-        self.truth, self.scans, self.odom, self.controls = [], [], [list(o)], []
-        for n, v, w in legs:
-            for _ in range(n):
-                p = list(t)
-                t[0] += v * math.cos(t[2]) * self.dt
-                t[1] += v * math.sin(t[2]) * self.dt
-                t[2] += w * self.dt
-                c, s = math.cos(p[2]), math.sin(p[2])
-                gx, gy = t[0] - p[0], t[1] - p[1]
-                bx, by, bt = c * gx + s * gy, -s * gx + c * gy, t[2] - p[2]
-                if bx != 0.0 or by != 0.0 or bt != 0.0:
-                    k = 1.0 + rng.normal(0.0, trans_drift)
-                    bx, by = bx * k, by * k
-                    bt = bt * (1.0 + rng.normal(0.0, rot_drift)) + rng.normal(0.0, rot_bias)
-                co, so = math.cos(o[2]), math.sin(o[2])
-                o = [o[0] + co * bx - so * by, o[1] + so * bx + co * by, o[2] + bt]
-                self.odom.append(list(o))
-                self.controls.append((math.copysign(math.hypot(bx, by), bx) / self.dt, bt / self.dt))
-                self.truth.append(list(t))
-                self.scans.append(np.ascontiguousarray(self._cast(base, t, rng, range_noise)))
+        self.truth, self.scans, self.odom, self.controls = [], [], [[0.0, 0.0, 0.0]], []
+        for t, o, u in drive_odometry(legs, start, self.dt, rng, trans_drift, rot_drift, rot_bias):
+            self.odom.append(o)
+            self.controls.append(u)
+            self.truth.append(t)
+            self.scans.append(np.ascontiguousarray(self._cast(base, t, rng, range_noise)))
         W, H = base.shape
         assert not any(base[int(math.floor(x / self.RES + W / 2.0)), int(math.floor(y / self.RES + H / 2.0))] for x, y, _ in self.truth)
-        ends = np.cumsum([n for n, _, _ in legs])
-        self.phases = {"drive": (0, ends[0]), "stop": (ends[0], ends[1]), "turn": (ends[1], ends[2]), "reverse": (ends[2], ends[3]),
-                       "drive_again": (ends[3], ends[4])}
+        self.phases = leg_phases(legs)
+
+    @property
+    def steps(self):
+        return len(self.truth)
+
+    def odom_pair(self, t):
+        """(previous, current) odometry pose of step t"""
+        return self.odom[t], self.odom[t + 1]
+
+
+class FsOdomScenario:
+    """FastSlamScenario's landmark world (a grid of landmarks 10 m apart, observed by get_observations within max_range) driven
+    by wheel odometry (FastSLAM's odometry motion model, DESIGN §3.15): a plan of (steps, v, yaw_rate) legs at dt 0.1 with a
+    stop, a turn in place and a reverse (drive_odometry: odometry with seeded drift, and the controls a caller of the velocity model
+    would derive from it).  truth[t] and obs[t] are the pose and the observations after step t; odom[0 .. steps] the odometry poses;
+    phases the step range of each leg."""
+    LEGS = ((30, 1.0, 0.05), (15, 0.0, 0.0), (15, 0.0, 1.0), (15, -0.5, 0.0), (25, 1.0, -0.05))
+
+    def __init__(self, side=8, start=(25.0, 25.0, 0.0), legs=LEGS, seed=21, max_range=20.0, trans_drift=0.02, rot_drift=0.05,
+                 rot_bias=0.002):
+        self.landmarks = grid_landmarks(side)
+        self.m = self.landmarks.shape[0]
+        self.start = list(start)
+        self.dt = 0.1
+        rng = np.random.default_rng(seed)
+        self.truth, self.obs, self.odom, self.controls = [], [], [[0.0, 0.0, 0.0]], []
+        for t, o, u in drive_odometry(legs, start, self.dt, rng, trans_drift, rot_drift, rot_bias):
+            self.odom.append(o)
+            self.controls.append(u)
+            self.truth.append(t)
+            self.obs.append(get_observations(t, self.landmarks, rng, max_range=max_range))
+        self.phases = leg_phases(legs)
 
     @property
     def steps(self):
