@@ -581,6 +581,9 @@ int  pfgpu_fs_post_trace(pfgpu_fs*, unsigned long long* out32);
 /* shape of the fused post-step kernel: tiles (one co-resident CTA each) x threads x values per thread, and whether the tiles
    live in shared memory (*global_tile = 0) or, for particle counts whose tile does not fit on chip, in global memory (1) */
 int  pfgpu_fs_post_shape(pfgpu_fs*, unsigned* tiles, unsigned* threads, unsigned* values_per_thread, int* global_tile);
+/* *k1 = 1 when the post-step kernel runs its instantiation for one value and at most one local slot per thread (512 threads,
+   shared-memory tiles; config 3 on one GPU), 0 when it runs the generic one (always, with PFGPU_POST_K1=0) */
+int  pfgpu_fs_post_k1(pfgpu_fs*, int* k1);
 /* how the coupled part of the step runs: 0 = one GPU, 2 = sharded over peer memory (NVLink loads / stores inside the kernels;
    no NCCL call and no host sync per step) */
 int  pfgpu_fs_shard_mode(pfgpu_fs*, int* mode);

@@ -115,7 +115,7 @@ EXPORTS = [
     "pfgpu_fs_get_observations", "pfgpu_fs_last_indices", "pfgpu_fs_last_neff", "pfgpu_fs_last_gate", "pfgpu_fs_set_variant", "pfgpu_fs_count", "pfgpu_fs_sync",
     "pfgpu_nccl_unique_id", "pfgpu_pf_stats", "pfgpu_fs_stats", "pfgpu_pf_time_main_kernel",
     "pfgpu_fs_time_main_kernel", "pfgpu_pf_mark", "pfgpu_pf_elapsed_ms", "pfgpu_fs_mark", "pfgpu_fs_elapsed_ms",
-    "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_shard_mode",
+    "pfgpu_pf_flush_l2", "pfgpu_fs_flush_l2", "pfgpu_fs_post_trace", "pfgpu_fs_post_shape", "pfgpu_fs_post_k1", "pfgpu_fs_shard_mode",
     "pfgpu_fs_moments", "pfgpu_fs_estimate_merge", "pfgpu_fs_step_unknown", "pfgpu_fs_assoc_counts",
     "pfgpu_fs_set_odom_noise", "pfgpu_fs_odom_noise", "pfgpu_fs_step_odom", "pfgpu_fs_step_unknown_odom",
     "pfgpu_fs_history_enable", "pfgpu_fs_history_window", "pfgpu_fs_path", "pfgpu_fs_path_moments",
@@ -245,6 +245,7 @@ def load_library():
         getattr(L, f"pfgpu_{k}_flush_l2").argtypes = [vp]
     L.pfgpu_fs_post_trace.argtypes = [vp, C.POINTER(C.c_ulonglong)]
     L.pfgpu_fs_post_shape.argtypes = [vp, C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_int)]
+    L.pfgpu_fs_post_k1.argtypes = [vp, C.POINTER(C.c_int)]
     L.pfgpu_fs_shard_mode.argtypes = [vp, C.POINTER(C.c_int)]
     L.pfgpu_fs_moments.argtypes = [vp, C.c_double, C.POINTER(_FsPoseMoments), c_dp]
     L.pfgpu_fs_estimate_merge.argtypes = [C.POINTER(_FsPoseMoments), C.POINTER(c_dp), C.c_int, C.c_size_t, c_dp, c_dp, c_dp, c_dp, c_dp]
@@ -1190,6 +1191,13 @@ class FastSlam1:
         t, nt, k, gl = C.c_uint(), C.c_uint(), C.c_uint(), C.c_int()
         _check(self.L, self.L.pfgpu_fs_post_shape(self.h, C.byref(t), C.byref(nt), C.byref(k), C.byref(gl)))
         return t.value, nt.value, k.value, "global" if gl.value else "shared"
+
+    def post_k1(self):
+        """True when the post-step kernel runs its instantiation for one value and at most one local slot per thread (config 3
+        on one GPU; PFGPU_POST_K1=0 at creation forces the generic kernel)."""
+        k1 = C.c_int()
+        _check(self.L, self.L.pfgpu_fs_post_k1(self.h, C.byref(k1)))
+        return bool(k1.value)
 
     # -- estimate (no reference counterpart: fs1.rs's callers read the best particle's map, keeping landmarks with cov00 < 100) --
     def moments(self, cov00_max=100.0, landmarks=True):

@@ -49,6 +49,7 @@
 #define FS3_SPIN_LIMIT (1u << 27)
 #define FS3_MAX_LM 65536          // landmarks per particle: row ids (< m) fit the u16 row list
 #define FS3_ROW_CHUNK 1024        // live rows a post-kernel CTA lists in shared memory at a time (more: several passes)
+#define FS3_K1_ROWS 8             // live rows whose gathers the one-value post kernel (KC = 1) keeps in flight per batch
 #define FS3_CERT_MAX_LOG2N 16     // certified CDF up to 2^16 particles: about 4 n^3 2^-53 comb values fall within its bound of a
                                   // CDF value, 1/8 at 2^16, 1 at 2^17, 64 at 2^19 (where it would almost always be refused)
 
@@ -614,8 +615,10 @@ __device__ __forceinline__ void fs3_grid_sync(const Fs3Sum& x, int round, unsign
     __syncthreads();
 }
 
+// The loops over the block's NT / 32 warp totals below run rolled (little code) or, with KC = 1 (the post kernel's config-3
+// instantiation, whose step path is short), unrolled with every shared-memory load in flight: the same adds in the same order.
 // exclusive prefix over the block's threads (thread order) of a double, ONE block barrier (sm: this round's scratch)
-template <int NT>
+template <int NT, int KC = 0>
 __device__ __forceinline__ double fs3_scan_d(double x, double* sm) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     double inc = x;
@@ -626,12 +629,17 @@ __device__ __forceinline__ double fs3_scan_d(double x, double* sm) {
     if (lane == 31) sm[wid] = inc;
     __syncthreads();
     double woff = 0.0;
+    if constexpr (KC == 1) {
+#pragma unroll
+        for (int w = 0; w < NT / 32 - 1; ++w) if (w < wid) woff += sm[w];
+    } else {
 #pragma unroll 1
-    for (int w = 0; w < wid; ++w) woff += sm[w];
+        for (int w = 0; w < wid; ++w) woff += sm[w];
+    }
     return woff + ex;
 }
 // the same for a (u64 increment sum, int count) pair; also returns the block totals
-template <int NT>
+template <int NT, int KC = 0>
 __device__ __forceinline__ void fs3_scan_ui(unsigned long long p, int c, unsigned long long* pex, int* cex, unsigned long long* ptot, int* ctot,
                                             unsigned long long* smu, int* smi) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -644,8 +652,13 @@ __device__ __forceinline__ void fs3_scan_ui(unsigned long long p, int c, unsigne
     if (lane == 31) { smu[wid] = ip; smi[wid] = ic; }
     __syncthreads();
     unsigned long long wp = 0, tp = 0; int wc = 0, tc = 0;
+    if constexpr (KC == 1) {
+#pragma unroll
+        for (int w = 0; w < NT / 32; ++w) { const unsigned long long a = smu[w]; const int b = smi[w]; if (w < wid) { wp += a; wc += b; } tp += a; tc += b; }
+    } else {
 #pragma unroll 1
-    for (int w = 0; w < NT / 32; ++w) { const unsigned long long a = smu[w]; const int b = smi[w]; if (w < wid) { wp += a; wc += b; } tp += a; tc += b; }
+        for (int w = 0; w < NT / 32; ++w) { const unsigned long long a = smu[w]; const int b = smi[w]; if (w < wid) { wp += a; wc += b; } tp += a; tc += b; }
+    }
     *pex = wp + ip - p; *cex = wc + ic - c; *ptot = tp; *ctot = tc;
 }
 __device__ __forceinline__ double fs3_warp_sum(double v) {
@@ -654,15 +667,20 @@ __device__ __forceinline__ double fs3_warp_sum(double v) {
     return v;
 }
 // block sums of two doubles at once (tree order, identical in every CTA; valid in all threads); ONE block barrier
-template <int NT>
+template <int NT, int KC = 0>
 __device__ __forceinline__ void fs3_block_sum2(double& x, double& y, double* smx, double* smy) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     x = fs3_warp_sum(x); y = fs3_warp_sum(y);
     if (lane == 0) { smx[wid] = x; smy[wid] = y; }
     __syncthreads();
     double a = 0.0, b = 0.0;
+    if constexpr (KC == 1) {
+#pragma unroll
+        for (int w = 0; w < NT / 32; ++w) { a += smx[w]; b += smy[w]; }
+    } else {
 #pragma unroll 1
-    for (int w = 0; w < NT / 32; ++w) { a += smx[w]; b += smy[w]; }
+        for (int w = 0; w < NT / 32; ++w) { a += smx[w]; b += smy[w]; }
+    }
     x = a; y = b;
 }
 
@@ -783,7 +801,7 @@ __device__ __forceinline__ void fs3_row_scan(const Fs3Dev& d, const Fs3ObsParam&
 // fs3_row_count: *pos = the position of the thread's first live row in that order, *nrows = how many rows are live, *newrow = the
 // row the identity landmarks get (the first free id: with an identity landmark at most m - 1 rows are live) or -1 when there is
 // none.  Contains one block barrier.
-template <int NT>
+template <int NT, int KC = 0>
 __device__ __forceinline__ void fs3_row_count(const Fs3Dev& d, Fs3Sh<NT>& sh, int par, unsigned nt, unsigned* pos, int* nrows, int* newrow) {
     const unsigned tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
     const unsigned W = fs3_bm_words(d.m);
@@ -811,8 +829,13 @@ __device__ __forceinline__ void fs3_row_count(const Fs3Dev& d, Fs3Sh<NT>& sh, in
     if (wid == 0) { any = __any_sync(0xffffffffu, any); if (lane == 0) sh.rany = any; }
     __syncthreads();
     unsigned p = (unsigned)(incl - cnt), tot = 0, mf = 0xFFFFFFFFu;
+    if constexpr (KC == 1) {
+#pragma unroll
+        for (unsigned v = 0; v < NT / 32; ++v) { const unsigned c = sh.rowscan[0][v]; if (v < wid) p += c; tot += c; mf = min(mf, sh.rowscan[1][v]); }
+    } else {
 #pragma unroll 1
-    for (unsigned v = 0; v < NT / 32; ++v) { const unsigned c = sh.rowscan[0][v]; if (v < wid) p += c; tot += c; mf = min(mf, sh.rowscan[1][v]); }
+        for (unsigned v = 0; v < NT / 32; ++v) { const unsigned c = sh.rowscan[0][v]; if (v < wid) p += c; tot += c; mf = min(mf, sh.rowscan[1][v]); }
+    }
     *pos = p; *nrows = (int)tot; *newrow = sh.rany ? (int)mf : -1;
 }
 // the live rows at positions [base, base + FS3_ROW_CHUNK) of the ascending order into sh.rowl (pos from fs3_row_count); the caller
@@ -881,7 +904,7 @@ __device__ __noinline__ double fs3_chain_wide(const Fs3Sum& x, Fs3Sh<NT>& sh, si
 // sh.fail = 1 the serial walk has already stored them to `out`).  Contains ONE grid barrier (`round`).
 // fs3_xsum_body is the sum inlined where it is on every step's path (the post kernel's S sum); fs3_xsum is its one out-of-line
 // copy for every other sum.
-template <int NT, bool GT = false>
+template <int NT, bool GT = false, int KC = 0>
 __device__ __forceinline__ double fs3_xsum_body(const Fs3Sum& x, Fs3Sh<NT>& sh, const double* vals, unsigned K, unsigned nt, double toff, int slot, int round,
                                                 unsigned m32, double* out, int par, double S2, double r0, double inv, double extraQ, int pub, Fs3Run* run,
                                                 const Fs3Hook* hook) {
@@ -896,7 +919,7 @@ __device__ __forceinline__ double fs3_xsum_body(const Fs3Sum& x, Fs3Sh<NT>& sh, 
 #pragma unroll 1
     for (unsigned k = 0; k < K; ++k) { const double v = vals[k * NT + tid]; ts += v; if (!(v >= 0.0) || !(v <= 1.7976931348623157e308)) bad = true; }
     if (slot == FS3_S) FS3_TRACE(28);
-    const double a_first = toff + fs3_scan_d<NT>(ts, sh.wd[pp]);
+    const double a_first = toff + fs3_scan_d<NT, KC>(ts, sh.wd[pp]);
     if (slot == FS3_S) FS3_TRACE(29);
     unsigned long long P = 0; int nd = 0;
     // Almost every thread's K prefixes stay inside one binade, clear of its edges: then each value is classified at that binade
@@ -921,7 +944,7 @@ __device__ __forceinline__ double fs3_xsum_body(const Fs3Sum& x, Fs3Sh<NT>& sh, 
     }
     if (slot == FS3_S) FS3_TRACE(30);
     unsigned long long Pex, Ptile; int dex, ndtile;
-    fs3_scan_ui<NT>(P, nd, &Pex, &dex, &Ptile, &ndtile, sh.wu[pp], sh.wi[pp]);
+    fs3_scan_ui<NT, KC>(P, nd, &Pex, &dex, &Ptile, &ndtile, sh.wu[pp], sh.wi[pp]);
     if (nd > 0) {                                              // rare: itemise this thread's dirty values (any order; sorted by the chain)
         const unsigned e0 = atomicAdd(x.entCnt + slot, (unsigned)nd);
         double a = a_first; unsigned long long Pr = Pex; unsigned e = e0;
@@ -1184,16 +1207,25 @@ __device__ __forceinline__ unsigned fs3_cdf_search(const double* cdf, const doub
 // ([tiles][K][NT] doubles of global memory, the same layout: every access stays coalesced), for particle counts whose tile does not
 // fit on chip.  A value stored by one thread is read by another only behind a __syncthreads(), which orders global memory inside
 // a CTA too.
+// The block workspace, one variable for fs3_post_kernel<NT, GTILE, 0> and <NT, GTILE, 1>: the out-of-line routines they share
+// (template tag GTILE) then address it directly, as when only one kernel called them, instead of taking it as an argument.
 template <int NT, bool GTILE>
+__shared__ Fs3Sh<NT> fs3_post_sh;
+// KC = 0: K values per thread, K taken at run time.  KC = 1: one value per thread and at most one local slot per thread (config 3:
+// 128 tiles x 512 threads x 1), so the loops over a thread's values fold away in the inlined hot-path bodies (the argument K is
+// ignored), and the clone phase handles one slot per thread.  The out-of-line rare paths are shared with <NT, GTILE, 0>.
+template <int NT, bool GTILE, int KC = 0>
 __global__ void __launch_bounds__(NT, 1)
 fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3ObsParam po, int k_last, double nth, uint64_t seed, unsigned step,
-                unsigned K, unsigned m32, int log2n, int early_launch, double* vtile) {
+                unsigned K_rt, unsigned m32, int log2n, int early_launch, double* vtile) {
+    static_assert(KC == 0 || (KC == 1 && !GTILE), "the one-value kernel keeps its tile in shared memory");
+    const unsigned K = KC ? (unsigned)KC : K_rt;
     pf_grid_dep_sync();
     if (early_launch) pf_grid_launch_dependents();
     double* vt;
     { extern __shared__ __align__(16) double vals[]; vt = GTILE ? vtile + (size_t)blockIdx.x * NT * K : vals; }
     double* const vals = vt;                                  // [K][NT]
-    __shared__ Fs3Sh<NT> sh;
+    Fs3Sh<NT>& sh = fs3_post_sh<NT, GTILE>;
     const Fs3Sum& x = d.x;
     Fs3State* st = d.st;
     const int tid = threadIdx.x;
@@ -1225,7 +1257,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
 #pragma unroll 8
         for (unsigned p = tid; p < pfirst; p += NT) toff += __ldcg(d.part[par] + p);
     }
-    fs3_block_sum2<NT>(toff, q, sh.red[0], sh.red[1]);
+    fs3_block_sum2<NT, KC>(toff, q, sh.red[0], sh.red[1]);
     FS3_TRACE(0);
     // the comb of a resample this step might need: r = Uniform::new(0, 1/n).sample(rng) (fs1.rs:219-220), one draw per resample, and
     // (n a power of two) its closed-form table, built by an otherwise idle warp inside the first exact sum
@@ -1238,7 +1270,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     Fs3Hook hook;
     hook.comb_n = log2n >= 0 ? (unsigned long long)ng : 0ull; hook.seed = seed; hook.step = step; hook.k_last = k_last; hook.po = &po;
     Fs3Run run;
-    const double S = fs3_xsum_body<NT, GTILE>(x, sh, vals, K, nt, toff, FS3_S, FS3_R_S, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
+    const double S = fs3_xsum_body<NT, GTILE, KC>(x, sh, vals, K, nt, toff, FS3_S, FS3_R_S, m32, nullptr, par, 0.0, r0, inv, q, cert_pub, &run, &hook);
     const int S_walked = sh.fail;
     FS3_TRACE(1);
     // ---------------- gate: neff = 1 / sum w^2 < NTH (compute_neff fs1.rs:186-193, fs1.rs:262-263) ----------------
@@ -1246,7 +1278,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     // aggregates of S: sum (w_raw_i / S)^2 differs from the reference's sequential sum of fl(w_raw_i / S)^2 by at most
     // (n + 64) 2^-51 relatively; only when neff lands that close to NTH is the exact sequential sum walked (below, once wn_all is written).
     double Q = (unsigned)tid < nt ? __ldcg(x.tileQ + tid) : 0.0, dummy = 0.0;
-    fs3_block_sum2<NT>(Q, dummy, sh.red[1], sh.wd[1]);
+    fs3_block_sum2<NT, KC>(Q, dummy, sh.red[1], sh.wd[1]);
     if (S > 0.0) Q = Q / S / S;
     double neff = Q > 0.0 ? 1.0 / Q : 0.0;
     const double slack = 16.0 * (double)(ng + 64) * 2.220446049250313e-16;
@@ -1293,8 +1325,13 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     if ((tid & 31) == 0) { sh.red[0][tid >> 5] = bw; sh.wi[0][tid >> 5] = (int)bi; }
     __syncthreads();
     if (tid == 0) {
+        if constexpr (KC == 1) {
+#pragma unroll
+            for (int w = 1; w < NT / 32; ++w) { const double ow = sh.red[0][w]; const unsigned oi = (unsigned)sh.wi[0][w]; if (ow > bw || (ow == bw && oi > bi)) { bw = ow; bi = oi; } }
+        } else {
 #pragma unroll 1
-        for (int w = 1; w < NT / 32; ++w) { const double ow = sh.red[0][w]; const unsigned oi = (unsigned)sh.wi[0][w]; if (ow > bw || (ow == bw && oi > bi)) { bw = ow; bi = oi; } }
+            for (int w = 1; w < NT / 32; ++w) { const double ow = sh.red[0][w]; const unsigned oi = (unsigned)sh.wi[0][w]; if (ow > bw || (ow == bw && oi > bi)) { bw = ow; bi = oi; } }
+        }
         d.tileBw[b] = bw; d.tileBi[b] = bi;
     }
     if (border) {                                              // rare
@@ -1379,7 +1416,7 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
         for (unsigned t = tid; t < nt; t += NT) sh.tend[t] = __ldcg(x.tileEnd + t);
         // the live rows: every CTA's fs3_row_scan (inside the S sum) is ordered before the grid barrier this CTA has just passed
         unsigned rpos; int nrows, newrow;
-        fs3_row_count<NT>(d, sh, par, nt, &rpos, &nrows, &newrow);            // (also orders the tileEnd copy)
+        fs3_row_count<NT, KC>(d, sh, par, nt, &rpos, &nrows, &newrow);            // (also orders the tileEnd copy)
         if (t_lo < t_hi) {
             if (tid < 64) {
                 const size_t te = (size_t)d.off + (tid < 32 ? t_lo : t_hi - 1);
@@ -1402,90 +1439,144 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
             __syncthreads();
             FS3_TRACE(23);
             unsigned* drows = d.rows[rcur ^ 1];
-            // rows in chunks of FS3_ROW_CHUNK (one chunk but for very large maps); the first chunk's pass also searches the slots and
-            // clones the poses, later passes take the ancestors from idx (this thread's own stores)
+            if constexpr (KC == 1) {
+                // one slot per thread (per <= NT): its search, pose clone and row composition.  The ancestor stays in registers
+                // across the row chunks, and the registers the generic kernel spends on four slots hold FS3_K1_ROWS rows of one.
+                const unsigned t = t_lo + (unsigned)tid;
+                const bool mine = t < t_hi;
+                unsigned j = 0;
+                if (mine) {
+                    const size_t tg = (size_t)d.off + t;
+                    const double r = log2n >= 0 ? x3_comb_eval(&sh.comb, inv, tg) : __ldcg(d.rcomb_all + tg);
+                    unsigned lo = 0, hi = len;
+                    if (staged) {
 #pragma unroll 1
-            for (unsigned rbase = 0; ; rbase += FS3_ROW_CHUNK) {
-                const int nr = min(nrows - (int)rbase, FS3_ROW_CHUNK);
-                // four slots per thread and trip: their searches, pose gathers and row gathers are independent, so the dependent memory
-                // round trips (index -> ancestor's pose -> ancestor's row entries) overlap four-fold
-#pragma unroll 1
-                for (unsigned t0 = t_lo + tid; t0 < t_hi; t0 += 4 * NT) {
-                    unsigned jj[4]; int jrk[4]; unsigned jcol[4];
-                    if (rbase == 0) {
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const unsigned t = t0 + (unsigned)u * NT;
-                            jj[u] = 0; jrk[u] = 0; jcol[u] = 0;
-                            if (t < t_hi) {
-                                const size_t tg = (size_t)d.off + t;
-                                const double r = log2n >= 0 ? x3_comb_eval(&sh.comb, inv, tg) : __ldcg(d.rcomb_all + tg);
-                                unsigned lo = 0, hi = len;
-                                if (staged) {
-#pragma unroll 1
-                                    while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (vals[mid] < r) lo = mid + 1; else hi = mid; }
-                                } else {
-#pragma unroll 1
-                                    while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (__ldcg(cdf + jlo + mid) < r) lo = mid + 1; else hi = mid; }
-                                }
-                                unsigned j = jlo + lo;
-                                if (j >= ng) j = (unsigned)ng - 1;
-                                jj[u] = j; jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;              // owner rank and column of the ancestor
-                            }
-                        }
-                        double gx[4], gy[4], ga[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const double* sx = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_px[cur]) : d.px[cur];
-                            const double* sy = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_py[cur]) : d.py[cur];
-                            const double* sa = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_pyaw[cur]) : d.pyaw[cur];
-                            gx[u] = sx[jcol[u]]; gy[u] = sy[jcol[u]]; ga[u] = sa[jcol[u]];
-                        }
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const unsigned t = t0 + (unsigned)u * NT;
-                            if (t < t_hi) {
-                                d.idx[t] = jj[u];
-                                d.px[cur ^ 1][t] = gx[u]; d.py[cur ^ 1][t] = gy[u]; d.pyaw[cur ^ 1][t] = ga[u];     // particles[j].clone() fs1.rs:227
-                                d.w[t] = inv;                                                            // fs1.rs:228
-                                if (newrow >= 0) drows[(size_t)newrow * d.ld + t] = fs3_ref(jrk[u], jcol[u]);
-                            }
-                        }
+                        while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (vals[mid] < r) lo = mid + 1; else hi = mid; }
                     } else {
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const unsigned t = t0 + (unsigned)u * NT;
-                            const unsigned j = t < t_hi ? d.idx[t] : 0u;
-                            jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;
-                        }
-                    }
-                    // the ancestors' row entries: eight rows x four slots of independent gathers in flight per batch (the rows were
-                    // written a resample ago; one dependent HBM round trip per batch instead of per row)
-                    const unsigned* srow[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u)
-                        srow[u] = (d.G > 1 ? reinterpret_cast<const unsigned*>(d.peer[jrk[u]] + d.o_rows[rcur]) : d.rows[rcur]) + jcol[u];
 #pragma unroll 1
-                    for (int x0 = 0; x0 < nr; x0 += 8) {
-                        unsigned e[8][4];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const size_t ro = (size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld;
-#pragma unroll
-                            for (int u = 0; u < 4; ++u) e[i][u] = (x0 + i < nr && t0 + (unsigned)u * NT < t_hi) ? srow[u][ro] : 0u;
-                        }
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const size_t ro = (size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld;
-#pragma unroll
-                            for (int u = 0; u < 4; ++u) { const unsigned t = t0 + (unsigned)u * NT; if (x0 + i < nr && t < t_hi) drows[ro + t] = e[i][u]; }
-                        }
+                        while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (__ldcg(cdf + jlo + mid) < r) lo = mid + 1; else hi = mid; }
+                    }
+                    j = jlo + lo;
+                    if (j >= ng) j = (unsigned)ng - 1;
+                }
+                const int jrk = (int)(j / d.n); const unsigned jcol = j % d.n;              // owner rank and column of the ancestor
+                {
+                    const double* sx = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk] + d.o_px[cur]) : d.px[cur];
+                    const double* sy = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk] + d.o_py[cur]) : d.py[cur];
+                    const double* sa = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk] + d.o_pyaw[cur]) : d.pyaw[cur];
+                    const double gx = sx[jcol], gy = sy[jcol], ga = sa[jcol];
+                    if (mine) {
+                        d.idx[t] = j;
+                        d.px[cur ^ 1][t] = gx; d.py[cur ^ 1][t] = gy; d.pyaw[cur ^ 1][t] = ga;     // particles[j].clone() fs1.rs:227
+                        d.w[t] = inv;                                                            // fs1.rs:228
+                        if (newrow >= 0) drows[(size_t)newrow * d.ld + t] = fs3_ref(jrk, jcol);
                     }
                 }
-                if ((int)(rbase + FS3_ROW_CHUNK) >= nrows) break;
-                __syncthreads();                               // everybody is through this chunk's rows
-                fs3_row_fill<NT>(d, sh, par, rbase + FS3_ROW_CHUNK, rpos);
-                __syncthreads();
+                const unsigned* srow = (d.G > 1 ? reinterpret_cast<const unsigned*>(d.peer[jrk] + d.o_rows[rcur]) : d.rows[rcur]) + jcol;
+#pragma unroll 1
+                for (unsigned rbase = 0; ; rbase += FS3_ROW_CHUNK) {
+                    const int nr = min(nrows - (int)rbase, FS3_ROW_CHUNK);
+                    if (mine) {
+#pragma unroll 1
+                        for (int x0 = 0; x0 < nr; x0 += FS3_K1_ROWS) {
+                            unsigned e[FS3_K1_ROWS];
+#pragma unroll
+                            for (int i = 0; i < FS3_K1_ROWS; ++i) e[i] = x0 + i < nr ? srow[(size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld] : 0u;
+#pragma unroll
+                            for (int i = 0; i < FS3_K1_ROWS; ++i) if (x0 + i < nr) drows[(size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld + t] = e[i];
+                        }
+                    }
+                    if ((int)(rbase + FS3_ROW_CHUNK) >= nrows) break;
+                    __syncthreads();                           // everybody is through this chunk's rows
+                    fs3_row_fill<NT>(d, sh, par, rbase + FS3_ROW_CHUNK, rpos);
+                    __syncthreads();
+                }
+            } else {
+                // rows in chunks of FS3_ROW_CHUNK (one chunk but for very large maps); the first chunk's pass also searches the slots and
+                // clones the poses, later passes take the ancestors from idx (this thread's own stores)
+#pragma unroll 1
+                for (unsigned rbase = 0; ; rbase += FS3_ROW_CHUNK) {
+                    const int nr = min(nrows - (int)rbase, FS3_ROW_CHUNK);
+                    // four slots per thread and trip: their searches, pose gathers and row gathers are independent, so the dependent memory
+                    // round trips (index -> ancestor's pose -> ancestor's row entries) overlap four-fold
+#pragma unroll 1
+                    for (unsigned t0 = t_lo + tid; t0 < t_hi; t0 += 4 * NT) {
+                        unsigned jj[4]; int jrk[4]; unsigned jcol[4];
+                        if (rbase == 0) {
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                const unsigned t = t0 + (unsigned)u * NT;
+                                jj[u] = 0; jrk[u] = 0; jcol[u] = 0;
+                                if (t < t_hi) {
+                                    const size_t tg = (size_t)d.off + t;
+                                    const double r = log2n >= 0 ? x3_comb_eval(&sh.comb, inv, tg) : __ldcg(d.rcomb_all + tg);
+                                    unsigned lo = 0, hi = len;
+                                    if (staged) {
+#pragma unroll 1
+                                        while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (vals[mid] < r) lo = mid + 1; else hi = mid; }
+                                    } else {
+#pragma unroll 1
+                                        while (lo < hi) { const unsigned mid = (lo + hi) >> 1; if (__ldcg(cdf + jlo + mid) < r) lo = mid + 1; else hi = mid; }
+                                    }
+                                    unsigned j = jlo + lo;
+                                    if (j >= ng) j = (unsigned)ng - 1;
+                                    jj[u] = j; jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;              // owner rank and column of the ancestor
+                                }
+                            }
+                            double gx[4], gy[4], ga[4];
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                const double* sx = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_px[cur]) : d.px[cur];
+                                const double* sy = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_py[cur]) : d.py[cur];
+                                const double* sa = d.G > 1 ? reinterpret_cast<const double*>(d.peer[jrk[u]] + d.o_pyaw[cur]) : d.pyaw[cur];
+                                gx[u] = sx[jcol[u]]; gy[u] = sy[jcol[u]]; ga[u] = sa[jcol[u]];
+                            }
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                const unsigned t = t0 + (unsigned)u * NT;
+                                if (t < t_hi) {
+                                    d.idx[t] = jj[u];
+                                    d.px[cur ^ 1][t] = gx[u]; d.py[cur ^ 1][t] = gy[u]; d.pyaw[cur ^ 1][t] = ga[u];     // particles[j].clone() fs1.rs:227
+                                    d.w[t] = inv;                                                            // fs1.rs:228
+                                    if (newrow >= 0) drows[(size_t)newrow * d.ld + t] = fs3_ref(jrk[u], jcol[u]);
+                                }
+                            }
+                        } else {
+#pragma unroll
+                            for (int u = 0; u < 4; ++u) {
+                                const unsigned t = t0 + (unsigned)u * NT;
+                                const unsigned j = t < t_hi ? d.idx[t] : 0u;
+                                jrk[u] = (int)(j / d.n); jcol[u] = j % d.n;
+                            }
+                        }
+                        // the ancestors' row entries: eight rows x four slots of independent gathers in flight per batch (the rows were
+                        // written a resample ago; one dependent HBM round trip per batch instead of per row)
+                        const unsigned* srow[4];
+#pragma unroll
+                        for (int u = 0; u < 4; ++u)
+                            srow[u] = (d.G > 1 ? reinterpret_cast<const unsigned*>(d.peer[jrk[u]] + d.o_rows[rcur]) : d.rows[rcur]) + jcol[u];
+#pragma unroll 1
+                        for (int x0 = 0; x0 < nr; x0 += 8) {
+                            unsigned e[8][4];
+#pragma unroll
+                            for (int i = 0; i < 8; ++i) {
+                                const size_t ro = (size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld;
+#pragma unroll
+                                for (int u = 0; u < 4; ++u) e[i][u] = (x0 + i < nr && t0 + (unsigned)u * NT < t_hi) ? srow[u][ro] : 0u;
+                            }
+#pragma unroll
+                            for (int i = 0; i < 8; ++i) {
+                                const size_t ro = (size_t)sh.rowl[min(x0 + i, nr - 1)] * d.ld;
+#pragma unroll
+                                for (int u = 0; u < 4; ++u) { const unsigned t = t0 + (unsigned)u * NT; if (x0 + i < nr && t < t_hi) drows[ro + t] = e[i][u]; }
+                            }
+                        }
+                    }
+                    if ((int)(rbase + FS3_ROW_CHUNK) >= nrows) break;
+                    __syncthreads();                               // everybody is through this chunk's rows
+                    fs3_row_fill<NT>(d, sh, par, rbase + FS3_ROW_CHUNK, rpos);
+                    __syncthreads();
+                }
             }
         }
         if (newrow >= 0) {     // the identity landmarks of this CTA's slice now read through the new row (every scan of lmst is over)
@@ -1509,8 +1600,20 @@ fs3_post_kernel(const __grid_constant__ Fs3Dev d, const __grid_constant__ Fs3Obs
     if (tid < 32) {
         // best particle: the last maximum over the tiles (no resample) / the last slot (after a resample every weight is 1/n)
         double bw2 = -INFINITY; unsigned bi2 = 0;
+        if constexpr (KC == 1) {                               // every tile's best in flight at once, then the same comparisons in order
+            double ow[(FS3_MAX_TILES + 31) / 32]; unsigned oi[(FS3_MAX_TILES + 31) / 32];
+#pragma unroll
+            for (unsigned i = 0; i < (FS3_MAX_TILES + 31) / 32; ++i) {
+                const unsigned u = tid + 32u * i;
+                ow[i] = u < nt ? __ldcg(d.tileBw + u) : 0.0; oi[i] = u < nt ? __ldcg(d.tileBi + u) : 0u;
+            }
+#pragma unroll
+            for (unsigned i = 0; i < (FS3_MAX_TILES + 31) / 32; ++i)
+                if (tid + 32u * i < nt && (ow[i] > bw2 || (ow[i] == bw2 && oi[i] > bi2))) { bw2 = ow[i]; bi2 = oi[i]; }
+        } else {
 #pragma unroll 1
-        for (unsigned u = tid; u < nt; u += 32) { const double ow = __ldcg(d.tileBw + u); const unsigned oi = __ldcg(d.tileBi + u); if (ow > bw2 || (ow == bw2 && oi > bi2)) { bw2 = ow; bi2 = oi; } }
+            for (unsigned u = tid; u < nt; u += 32) { const double ow = __ldcg(d.tileBw + u); const unsigned oi = __ldcg(d.tileBi + u); if (ow > bw2 || (ow == bw2 && oi > bi2)) { bw2 = ow; bi2 = oi; } }
+        }
 #pragma unroll 1
         for (int o = 16; o > 0; o >>= 1) {
             const double ow = __shfl_xor_sync(0xffffffffu, bw2, o); const unsigned oi = __shfl_xor_sync(0xffffffffu, bi2, o);

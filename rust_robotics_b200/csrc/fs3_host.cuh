@@ -31,6 +31,7 @@ struct pfgpu_fs {
     int post_nt = 256; unsigned post_K = 1, post_tiles = 1, m32 = 0; int log2n = -1; size_t post_smem = 0;
     bool post_global = false;         // the post kernel keeps its weight tiles in global memory (fs3_post_kernel<512, true>) ...
     double* vtile = nullptr;          // ... here: [post_tiles][post_K][512]
+    bool post_k1 = false;             // fs3_post_kernel<512, false, 1>: one weight and at most one local slot per thread (PFGPU_POST_K1=0: off)
     char* est = nullptr; size_t est_bytes = 0;   // pfgpu_fs_moments scratch, allocated by the first call (fs3_est.cuh)
     double* zbuf = nullptr; size_t zcap = 0;     // pfgpu_fs_step_unknown: the (d, angle) list of the step (grows, never shrinks)
     unsigned long long* acnt = nullptr;         // [8] association counters: this launch's, then the last unknown step's (fs3_assoc.cuh);
@@ -53,11 +54,11 @@ extern "C" void pfgpu_fs_default_config(pfgpu_fs_config* c) {            // fs1.
     c->init_weight = 1.0 / 100.0;
 }
 
-template <int NT, bool GTILE>
+template <int NT, bool GTILE, int KC = 0>
 static int fs3_post_prepare(pfgpu_fs* h) {
-    if (cudaFuncSetAttribute(fs3_post_kernel<NT, GTILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
+    if (cudaFuncSetAttribute(fs3_post_kernel<NT, GTILE, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
     int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fs3_post_kernel<NT, GTILE>, NT, h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fs3_post_kernel<NT, GTILE, KC>, NT, h->post_smem) != cudaSuccess) { cudaGetLastError(); return 1; }
     return (size_t)nb * (size_t)h->ctx.num_sms >= h->post_tiles ? 0 : 1;
 }
 
@@ -183,6 +184,12 @@ static int fs_create_impl(const pfgpu_fs_config* cfg, size_t n, size_t n_global,
                 return fail(PFGPU_ERR_UNSUPPORTED);
             }
         }
+        // the shape config 3 runs (2^16 weights on one GPU: 128 tiles x 512 threads x 1) has a kernel compiled for it, with less code
+        // on the path of every step; it needs one value per thread and at most one local slot per thread.  Should it not fit where
+        // the generic kernel does, the generic kernel (the same results) runs.
+        const char* ek = getenv("PFGPU_POST_K1");
+        if (!(ek && ek[0] == '0') && !h->post_global && h->post_nt == 512 && h->post_K == 1 && n <= (size_t)h->post_tiles * 512)
+            h->post_k1 = fs3_post_prepare<512, false, 1>(h) == 0;
     }
     // ONE allocation for everything a peer may touch, same layout on every rank: one IPC mapping per peer exposes all of it
     {
@@ -435,7 +442,8 @@ static int fs_step_end(pfgpu_fs* h, const Fs3ObsParam& po, int k_last, bool host
         PF_LAUNCH(h->ctx, fs3_signal_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
         PF_LAUNCH(h->ctx, fs3_wait_kernel, 1, 32, 0, d, 0, (unsigned)h->n_step + 1u);
     }
-    auto post = h->post_global ? fs3_post_kernel<512, true> : h->post_nt == 512 ? fs3_post_kernel<512, false> : fs3_post_kernel<256, false>;
+    auto post = h->post_global ? fs3_post_kernel<512, true> : h->post_k1 ? fs3_post_kernel<512, false, 1>
+              : h->post_nt == 512 ? fs3_post_kernel<512, false> : fs3_post_kernel<256, false>;
     PF_LAUNCH_PDL(h->ctx, h->pdl, post, h->post_tiles, h->post_nt, h->post_smem, d, po, k_last, h->cfg.nth, h->seed, (unsigned)h->n_step, h->post_K,
                   h->m32, h->log2n, h->early && h->pdl && !host_waits ? 1 : 0, h->vtile);
     h->n_step++;
@@ -831,6 +839,11 @@ extern "C" int pfgpu_fs_post_shape(pfgpu_fs* h, unsigned* tiles, unsigned* threa
     if (threads) *threads = (unsigned)h->post_nt;
     if (values_per_thread) *values_per_thread = h->post_K;
     if (global_tile) *global_tile = h->post_global ? 1 : 0;
+    return 0;
+}
+extern "C" int pfgpu_fs_post_k1(pfgpu_fs* h, int* k1) {
+    if (!h || !k1) return PFGPU_ERR_INVALID;
+    *k1 = h->post_k1 ? 1 : 0;
     return 0;
 }
 extern "C" int pfgpu_fs_time_main_kernel(pfgpu_fs* h, int on) {
