@@ -383,6 +383,86 @@ int  pfgpu_csm_table_info(pfgpu_csm*, double resolution, int64_t* origin_x, int6
                           int32_t* radius);
 int  pfgpu_csm_table_read(pfgpu_csm*, size_t first, size_t count, double* out);
 
+/* ====================================== Grid-based FastSLAM ========================================= */
+
+/* Laser SLAM: a Rao-Blackwellised particle filter with one occupancy grid per particle (not in the reference; "FastSLAM with
+ * occupancy grids", Probabilistic Robotics Table 13.4, the filter GMapping is built on; DESIGN §3.16).  A handle holds N particles on
+ * one GPU, each a pose (x, y, yaw), a weight w and its own grid, laid out and configured exactly as pfgpu_ogm's (cell ix * H + iy,
+ * world (0, 0) at the centre, world_to_grid with the saturating cast).  Every particle starts at the start pose with w = 1/N, its
+ * grid at prior_log_odds.
+ * pfgpu_gs_step(odom, ranges r_0 .. r_{B-1}, angle_min, angle_inc), in this order:
+ *   move       every particle: m = pf_odom_increment(odom, alpha) once per call, then fs_odom_move (include/fs_odom_math.h: pf_odom_move,
+ *              yaw = normalize(yaw)) with (za, zb) = the pair of Philox block (seed, PFC_STREAM_FS_PREDICT, call, slot) and zc = the first
+ *              normal of block (seed, PFC_STREAM_FS_ODOM, call, slot); call = the handle's step counter (0 for the first step).  The
+ *              alphas start at 0.2 each (pfgpu_gs_set_odom_noise: pfgpu_pf_set_odom_noise's rule).
+ *   weigh      every particle against its own grid as it was before this step's scan (an endpoint, "map matching", model).  Used
+ *              beams are the likelihood field's: candidates i = 0, s, 2s, .. < B with s = max(1, (B - 1) / (max_beams - 1)); a
+ *              candidate is used unless r <= 0, r is not finite or r >= max_range.  Per used beam, in ascending i:
+ *              angle = (yaw + angle_min) + i as f64 * angle_inc (one sincos), c = world_to_grid(x + r cos, y + r sin) (saturating,
+ *              inside or not); l* = the maximum log-odds over the cells of the (2R + 1)^2 window around c that lie inside the grid (a
+ *              NaN cell is skipped; no window cell inside, or every one NaN: q = q_out); else q = z_hit * p + q_out with
+ *              p = 1.0 - 1.0 / (1.0 + exp(l*)) (is_occupied's probability, contract exp), q_out = z_rand / max_range.
+ *              w_raw = 1 * q_0 * q_1 * .. over the used beams, w = w * w_raw (weights accumulate between resamples).
+ *   normalise  fs1.rs:186-203: S = the sequential sum of w, w = w / S when S > 0; N_eff = 1 / (the sequential sum of w * w), 0 when
+ *              that sum is 0.  The gate opens when N_eff < nth (absolute, like fs1.rs's NTH).
+ *   fuse       every particle's scan at its moved pose into its own grid: exactly update_with_scan (the pfgpu_ogm rule above, every
+ *              beam, unchanged).
+ *   resample   when the gate opened, fs1.rs:206-234: normalise again (as above), cum = the sequential CDF, r_0 = u * (1/N - 0) + 0
+ *              with u = pfc_u01_52 of the first u64 of block (seed, PFC_STREAM_FS_RESAMPLE, k, 0), k = the resamples so far; slot t
+ *              takes ancestor j (the loop `while r > cum[j + 1] && j < N - 1: j += 1`, r += 1/N per slot): j's pose and a copy of
+ *              j's fused grid; every weight becomes 1/N.
+ *   bound      L = the likelihood field's rule with q_lo = q_out and q_hi = z_hit + q_out: the largest count <= 4096 with
+ *              q_out^(L+1) >= DBL_MIN and q_hi^(L+1) <= DBL_MAX.  A scan with more than L used beams is PFGPU_ERR_INVALID, so
+ *              DBL_MIN <= w_raw <= DBL_MAX.  Why S > 0 always holds: after a normalisation the weights sum to 1 within rounding, so the
+ *              largest is at least about 1/N; that particle's w * w_raw is then at least DBL_MIN / N, a positive (possibly subnormal)
+ *              number for any N below 2^52, and S is at least that term.  Likewise S stays finite: every w <= 1 and w_raw <= DBL_MAX.
+ *   buffers    a resample copies N - (distinct ancestors) grids: the fuse runs once per parent (children share its pose, so they
+ *              share its fused grid), the lowest slot among a parent's children keeps the parent's buffer, and every further child's
+ *              grid is copied into the buffer of a parent without children.  Memory: N grids and a slot -> buffer table, not 2N.
+ *   bits       poses, weights, ancestry and every grid equal the sequential statement above bit for bit.  No floating-point atomics.
+ * pfgpu_gs_create: the ogm fields as pfgpu_ogm_create's; n_particles >= 1 and < 2^32; nth not NaN; z_hit >= 0 and finite; z_rand and
+ *   max_range positive and finite; max_beams >= 2; 0 <= search_radius <= 8; L >= 1; start_pose finite; else PFGPU_ERR_INVALID.  N
+ *   grids that do not fit in the device's free memory: PFGPU_ERR_UNSUPPORTED; an allocation that fails: PFGPU_ERR_CUDA.  Nothing is
+ *   leaked on any refusal.
+ * pfgpu_gs_step: enqueues only, no host synchronisation.  A non-finite odom component, angle_min or angle_inc, ranges NULL with B > 0,
+ *   or more than L used beams: PFGPU_ERR_INVALID, and nothing changes (the step counter included).
+ * pfgpu_gs_download: poses3 (n x 3) and weights (n), both nullable; n must be N.  pfgpu_gs_best: the largest weight, ties to the
+ *   lowest slot.  pfgpu_gs_grid_read: count cells of slot's grid from `first`.  pfgpu_gs_grid_to_ogm: slot's grid into `ogm`, device
+ *   to device; ogm must have the same config (every field) and live on the same device, else PFGPU_ERR_INVALID.
+ * pfgpu_gs_last_indices: the ancestors of the last step's resample; *n = 0 when it did not resample.
+ * pfgpu_gs_info: W, H, N, L and the last step's stats (all nullable).  Every query synchronises. */
+typedef struct {
+    pfgpu_ogm_config ogm;        /* the grid of every particle                             */
+    uint64_t n_particles;        /* 100                                                    */
+    double   nth;                /* 50: resample when N_eff < nth                          */
+    double   z_hit;              /* 0.95                                                   */
+    double   z_rand;             /* 0.05                                                   */
+    double   max_range;          /* 30                                                     */
+    uint32_t max_beams;          /* 60                                                     */
+    uint32_t search_radius;      /* 1: R, the window is (2R + 1)^2 cells                  */
+} pfgpu_gs_config;
+typedef struct {
+    uint64_t steps;              /* steps so far                                           */
+    double   neff;               /* N_eff of the last step                                */
+    uint64_t resampled;          /* 1 when the last step resampled                        */
+    uint64_t copies;             /* grids the last step copied: N - distinct ancestors    */
+    uint64_t events;             /* cell updates the last step's fuse applied: each parent's scan once when it resampled, else every particle's */
+} pfgpu_gs_stats;
+typedef struct pfgpu_gs pfgpu_gs;
+void pfgpu_gs_default_config(pfgpu_gs_config* cfg);
+int  pfgpu_gs_create(const pfgpu_gs_config* cfg, uint64_t seed, const double start_pose[3], int device, pfgpu_gs** out);
+void pfgpu_gs_destroy(pfgpu_gs*);
+int  pfgpu_gs_set_odom_noise(pfgpu_gs*, const double alpha[4]);
+int  pfgpu_gs_odom_noise(pfgpu_gs*, double alpha[4]);
+int  pfgpu_gs_step(pfgpu_gs*, const double odom[6], const double* ranges, size_t n_ranges, double angle_min, double angle_inc);
+int  pfgpu_gs_download(pfgpu_gs*, double* poses3, double* weights, size_t n);
+int  pfgpu_gs_best(pfgpu_gs*, size_t* slot, double pose3[3]);
+int  pfgpu_gs_grid_read(pfgpu_gs*, size_t slot, size_t first, size_t count, double* out);
+int  pfgpu_gs_grid_to_ogm(pfgpu_gs*, size_t slot, pfgpu_ogm* ogm);
+int  pfgpu_gs_last_indices(pfgpu_gs*, uint32_t* idx, size_t cap, size_t* n);
+int  pfgpu_gs_info(pfgpu_gs*, size_t* width, size_t* height, size_t* n, uint64_t* max_used_beams, pfgpu_gs_stats* stats);
+int  pfgpu_gs_sync(pfgpu_gs*);
+
 /* ============================================ FastSLAM 1.0 ========================================== */
 
 /* Module constants of fs1.rs:13-23 as fields; pfgpu_fs_default_config() fills in the reference values. */

@@ -62,6 +62,15 @@ class _OgmStats(C.Structure):
     _fields_ = [("events", C.c_uint64), ("chunks", C.c_uint64), ("longest_run", C.c_uint64), ("event_cap", C.c_uint64)]
 
 
+class _GsCfg(C.Structure):
+    _fields_ = [("ogm", _OgmCfg), ("n_particles", C.c_uint64), ("nth", C.c_double), ("z_hit", C.c_double), ("z_rand", C.c_double),
+                ("max_range", C.c_double), ("max_beams", C.c_uint32), ("search_radius", C.c_uint32)]
+
+
+class _GsStats(C.Structure):
+    _fields_ = [("steps", C.c_uint64), ("neff", C.c_double), ("resampled", C.c_uint64), ("copies", C.c_uint64), ("events", C.c_uint64)]
+
+
 class _CsmCfg(C.Structure):
     _fields_ = [("linear_search_range", C.c_double), ("angular_search_range", C.c_double), ("linear_step", C.c_double),
                 ("angular_step", C.c_double), ("grid_resolution", C.c_double)]
@@ -131,6 +140,9 @@ EXPORTS = [
     "pfgpu_ogm_info", "pfgpu_pf_lfield_set_grid", "pfgpu_pf_beam_set_grid",
     "pfgpu_csm_create", "pfgpu_csm_destroy", "pfgpu_csm_set_reference", "pfgpu_csm_set_reference_grid", "pfgpu_csm_reference_size",
     "pfgpu_csm_match", "pfgpu_csm_table_info", "pfgpu_csm_table_read",
+    "pfgpu_gs_default_config", "pfgpu_gs_create", "pfgpu_gs_destroy", "pfgpu_gs_set_odom_noise", "pfgpu_gs_odom_noise", "pfgpu_gs_step",
+    "pfgpu_gs_download", "pfgpu_gs_best", "pfgpu_gs_grid_read", "pfgpu_gs_grid_to_ogm", "pfgpu_gs_last_indices", "pfgpu_gs_info",
+    "pfgpu_gs_sync",
 ]
 
 
@@ -262,6 +274,20 @@ def load_library():
     L.pfgpu_fs_existence_enable.argtypes = [vp, C.c_double]
     L.pfgpu_fs_existence_counts.argtypes = [vp, C.c_size_t, C.c_size_t, C.POINTER(C.c_int32)]
     L.pfgpu_fs_existence_removed.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.pfgpu_gs_default_config.argtypes, L.pfgpu_gs_default_config.restype = [C.POINTER(_GsCfg)], None
+    L.pfgpu_gs_create.argtypes = [C.POINTER(_GsCfg), C.c_uint64, c_dp, C.c_int, C.POINTER(vp)]
+    L.pfgpu_gs_destroy.argtypes, L.pfgpu_gs_destroy.restype = [vp], None
+    L.pfgpu_gs_set_odom_noise.argtypes = [vp, c_dp]
+    L.pfgpu_gs_odom_noise.argtypes = [vp, c_dp]
+    L.pfgpu_gs_step.argtypes = [vp, c_dp, c_dp, C.c_size_t, C.c_double, C.c_double]
+    L.pfgpu_gs_download.argtypes = [vp, c_dp, c_dp, C.c_size_t]
+    L.pfgpu_gs_best.argtypes = [vp, C.POINTER(C.c_size_t), c_dp]
+    L.pfgpu_gs_grid_read.argtypes = [vp, C.c_size_t, C.c_size_t, C.c_size_t, c_dp]
+    L.pfgpu_gs_grid_to_ogm.argtypes = [vp, C.c_size_t, vp]
+    L.pfgpu_gs_last_indices.argtypes = [vp, c_u32p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.pfgpu_gs_info.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64),
+                                C.POINTER(_GsStats)]
+    L.pfgpu_gs_sync.argtypes = [vp]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
     L.pfgpu_test_pf_tail.argtypes = [vp, c_dp, C.c_size_t, c_dp, C.POINTER(C.c_int)]
@@ -811,6 +837,123 @@ class OccupancyGridMap:
         out = np.empty(1)
         _check(self.L, self.L.pfgpu_ogm_read(self.h, ix * self.H + iy, 1, _dp(out)))
         return float(out[0])
+
+
+# ------------------------------------------------------------------------------------------------
+class GridFastSlamConfig:
+    """Grid-based FastSLAM (DESIGN §3.16): every particle's grid (an OccupancyGridConfig), the particle count, the N_eff threshold
+    (absolute; None = n_particles / 2) and the endpoint model (z_hit, z_rand, max_range, max_beams, search_radius R: the window is
+    (2R + 1)^2 cells)"""
+
+    def __init__(self, grid=None, n_particles=100, nth=None, z_hit=0.95, z_rand=0.05, max_range=30.0, max_beams=60, search_radius=1):
+        self.grid = grid or OccupancyGridConfig()
+        self.n_particles, self.nth = n_particles, nth
+        self.z_hit, self.z_rand, self.max_range, self.max_beams, self.search_radius = z_hit, z_rand, max_range, max_beams, search_radius
+
+    def _c(self):
+        n = int(self.n_particles)
+        if not (0 <= n < 2 ** 64 and 0 <= int(self.max_beams) < 2 ** 32 and 0 <= int(self.search_radius) < 2 ** 32):
+            raise InvalidParameter("n_particles, max_beams, search_radius: out of range")
+        nth = n / 2.0 if self.nth is None else float(self.nth)
+        return _GsCfg(self.grid._c(), n, nth, float(self.z_hit), float(self.z_rand), float(self.max_range), int(self.max_beams),
+                      int(self.search_radius))
+
+
+# GridFastSlam.stats(): steps so far, and the last step's N_eff, whether it resampled, the grids it copied (N - distinct ancestors)
+# and the cell updates its fuse applied
+GsStats = collections.namedtuple("GsStats", ["steps", "neff", "resampled", "copies", "events"])
+
+
+class GridFastSlam:
+    """FastSLAM with occupancy grids (Probabilistic Robotics Table 13.4) on the device: N particles, each a pose, a weight and its
+    own log-odds grid laid out as OccupancyGridMap's.  A step moves every particle by two odometry poses, weighs it by the scan's
+    endpoints against its own grid, normalises, fuses the scan into every grid and resamples when N_eff < nth; see include/pfgpu.h
+    for the rule, which the device follows bit for bit."""
+
+    def __init__(self, config=None, start_pose=(0.0, 0.0, 0.0), seed=0, device=0):
+        self.config = config or GridFastSlamConfig()
+        self.L = load_library()
+        self.h = C.c_void_p()
+        self.device = device
+        _check(self.L, self.L.pfgpu_gs_create(C.byref(self.config._c()), int(seed), _dp(_f64(start_pose)), device, C.byref(self.h)))
+        self.n = int(self.config.n_particles)
+        self.W, self.H = int(self.config.grid.width), int(self.config.grid.height)
+
+    def close(self):
+        if getattr(self, "h", None) and self.h.value:
+            self.L.pfgpu_gs_destroy(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_odometry_noise(self, alpha):
+        """alpha = (alpha1 .. alpha4), each finite and >= 0 (AMCL's odom_alpha1..4; 0.2 each at the start)"""
+        _check(self.L, self.L.pfgpu_gs_set_odom_noise(self.h, _dp(_f64(alpha))))
+
+    def odometry_noise(self):
+        a = np.empty(4)
+        _check(self.L, self.L.pfgpu_gs_odom_noise(self.h, _dp(a)))
+        return tuple(float(v) for v in a)
+
+    def step(self, odom_prev, odom_cur, ranges, angle_min, angle_increment):
+        """One step with the odometry poses (x, y, yaw) before and after it and the scan taken after it; enqueued, not waited for"""
+        o = _f64(list(odom_prev) + list(odom_cur))
+        if o.shape != (6,):
+            raise InvalidParameter("odom_prev, odom_cur: (x, y, yaw) each")
+        r = _f64(ranges).ravel()
+        _check(self.L, self.L.pfgpu_gs_step(self.h, _dp(o), _dp(r), r.size, float(angle_min), float(angle_increment)))
+
+    def particles(self):
+        """(N, 3) poses"""
+        p = np.empty((self.n, 3))
+        _check(self.L, self.L.pfgpu_gs_download(self.h, _dp(p), None, self.n))
+        return p
+
+    def weights(self):
+        w = np.empty(self.n)
+        _check(self.L, self.L.pfgpu_gs_download(self.h, None, _dp(w), self.n))
+        return w
+
+    def best(self):
+        """(slot, pose (3,)) of the largest weight, ties to the lowest slot"""
+        s, p = C.c_size_t(), np.empty(3)
+        _check(self.L, self.L.pfgpu_gs_best(self.h, C.byref(s), _dp(p)))
+        return int(s.value), p
+
+    def grid(self, slot):
+        """slot's log-odds grid, (W, H) f64, downloaded"""
+        out = np.empty((self.W, self.H))
+        _check(self.L, self.L.pfgpu_gs_grid_read(self.h, int(slot), 0, out.size, _dp(out)))
+        return out
+
+    def copy_grid_to(self, slot, grid_map):
+        """slot's grid into an OccupancyGridMap of the same config on the same device, without leaving the device"""
+        _check(self.L, self.L.pfgpu_gs_grid_to_ogm(self.h, int(slot), grid_map.h))
+
+    def last_indices(self):
+        """ancestors of the last step's resample; empty when it did not resample"""
+        idx = np.empty(self.n, dtype=np.uint32)
+        k = C.c_size_t()
+        _check(self.L, self.L.pfgpu_gs_last_indices(self.h, idx.ctypes.data_as(c_u32p), idx.size, C.byref(k)))
+        return idx[:k.value].copy()
+
+    def max_used_beams(self):
+        """L: the most used beams a scan may have"""
+        L = C.c_uint64()
+        _check(self.L, self.L.pfgpu_gs_info(self.h, None, None, None, C.byref(L), None))
+        return int(L.value)
+
+    def stats(self):
+        s = _GsStats()
+        _check(self.L, self.L.pfgpu_gs_info(self.h, None, None, None, None, C.byref(s)))
+        return GsStats(int(s.steps), float(s.neff), bool(s.resampled), int(s.copies), int(s.events))
+
+    def sync(self):
+        _check(self.L, self.L.pfgpu_gs_sync(self.h))
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1465,6 +1465,11 @@ extern "C" int pfgpu_pf_beam_set_grid(pfgpu_pf* h, const pfgpu_ogm* grid, double
 }
 
 // ====================================================================================================
+// Grid-based FastSLAM (DESIGN §3.16): gslam_host.cuh (entry points) + gslam.cuh (kernels)
+// ====================================================================================================
+#include "gslam_host.cuh"
+
+// ====================================================================================================
 // Correlative scan matching (DESIGN §3.13, csm.cuh)
 // ====================================================================================================
 #define PF_CSM_WS_CAP ((size_t)1 << 28)         // bytes of cell indices per launch (X and Y)

@@ -113,6 +113,30 @@ pub struct pfgpu_ogm_stats {
 pub enum pfgpu_pf {}
 pub enum pfgpu_fs {}
 pub enum pfgpu_ogm {}
+/// grid-based FastSLAM (pfgpu_gs_create; defaults 100 particles, nth 50, 0.95, 0.05, 30, 60 beams, R = 1)
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct pfgpu_gs_config {
+    pub ogm: pfgpu_ogm_config,
+    pub n_particles: u64,
+    pub nth: f64,
+    pub z_hit: f64,
+    pub z_rand: f64,
+    pub max_range: f64,
+    pub max_beams: u32,
+    pub search_radius: u32,
+}
+/// steps so far and the last step's N_eff, resampled flag, grids copied and fuse cell updates
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct pfgpu_gs_stats {
+    pub steps: u64,
+    pub neff: f64,
+    pub resampled: u64,
+    pub copies: u64,
+    pub events: u64,
+}
+pub enum pfgpu_gs {}
 /// CorrelativeScanMatcherConfig (pfgpu_csm_match; the reference's defaults 1.0, 0.2, 0.1, 0.02, 0.05)
 #[repr(C)]
 #[derive(Clone, Copy)]
@@ -194,6 +218,20 @@ extern "C" {
     pub fn pfgpu_ogm_info(h: *mut pfgpu_ogm, width: *mut usize, height: *mut usize, stats: *mut pfgpu_ogm_stats) -> c_int;
     pub fn pfgpu_pf_lfield_set_grid(h: *mut pfgpu_pf, grid: *const pfgpu_ogm, threshold: f64, cfg: *const pfgpu_lfield_config) -> c_int;
     pub fn pfgpu_pf_beam_set_grid(h: *mut pfgpu_pf, grid: *const pfgpu_ogm, threshold: f64, cfg: *const pfgpu_beam_config) -> c_int;
+    pub fn pfgpu_gs_default_config(cfg: *mut pfgpu_gs_config);
+    pub fn pfgpu_gs_create(cfg: *const pfgpu_gs_config, seed: u64, start_pose: *const f64, device: c_int, out: *mut *mut pfgpu_gs) -> c_int;
+    pub fn pfgpu_gs_destroy(h: *mut pfgpu_gs);
+    pub fn pfgpu_gs_set_odom_noise(h: *mut pfgpu_gs, alpha: *const f64) -> c_int;
+    pub fn pfgpu_gs_odom_noise(h: *mut pfgpu_gs, alpha: *mut f64) -> c_int;
+    pub fn pfgpu_gs_step(h: *mut pfgpu_gs, odom: *const f64, ranges: *const f64, n_ranges: usize, angle_min: f64, angle_inc: f64) -> c_int;
+    pub fn pfgpu_gs_download(h: *mut pfgpu_gs, poses3: *mut f64, weights: *mut f64, n: usize) -> c_int;
+    pub fn pfgpu_gs_best(h: *mut pfgpu_gs, slot: *mut usize, pose3: *mut f64) -> c_int;
+    pub fn pfgpu_gs_grid_read(h: *mut pfgpu_gs, slot: usize, first: usize, count: usize, out: *mut f64) -> c_int;
+    pub fn pfgpu_gs_grid_to_ogm(h: *mut pfgpu_gs, slot: usize, ogm: *mut pfgpu_ogm) -> c_int;
+    pub fn pfgpu_gs_last_indices(h: *mut pfgpu_gs, idx: *mut u32, cap: usize, n: *mut usize) -> c_int;
+    pub fn pfgpu_gs_info(h: *mut pfgpu_gs, width: *mut usize, height: *mut usize, n: *mut usize, max_used_beams: *mut u64,
+                         stats: *mut pfgpu_gs_stats) -> c_int;
+    pub fn pfgpu_gs_sync(h: *mut pfgpu_gs) -> c_int;
     pub fn pfgpu_csm_create(device: c_int, out: *mut *mut pfgpu_csm) -> c_int;
     pub fn pfgpu_csm_destroy(h: *mut pfgpu_csm);
     pub fn pfgpu_csm_set_reference(h: *mut pfgpu_csm, x: *const f64, y: *const f64, n: usize) -> c_int;

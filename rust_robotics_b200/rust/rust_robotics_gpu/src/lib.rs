@@ -9,10 +9,12 @@
 pub mod correlative_scan_matching;
 pub mod fastslam1;
 pub mod fastslam2;
+pub mod grid_fastslam;
 pub mod monte_carlo_localization;
 pub mod occupancy_grid_map;
 pub mod particle_filter;
 pub use correlative_scan_matching::{correlative_scan_match, CorrelativeScanMatcher, CorrelativeScanMatcherConfig, ScanMatchResult};
+pub use grid_fastslam::{GridFastSlam, GridFastSlamConfig};
 pub use monte_carlo_localization::{MonteCarloLocalizationConfig, MonteCarloLocalizer};
 pub use occupancy_grid_map::{OccupancyGridConfig, OccupancyGridMap};
 pub use particle_filter::{ParticleFilterConfig, ParticleFilterLocalizer};
