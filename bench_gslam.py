@@ -2,6 +2,7 @@
 """bench_gslam.py — grid-based FastSLAM on the device (DESIGN §3.16): what one step of laser SLAM with a grid per particle costs.
 
     python bench_gslam.py [--runs 3] [--sizes 256,1024,4096] [--steps 40]
+    python bench_gslam.py --proposal [--runs 3] [--sizes 32,128,1024] [--steps 40]
 
 Workload: OdomScenario (82 steps of 360-beam scans and wheel odometry in the 40 m x 30 m floor plan), every particle's grid 800 x 600
 at 5 cm (3.84 MB), N = 2^8, 2^10 and 2^12 particles, the default model (R = 1, 60 beams, nth = N / 2).  Per N and run:
@@ -14,6 +15,9 @@ at 5 cm (3.84 MB), N = 2^8, 2^10 and 2^12 particles, the default model (R = 1, 6
                   gate + comb (the exact-sum pipeline, normalisation, search, plan, CUB scans), copy, fuse
   cpu_oracle      tests/host/gs_oracle.c built with glibc libm (compiled into a temporary directory), one host thread, N = 64, at
                   the same grid: ms per step
+With --proposal (DESIGN §3.17) the same workload runs with the scan-matched proposal on (the default GridFastSlamProposal) and off,
+alternated within each run, at N = 32, 128 and 1024 by default; per N and arm: step_us, resamples and grids copied per step, the
+share of particles that took the proposal, and split_ms_per_step with the proposal kernel as "propose".
 Runs alternate their order; medians are reported.  The card's name, power limit and SM clock are on the same JSON line.  Writes
 nothing into the tree.
 """
@@ -42,10 +46,13 @@ HBM_TBS = 3.35
 WARM = 5
 
 
-def make(sc, n, seed=7):
+def make(sc, n, seed=7, prop=False):
     W, H = sc.obstacles.shape
-    return rr.GridFastSlam(rr.GridFastSlamConfig(rr.OccupancyGridConfig(resolution=sc.RES, width=W, height=H), n_particles=n),
-                           start_pose=sc.start, seed=seed)
+    g = rr.GridFastSlam(rr.GridFastSlamConfig(rr.OccupancyGridConfig(resolution=sc.RES, width=W, height=H), n_particles=n),
+                        start_pose=sc.start, seed=seed)
+    if prop:
+        g.set_proposal(rr.GridFastSlamProposal())
+    return g
 
 
 def step(sc, g, t):
@@ -53,9 +60,9 @@ def step(sc, g, t):
     g.step(prev, cur, sc.scans[t], sc.ANGLE_MIN, sc.ANGLE_INC)
 
 
-def timed_run(sc, n, steps, flusher):
-    g = make(sc, n)
-    us, events, copies = [], [], []
+def timed_run(sc, n, steps, flusher, prop=False):
+    g = make(sc, n, prop=prop)
+    us, events, copies, took = [], [], [], []
     for t in range(steps):
         flusher.flush_l2()
         flusher.sync()
@@ -70,13 +77,18 @@ def timed_run(sc, n, steps, flusher):
             events.append(s.events)
             if s.resampled:
                 copies.append(s.copies)
+            if prop:
+                took.append(float(np.mean(g.last_proposal().took)))
     g.close()
-    return statistics.median(us), float(np.mean(events)), (float(np.mean(copies)) if copies else 0.0), len(copies)
+    r = statistics.median(us), float(np.mean(events)), (float(np.mean(copies)) if copies else 0.0), len(copies)
+    return r + ((float(np.mean(took)), float(np.sum(copies)) / len(us)) if prop else ())
 
 
 def kind_of(name):
     if "gs_move_weigh" in name:
         return "move_weigh"
+    if "gs_propose" in name:
+        return "propose"
     if "gs_fuse" in name:
         return "fuse"
     if "gs_copy" in name:
@@ -86,9 +98,9 @@ def kind_of(name):
     return "sums_gate_comb"
 
 
-def profile(sc, n, steps):
+def profile(sc, n, steps, prop=False):
     from torch.profiler import ProfilerActivity, profile as prof
-    g = make(sc, n)
+    g = make(sc, n, prop=prop)
     for t in range(WARM):
         step(sc, g, t)
     g.sync()
@@ -135,14 +147,45 @@ def cpu_oracle(sc, steps, n=64):
     return statistics.median(ms[WARM:])
 
 
+def proposal_arm(sc, sizes, runs, steps):
+    flusher = rr.MonteCarloLocalizer(rr.MonteCarloLocalizationConfig(1024, 1024), seed=1)
+    sampler = bench.ClockSampler(0)
+    res = {(n, p): [] for n in sizes for p in (True, False)}
+    for r in range(runs):
+        for n in (sizes if r % 2 == 0 else sizes[::-1]):
+            for p in ((True, False) if r % 2 == 0 else (False, True)):
+                res[(n, p)].append(timed_run(sc, n, steps, flusher, prop=p))
+    clocks = sampler.stop()
+    out = {}
+    for n in sizes:
+        for p in (True, False):
+            x = res[(n, p)]
+            arm = {"step_us": statistics.median(v[0] for v in x), "step_us_runs": [round(v[0], 1) for v in x],
+                   "resamples_per_step": x[0][3] / (steps - WARM), "copies_per_resample": x[0][2],
+                   "split_ms_per_step": profile(sc, n, steps, prop=p)}
+            if p:
+                arm["copies_per_step"], arm["took_share"] = x[0][5], x[0][4]
+            else:
+                arm["copies_per_step"] = x[0][2] * x[0][3] / (steps - WARM)
+            out[f"{n}_{'proposal' if p else 'plain'}"] = arm
+    W, H = sc.obstacles.shape
+    print(json.dumps({"metric": "grid FastSLAM proposal", "runs": runs, "steps": steps, "grid": [W, H], "results": out,
+                      "gpu": bench.gpu_info(0), "clocks": clocks}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--sizes", default="256,1024,4096")
+    ap.add_argument("--sizes", default=None)
     ap.add_argument("--steps", type=int, default=40)
     ap.add_argument("--cpu-steps", type=int, default=12)
+    ap.add_argument("--proposal", action="store_true")
     a = ap.parse_args()
     sc = scenarios.OdomScenario()
+    if a.proposal:
+        proposal_arm(sc, [int(s) for s in (a.sizes or "32,128,1024").split(",")], a.runs, min(a.steps, sc.steps))
+        return
+    a.sizes = a.sizes or "256,1024,4096"
     steps = min(a.steps, sc.steps)
     sizes = [int(s) for s in a.sizes.split(",")]
     flusher = rr.MonteCarloLocalizer(rr.MonteCarloLocalizationConfig(1024, 1024), seed=1)

@@ -463,6 +463,63 @@ int  pfgpu_gs_last_indices(pfgpu_gs*, uint32_t* idx, size_t cap, size_t* n);
 int  pfgpu_gs_info(pfgpu_gs*, size_t* width, size_t* height, size_t* n, uint64_t* max_used_beams, pfgpu_gs_stats* stats);
 int  pfgpu_gs_sync(pfgpu_gs*);
 
+/* The scan-matched proposal (GMapping's improved proposal: Grisetti, Stachniss and Burgard, IEEE T-RO 23(1), 2007; DESIGN §3.17;
+ * arithmetic in include/gs_prop_math.h).  Off by default; while it is off a step is exactly the rule above.  When it is on, the
+ * move and weigh of pfgpu_gs_step become the following for every particle; normalise, gate, fuse and resample stay as they are,
+ * the fuse at the pose chosen here.  m = pf_odom_increment(odom, alpha), p = the particle's pose before the step.
+ *   0 fallback  the move and weigh above for this particle, unchanged (fs_odom_move with the FS_PREDICT pair and the FS_ODOM normal,
+ *               w = w * w_raw(x')).  Taken when m stands still (every sigma 0, fs2_odom_case's STILL), when the prior covariance
+ *               has no inverse, when the match is uninformative (2) or when eta is not a normal number (4).
+ *   1 prior     (mu, Sigma) = fs_odom_prior(m, p): mu the noise-free move, Sigma with its eps = 1e-8 floor; A = fs2_inv33(Sigma).
+ *   2 match     a brute-force correlative window around mu with CSM's conventions (pfgpu_csm_match): n_l = round(linear_range /
+ *               linear_step), n_a = round(angular_range / angular_step); candidates (mu_x + a ls, mu_y + b ls, normalize(mu_yaw +
+ *               e as)) with a as f64 times the step, |a|, |b| <= n_l, |e| <= n_a, loop index ((a + n_l) NL + b + n_l) NA + e + n_a
+ *               (a outermost, e fastest; NL = 2 n_l + 1, NA = 2 n_a + 1).  A candidate's score is w_raw at its pose (the weigh's
+ *               used beams, arithmetic and beam order); its penalty (dx dx + dy dy) + dyaw dyaw of its offsets.  The winner x^:
+ *               the larger score, then the smaller penalty, then the earlier loop index.  h(x^) = the used beams whose window
+ *               holds a cell inside the grid with l* > 0; h(x^) < min_hits is the uninformative match (e.g. every grid of the
+ *               first step, at prior 0).
+ *   3 lattice   K = (2k + 1)^3 points x_j = (x^_x + a kl, x^_y + b kl, normalize(x^_yaw + e ka)), offsets o_j = (a kl, b kl, e ka),
+ *               |a|, |b|, |e| <= k, in the match's loop order.  L_j = w_raw(x_j); d_j = x_j - mu (yaw difference normalised);
+ *               pi_j = exp(-0.5 * d_j^T A d_j) (contract exp; the quadratic form as gs_prop_quad orders it); tau_j = L_j pi_j.
+ *               Sequential sums in lattice order: T = sum tau_j, m_o = (sum tau_j o_j) / T, C = (sum tau_j (o_j - m_o)(o_j -
+ *               m_o)^T) / T + eps I.
+ *   4 sample    the pose is FastSLAM 2.0's sample of N(x^ + m_o (yaw normalised), C): fs2_propose_pose's Cholesky factor (with its
+ *               diagonal fallback), mean + L (n0, n1, n2) and set_pose's wrap; (n0, n1) = the FS_PREDICT pair, n2 = the first
+ *               normal of block (seed, PFC_STREAM_FS2_POSE3, call, slot) (the draws of DESIGN §3.15).  eta = c T with
+ *               c = kl kl ka / sqrt((2 pi)^3 det Sigma_0) (gs_prop_norm), Sigma_0 the prior covariance at yaw + rot1 = 0: V =
+ *               blockdiag(R(yaw + rot1), 1) V_0 makes det Sigma the same for every particle in exact arithmetic, so c is one number
+ *               per step, computed on the host.  eta is a Riemann estimate of the integral of p(z | m, x) p(x | p, u) over x, the
+ *               quantity a fallback particle's w_raw(x') estimates with one sample, so the two kinds weigh against each other.
+ *               w = w * eta.
+ *   bound       every factor a weight is multiplied by stays in [DBL_MIN, DBL_MAX], so §3.16's argument for S > 0 and finite
+ *               carries over.  w_raw is there by L.  eta: pi_j <= 1 and L_j <= q_hi^k (q_hi = z_hit + q_out), so eta <= c K q_hi^k;
+ *               a non-still step where c K q_hi^k (evaluated as c K, then times q_hi once per used beam) is not <= DBL_MAX is
+ *               PFGPU_ERR_INVALID with nothing changed (it needs q_hi > 1 and many beams; never at the defaults); eta below
+ *               DBL_MIN (or 0, or NaN) takes the fallback.
+ * pfgpu_gs_set_proposal: the ranges finite and >= 0, the four steps finite and > 0, enabled 0 or 1, else PFGPU_ERR_INVALID; a
+ *   half_width above 3, more than 2048 match candidates or more than 1024 match yaws: PFGPU_ERR_UNSUPPORTED.  A refusal changes
+ *   nothing.  It applies from the next step.
+ * pfgpu_gs_last_proposal: per slot, of the last step: x^ (NaN when no match ran), eta (NaN when no lattice ran) and took (1 when
+ *   the particle took the proposal, 0 for the fallback); all NaN / 0 when the last step ran without the proposal.  All nullable;
+ *   n must be N.  Synchronises. */
+typedef struct {
+    uint32_t enabled;               /* 0                                                       */
+    uint32_t half_width;            /* 1: the lattice's k, at most 3                          */
+    double   linear_range;          /* 0.1 m: the match window                                */
+    double   linear_step;           /* 0.025 m                                                 */
+    double   angular_range;         /* 0.05 rad                                                */
+    double   angular_step;          /* 0.0125 rad                                              */
+    double   lattice_linear_step;   /* 0.01 m: kl (GMapping's sample step)                     */
+    double   lattice_angular_step;  /* 0.005 rad: ka                                           */
+    uint32_t min_hits;              /* 10: the fewest hits of an informative match             */
+    uint32_t _pad;
+} pfgpu_gs_proposal;
+void pfgpu_gs_default_proposal(pfgpu_gs_proposal* p);
+int  pfgpu_gs_set_proposal(pfgpu_gs*, const pfgpu_gs_proposal* p);
+int  pfgpu_gs_get_proposal(pfgpu_gs*, pfgpu_gs_proposal* p);
+int  pfgpu_gs_last_proposal(pfgpu_gs*, double* matched3, double* eta, uint8_t* took, size_t n);
+
 /* ============================================ FastSLAM 1.0 ========================================== */
 
 /* Module constants of fs1.rs:13-23 as fields; pfgpu_fs_default_config() fills in the reference values. */

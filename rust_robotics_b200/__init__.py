@@ -5,6 +5,6 @@ reference's public types (ParticleFilterLocalizer, MonteCarloLocalizer, fastslam
 ctypes.  There is no CPU fallback: constructing any filter without a CUDA device raises.
 """
 from .api import (CorrelativeScanMatcher, CorrelativeScanMatcherConfig, FastSlam1, FastSlam2, FsConfig, InvalidParameter,  # noqa: F401
-                  GridFastSlam, GridFastSlamConfig, GsStats, MonteCarloLocalizationConfig, MonteCarloLocalizer,
+                  GridFastSlam, GridFastSlamConfig, GridFastSlamProposal, GsProposal, GsStats, MonteCarloLocalizationConfig, MonteCarloLocalizer,
                   OccupancyGridConfig, OccupancyGridMap, OgmStats, ParticleFilterConfig, ParticleFilterLocalizer, PfgpuError, PfHypothesis,
                   ScanMatchResult, correlative_scan_match, load_library, obstacles_from_log_odds)

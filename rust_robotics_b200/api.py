@@ -71,6 +71,12 @@ class _GsStats(C.Structure):
     _fields_ = [("steps", C.c_uint64), ("neff", C.c_double), ("resampled", C.c_uint64), ("copies", C.c_uint64), ("events", C.c_uint64)]
 
 
+class _GsProp(C.Structure):
+    _fields_ = [("enabled", C.c_uint32), ("half_width", C.c_uint32), ("linear_range", C.c_double), ("linear_step", C.c_double),
+                ("angular_range", C.c_double), ("angular_step", C.c_double), ("lattice_linear_step", C.c_double),
+                ("lattice_angular_step", C.c_double), ("min_hits", C.c_uint32), ("_pad", C.c_uint32)]
+
+
 class _CsmCfg(C.Structure):
     _fields_ = [("linear_search_range", C.c_double), ("angular_search_range", C.c_double), ("linear_step", C.c_double),
                 ("angular_step", C.c_double), ("grid_resolution", C.c_double)]
@@ -142,7 +148,7 @@ EXPORTS = [
     "pfgpu_csm_match", "pfgpu_csm_table_info", "pfgpu_csm_table_read",
     "pfgpu_gs_default_config", "pfgpu_gs_create", "pfgpu_gs_destroy", "pfgpu_gs_set_odom_noise", "pfgpu_gs_odom_noise", "pfgpu_gs_step",
     "pfgpu_gs_download", "pfgpu_gs_best", "pfgpu_gs_grid_read", "pfgpu_gs_grid_to_ogm", "pfgpu_gs_last_indices", "pfgpu_gs_info",
-    "pfgpu_gs_sync",
+    "pfgpu_gs_sync", "pfgpu_gs_default_proposal", "pfgpu_gs_set_proposal", "pfgpu_gs_get_proposal", "pfgpu_gs_last_proposal",
 ]
 
 
@@ -288,6 +294,10 @@ def load_library():
     L.pfgpu_gs_info.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64),
                                 C.POINTER(_GsStats)]
     L.pfgpu_gs_sync.argtypes = [vp]
+    L.pfgpu_gs_default_proposal.argtypes, L.pfgpu_gs_default_proposal.restype = [C.POINTER(_GsProp)], None
+    L.pfgpu_gs_set_proposal.argtypes = [vp, C.POINTER(_GsProp)]
+    L.pfgpu_gs_get_proposal.argtypes = [vp, C.POINTER(_GsProp)]
+    L.pfgpu_gs_last_proposal.argtypes = [vp, c_dp, c_dp, C.POINTER(C.c_uint8), C.c_size_t]
     L.pfgpu_test_div.argtypes = [C.c_ulonglong, C.c_uint64, C.POINTER(C.c_ulonglong), C.c_int]
     L.pfgpu_test_xsum.argtypes = [c_dp, C.c_size_t, c_dp, c_dp, C.POINTER(C.c_int), C.c_int]
     L.pfgpu_test_pf_tail.argtypes = [vp, c_dp, C.c_size_t, c_dp, C.POINTER(C.c_int)]
@@ -859,6 +869,35 @@ class GridFastSlamConfig:
                       int(self.search_radius))
 
 
+class GridFastSlamProposal:
+    """The scan-matched proposal of grid FastSLAM (GMapping's improved proposal, DESIGN §3.17): a correlative match of each particle's
+    scan against its own grid in a window of +-linear_range (linear_step) and +-angular_range (angular_step) around the odometry
+    move, then a lattice of (2 half_width + 1)^3 points at (lattice_linear_step, lattice_angular_step) around the winner; a match with
+    fewer than min_hits beams on occupied cells falls back to the plain odometry move.  See include/pfgpu.h for the rule."""
+
+    def __init__(self, linear_range=0.1, linear_step=0.025, angular_range=0.05, angular_step=0.0125, half_width=1,
+                 lattice_linear_step=0.01, lattice_angular_step=0.005, min_hits=10):
+        self.linear_range, self.linear_step, self.angular_range, self.angular_step = linear_range, linear_step, angular_range, angular_step
+        self.half_width, self.lattice_linear_step, self.lattice_angular_step = half_width, lattice_linear_step, lattice_angular_step
+        self.min_hits = min_hits
+
+    def _c(self, enabled=True):
+        if not (0 <= int(self.half_width) < 2 ** 32 and 0 <= int(self.min_hits) < 2 ** 32):
+            raise InvalidParameter("half_width, min_hits: out of range")
+        return _GsProp(int(enabled), int(self.half_width), float(self.linear_range), float(self.linear_step), float(self.angular_range),
+                       float(self.angular_step), float(self.lattice_linear_step), float(self.lattice_angular_step), int(self.min_hits), 0)
+
+    def as_dict(self):
+        return dict(linear_range=self.linear_range, linear_step=self.linear_step, angular_range=self.angular_range,
+                    angular_step=self.angular_step, half_width=self.half_width, lattice_linear_step=self.lattice_linear_step,
+                    lattice_angular_step=self.lattice_angular_step, min_hits=self.min_hits)
+
+
+# GridFastSlam.last_proposal(): per slot, the last step's match winner (N, 3) (NaN where no match ran), eta (N,) (NaN where no
+# lattice ran) and took (N,) bool: whether the particle took the proposal rather than the fallback
+GsProposal = collections.namedtuple("GsProposal", ["matched", "eta", "took"])
+
+
 # GridFastSlam.stats(): steps so far, and the last step's N_eff, whether it resampled, the grids it copied (N - distinct ancestors)
 # and the cell updates its fuse applied
 GsStats = collections.namedtuple("GsStats", ["steps", "neff", "resampled", "copies", "events"])
@@ -951,6 +990,26 @@ class GridFastSlam:
         s = _GsStats()
         _check(self.L, self.L.pfgpu_gs_info(self.h, None, None, None, None, C.byref(s)))
         return GsStats(int(s.steps), float(s.neff), bool(s.resampled), int(s.copies), int(s.events))
+
+    def set_proposal(self, proposal):
+        """enable the scan-matched proposal with a GridFastSlamProposal, or disable it with None; applies from the next step"""
+        c = GridFastSlamProposal()._c(False) if proposal is None else proposal._c(True)
+        _check(self.L, self.L.pfgpu_gs_set_proposal(self.h, C.byref(c)))
+
+    def proposal(self):
+        """the GridFastSlamProposal in use, or None when the proposal is off"""
+        c = _GsProp()
+        _check(self.L, self.L.pfgpu_gs_get_proposal(self.h, C.byref(c)))
+        if not c.enabled:
+            return None
+        return GridFastSlamProposal(c.linear_range, c.linear_step, c.angular_range, c.angular_step, int(c.half_width),
+                                    c.lattice_linear_step, c.lattice_angular_step, int(c.min_hits))
+
+    def last_proposal(self):
+        """GsProposal of the last step (all NaN / False when it ran without the proposal)"""
+        xh, eta, took = np.empty((self.n, 3)), np.empty(self.n), np.zeros(self.n, dtype=np.uint8)
+        _check(self.L, self.L.pfgpu_gs_last_proposal(self.h, _dp(xh), _dp(eta), took.ctypes.data_as(C.POINTER(C.c_uint8)), self.n))
+        return GsProposal(xh, eta, took.astype(bool))
 
     def sync(self):
         _check(self.L, self.L.pfgpu_gs_sync(self.h))

@@ -13,7 +13,10 @@
 #include "common.cuh"
 #include "xsum.cuh"
 #include "ogm.cuh"
+#include "csm.cuh"                  // pf_csm_better, pf_csm_block_best: the proposal's match winner
 #include "../../include/fs_odom_math.h"
+#include "../../include/gs_prop_math.h"
+#include <limits>
 
 #define GS_WARPS 8                  // particles per CTA of the move + weigh kernel
 #define GS_FUSE_NT 256
@@ -268,6 +271,149 @@ __global__ void __launch_bounds__(256) gs_finish_kernel(GsDev d) {
     d.px[t] = d.tx[t]; d.py[t] = d.ty[t]; d.pyaw[t] = d.tyaw[t];
     d.buf[t] = d.nbuf[t];
     d.w[t] = 1.0 / (double)d.n;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// The scan-matched proposal (DESIGN §3.17, include/gs_prop_math.h): launched instead of gs_move_weigh_kernel when it is enabled.
+#define GS_PROP_NT PF_CSM_NT        // pf_csm_block_best's block size
+#define GS_PROP_TRIG 1024           // (r cos, r sin) pairs per tile of (yaw, beam)
+
+struct GsProp {                     // one step's proposal: the match window, the lattice and c
+    double ls, as, kl, ka, c;
+    int nl, na, k;
+    unsigned min_hits;
+};
+struct GsPropOut {                  // per slot: the match winner x^ (NaN when no match ran), eta (NaN when no lattice ran), took
+    double* xh;
+    double* eta;
+    unsigned char* took;
+};
+
+// w_raw and hit counts of the poses (x0 + a ls, y0 + b ls, normalize(yaw0 + e as)), |a|, |b| <= nl, |e| <= na, pose index
+// ((a + nl) NL + b + nl) NA + e + na, into s_prod / s_hit: the weigh's used beams and arithmetic in beam order (x + r cos is one add
+// on the tile's product), a hit being a beam whose window has a cell inside with l* > 0.  Thread t owns poses t, t + NT, ..; every
+// thread of the CTA calls it.
+__device__ void gs_prop_score(const double* g, const GsModel& m, const double* pairs, unsigned k, double x0, double y0, double yaw0,
+                              int nl, double ls, int na, double as, double2* s_rc, double* s_prod, int* s_hit) {
+    const int NL = 2 * nl + 1, NA = 2 * na + 1, n = NL * NL * NA;
+    for (int c = threadIdx.x; c < n; c += GS_PROP_NT) { s_prod[c] = 1.0; s_hit[c] = 0; }
+    const unsigned bt = GS_PROP_TRIG / (unsigned)NA;
+    const pfc_rcp_t rres = pfc_rcp_make(m.res);
+    for (unsigned b0 = 0; b0 < k; b0 += bt) {
+        const unsigned nb = k - b0 < bt ? k - b0 : bt;
+        __syncthreads();
+        for (unsigned t = threadIdx.x; t < nb * (unsigned)NA; t += GS_PROP_NT) {
+            const unsigned e = t / nb, j = b0 + (t - e * nb);
+            const double yaw = fs_normalize_angle(yaw0 + (double)((int)e - na) * as);
+            const double r = pairs[2 * j], a = pairs[2 * j + 1];
+            double sn, cs;
+            pfc_sincos((yaw + m.angle_min) + a, &sn, &cs);
+            s_rc[t] = make_double2(r * cs, r * sn);
+        }
+        __syncthreads();
+        for (int c = threadIdx.x; c < n; c += GS_PROP_NT) {
+            const int e = c % NA, ab = c / NA;
+            const double x = x0 + (double)(ab / NL - nl) * ls, y = y0 + (double)(ab % NL - nl) * ls;
+            const double2* rc = s_rc + (size_t)e * nb;
+            double p = s_prod[c];
+            int h = s_hit[c];
+            for (unsigned jj = 0; jj < nb; ++jj) {
+                const int cx = pf_lf_sat_i32(floor(pf_ogm_pre(x + rc[jj].x, rres, m.half_w)));
+                const int cy = pf_lf_sat_i32(floor(pf_ogm_pre(y + rc[jj].y, rres, m.half_h)));
+                int any;
+                const double l = gs_window_max(g, m, cx, cy, &any);
+                p = p * (any ? m.z_hit * (1.0 - 1.0 / (1.0 + pfc_exp(l))) + m.q_out : m.q_out);
+                h += (any && l > 0.0) ? 1 : 0;
+            }
+            s_prod[c] = p;
+            s_hit[c] = h;
+        }
+    }
+    __syncthreads();
+}
+
+// One CTA per particle (grid-striding): prior, match, lattice and sample of the rule at include/pfgpu.h pfgpu_gs_proposal, or the
+// fallback (gs_move_weigh_kernel's move and weight).  Thread 0 does the per-particle scalar work; no floating-point atomics.
+__global__ void __launch_bounds__(GS_PROP_NT) gs_propose_kernel(GsDev d, PfOdom om, uint64_t seed, uint32_t call, GsModel m,
+                                                                const double* pairs, unsigned k, GsProp P, GsPropOut out) {
+    __shared__ double2 s_rc[GS_PROP_TRIG];
+    __shared__ double s_prod[GS_PROP_MAX_CAND];
+    __shared__ int s_hit[GS_PROP_MAX_CAND];
+    __shared__ double s_mu[3], s_A[9], s_xh[3], s_x[3];
+    __shared__ int s_go;
+    const int K = (2 * P.k + 1) * (2 * P.k + 1) * (2 * P.k + 1);
+    for (size_t i = blockIdx.x; i < d.n; i += gridDim.x) {
+        const double* g = d.grids + (size_t)d.buf[i] * d.cells;
+        __syncthreads();                                    // the previous particle's shared state is read
+        if (threadIdx.x == 0) {
+            double cov[9];
+            fs_odom_prior(&om, d.px[i], d.py[i], d.pyaw[i], s_mu, cov);
+            s_go = !gs_prop_still(&om) && fs2_inv33(cov, s_A);
+            const double nan = __longlong_as_double(0x7FF8000000000000ll);
+            out.xh[3 * i] = nan; out.xh[3 * i + 1] = nan; out.xh[3 * i + 2] = nan;
+            out.eta[i] = nan;
+            out.took[i] = 0;
+        }
+        __syncthreads();
+        if (s_go) {                                         // the match
+            gs_prop_score(g, m, pairs, k, s_mu[0], s_mu[1], s_mu[2], P.nl, P.ls, P.na, P.as, s_rc, s_prod, s_hit);
+            const int NL = 2 * P.nl + 1, NA = 2 * P.na + 1, n = NL * NL * NA;
+            PfCsmBest b{-1.0, __longlong_as_double(0x7FF0000000000000ll), ~0ull};
+            for (int c = threadIdx.x; c < n; c += GS_PROP_NT) {
+                int a, bb, e;
+                gs_prop_index(c, P.nl, P.na, &a, &bb, &e);
+                const double dx = (double)a * P.ls, dy = (double)bb * P.ls, dyaw = (double)e * P.as;
+                const PfCsmBest cur{s_prod[c], (dx * dx + dy * dy) + dyaw * dyaw, (unsigned long long)c};
+                if (pf_csm_better(cur, b)) b = cur;
+            }
+            b = pf_csm_block_best(b);
+            if (threadIdx.x == 0) {
+                int a, bb, e;
+                gs_prop_index((int)b.idx, P.nl, P.na, &a, &bb, &e);
+                s_xh[0] = s_mu[0] + (double)a * P.ls;
+                s_xh[1] = s_mu[1] + (double)bb * P.ls;
+                s_xh[2] = fs_normalize_angle(s_mu[2] + (double)e * P.as);
+                for (int j = 0; j < 3; ++j) out.xh[3 * i + j] = s_xh[j];
+                s_go = (unsigned)s_hit[b.idx] >= P.min_hits;
+            }
+            __syncthreads();
+        }
+        if (s_go) {                                         // the lattice, then the sums and the sample in thread 0
+            gs_prop_score(g, m, pairs, k, s_xh[0], s_xh[1], s_xh[2], P.k, P.kl, P.k, P.ka, s_rc, s_prod, s_hit);
+            for (int j = threadIdx.x; j < K; j += GS_PROP_NT) s_prod[j] = gs_prop_tau(j, P.k, P.kl, P.ka, s_xh, s_mu, s_A, s_prod[j]);
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                double n0, n1, n2, unused, pose[3], eta;
+                pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_PREDICT, call, (uint64_t)i), &n0, &n1);
+                pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS2_POSE3, call, (uint64_t)i), &n2, &unused);
+                s_go = gs_prop_sample(s_prod, P.k, P.kl, P.ka, s_xh, P.c, n0, n1, n2, pose, &eta);
+                out.eta[i] = eta;
+                if (s_go) {
+                    d.px[i] = pose[0]; d.py[i] = pose[1]; d.pyaw[i] = pose[2];
+                    d.w[i] = d.w[i] * eta;
+                    out.took[i] = 1;
+                }
+            }
+            __syncthreads();
+        }
+        if (!s_go) {                                        // the fallback: gs_move_weigh_kernel's move and weight
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                double za, zb, zc, unused;
+                pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_PREDICT, call, (uint64_t)i), &za, &zb);
+                pfc_normal_pair(pfc_rng_block(seed, PFC_STREAM_FS_ODOM, call, (uint64_t)i), &zc, &unused);
+                double x = d.px[i], y = d.py[i], yaw = d.pyaw[i];
+                fs_odom_move(&om, za, zb, zc, &x, &y, &yaw);
+                s_x[0] = x; s_x[1] = y; s_x[2] = yaw;
+            }
+            __syncthreads();
+            gs_prop_score(g, m, pairs, k, s_x[0], s_x[1], s_x[2], 0, 0.0, 0, 0.0, s_rc, s_prod, s_hit);
+            if (threadIdx.x == 0) {
+                d.px[i] = s_x[0]; d.py[i] = s_x[1]; d.pyaw[i] = s_x[2];
+                d.w[i] = d.w[i] * s_prod[0];
+            }
+        }
+    }
 }
 
 __global__ void __launch_bounds__(256) gs_init_kernel(GsDev d, double x, double y, double yaw) {

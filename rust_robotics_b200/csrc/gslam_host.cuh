@@ -16,12 +16,16 @@ struct pfgpu_gs {
     double* pairs = nullptr;           // [2 * L] its used beams (r, i * angle_inc)
     size_t rcap = 0;
     std::vector<double> hp;            // host staging of the used beams
+    pfgpu_gs_proposal prop = {};       // the scan-matched proposal (DESIGN §3.17); off until pfgpu_gs_set_proposal enables it
+    GsPropOut pout = {};               // [3n], [n], [n]: allocated when the proposal is first enabled
+    bool last_prop = false;            // the last step ran the proposal
 };
 
 static void gs_free(pfgpu_gs* h) {
     GsDev& d = h->d;
     void* p[] = { d.px, d.py, d.pyaw, d.w, d.tx, d.ty, d.tyaw, d.grids, d.buf, d.nbuf, d.idx, d.cum, d.comb, d.nf, d.enf, d.cl, d.ecl,
-                  d.has_child, d.free_buf, d.job_src, d.job_dst, d.scal, d.gate, d.cnt, h->tmp, h->ranges, h->pairs };
+                  d.has_child, d.free_buf, d.job_src, d.job_dst, d.scal, d.gate, d.cnt, h->tmp, h->ranges, h->pairs,
+                  h->pout.xh, h->pout.eta, h->pout.took };
     for (void* q : p) cudaFree(q);
     if (h->xs.flags) xs_work_free(h->xs);
     if (h->ctx.stream) cudaStreamDestroy(h->ctx.stream);
@@ -41,6 +45,18 @@ extern "C" void pfgpu_gs_default_config(pfgpu_gs_config* c) {
     c->ogm.max_log_odds = 5.0; c->ogm.min_log_odds = -5.0;
     c->n_particles = 100; c->nth = 50.0;
     c->z_hit = 0.95; c->z_rand = 0.05; c->max_range = 30.0; c->max_beams = 60; c->search_radius = 1;
+}
+extern "C" void pfgpu_gs_default_proposal(pfgpu_gs_proposal* p) {
+    if (!p) return;
+    *p = pfgpu_gs_proposal();
+    p->enabled = 0; p->half_width = 1; p->min_hits = 10;
+    p->linear_range = 0.1; p->linear_step = 0.025; p->angular_range = 0.05; p->angular_step = 0.0125;
+    p->lattice_linear_step = 0.01; p->lattice_angular_step = 0.005;
+}
+// the match's half-widths n = round(range / step) (CSM's rule) of a validated config
+static void gs_prop_window(const pfgpu_gs_proposal& p, int* nl, int* na) {
+    *nl = (int)round(p.linear_range / p.linear_step);
+    *na = (int)round(p.angular_range / p.angular_step);
 }
 // pfgpu_ogm_create's checks of the grid fields
 static bool gs_ogm_cfg_ok(const pfgpu_ogm_config* c) {
@@ -88,6 +104,7 @@ extern "C" int pfgpu_gs_create(const pfgpu_gs_config* c, uint64_t seed, const do
     pfgpu_gs* h = new (std::nothrow) pfgpu_gs();
     if (!h) return PFGPU_ERR_CUDA;
     h->cfg = *c; h->seed = seed; h->L = L; h->q_out = q_out;
+    pfgpu_gs_default_proposal(&h->prop);
     h->d.n = n; h->d.cells = cells;
     int rc = ctx_open(h->ctx, device);
     if (rc) { gs_free(h); delete h; return rc; }
@@ -150,6 +167,25 @@ extern "C" int pfgpu_gs_step(pfgpu_gs* h, const double odom[6], const double* ra
     }
     const size_t k = hp.size() / 2;
     if (k > h->L) return PFGPU_ERR_INVALID;
+    // the proposal's constants, and the high side of its bound: c K q_hi^k <= DBL_MAX (a still step proposes nothing)
+    const pfgpu_gs_proposal& pc = h->prop;
+    GsProp P = {};
+    if (pc.enabled) {
+        gs_prop_window(pc, &P.nl, &P.na);
+        P.ls = pc.linear_step; P.as = pc.angular_step; P.kl = pc.lattice_linear_step; P.ka = pc.lattice_angular_step;
+        P.k = (int)pc.half_width; P.min_hits = pc.min_hits;
+        P.c = gs_prop_norm(&om, P.kl, P.ka);
+        if (!gs_prop_still(&om)) {
+            const double S = (double)(2 * P.k + 1);
+            double hi = P.c * ((S * S) * S);
+            const double q_hi = c.z_hit + h->q_out;
+            for (size_t j = 0; j < k; ++j) hi = hi * q_hi;
+            if (!(hi <= DBL_MAX)) {
+                snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "grid FastSLAM proposal: eta's bound c K q_hi^k exceeds DBL_MAX at %zu used beams", k);
+                return PFGPU_ERR_INVALID;
+            }
+        }
+    }
     PF_CUDA(cudaSetDevice(h->ctx.device));
     Ctx& ctx = h->ctx;
     GsDev& d = h->d;
@@ -168,8 +204,13 @@ extern "C" int pfgpu_gs_step(pfgpu_gs* h, const double odom[6], const double* ra
     m.z_hit = c.z_hit; m.q_out = h->q_out; m.angle_min = angle_min;
     const size_t n = d.n;
     // move + weigh, normalise, N_eff and the gate
-    PF_LAUNCH(ctx, gs_move_weigh_kernel, cdiv_u(n, GS_WARPS), GS_WARPS * 32, 0, d, om, h->seed, (uint32_t)h->steps, m,
-              (const double*)h->pairs, (unsigned)k);
+    if (pc.enabled)
+        PF_LAUNCH(ctx, gs_propose_kernel, (unsigned)std::min<size_t>(n, (size_t)1 << 20), GS_PROP_NT, 0, d, om, h->seed, (uint32_t)h->steps,
+                  m, (const double*)h->pairs, (unsigned)k, P, h->pout);
+    else
+        PF_LAUNCH(ctx, gs_move_weigh_kernel, cdiv_u(n, GS_WARPS), GS_WARPS * 32, 0, d, om, h->seed, (uint32_t)h->steps, m,
+                  (const double*)h->pairs, (unsigned)k);
+    h->last_prop = pc.enabled != 0;
     int rc = gs_normalize(h, d.scal + 0, nullptr);
     if (rc) return rc;
     rc = xs_total(ctx, h->xs, PfValWSq{d.w}, n, n, 0.0, d.scal + 1);
@@ -306,5 +347,57 @@ extern "C" int pfgpu_gs_info(pfgpu_gs* h, size_t* W, size_t* H, size_t* n, uint6
         st->copies = gate ? cnt[1] : 0;
         st->events = h->steps ? cnt[2] : 0;
     }
+    return 0;
+}
+extern "C" int pfgpu_gs_set_proposal(pfgpu_gs* h, const pfgpu_gs_proposal* p) {
+    if (!h || !p || p->enabled > 1) return PFGPU_ERR_INVALID;
+    auto step_ok = [](double v) { return finite_d(v) && v > 0.0; };
+    auto range_ok = [](double v) { return finite_d(v) && v >= 0.0; };
+    if (!range_ok(p->linear_range) || !step_ok(p->linear_step) || !range_ok(p->angular_range) || !step_ok(p->angular_step) ||
+        !step_ok(p->lattice_linear_step) || !step_ok(p->lattice_angular_step))
+        return PFGPU_ERR_INVALID;
+    const double rl = round(p->linear_range / p->linear_step), ra = round(p->angular_range / p->angular_step);
+    const double cand = (2.0 * rl + 1.0) * (2.0 * rl + 1.0) * (2.0 * ra + 1.0);
+    if (p->half_width > GS_PROP_MAX_K || !(cand <= GS_PROP_MAX_CAND) || !(2.0 * ra + 1.0 <= GS_PROP_MAX_YAWS)) {
+        snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "grid FastSLAM proposal: lattice half-width %u (at most %d) or %.0f match candidates "
+                 "(at most %d)", p->half_width, GS_PROP_MAX_K, cand, GS_PROP_MAX_CAND);
+        return PFGPU_ERR_UNSUPPORTED;
+    }
+    if (p->enabled && !h->pout.xh) {
+        const size_t n = h->d.n;
+        PF_CUDA(cudaSetDevice(h->ctx.device));
+        GsPropOut o = {};
+        if (cudaMalloc(&o.xh, 3 * n * sizeof(double)) != cudaSuccess || cudaMalloc(&o.eta, n * sizeof(double)) != cudaSuccess ||
+            cudaMalloc(&o.took, n) != cudaSuccess) {
+            cudaFree(o.xh); cudaFree(o.eta); cudaFree(o.took);
+            cudaGetLastError();
+            snprintf(g_pfgpu_err, sizeof(g_pfgpu_err), "grid FastSLAM proposal: out of device memory for %zu slots", n);
+            return PFGPU_ERR_CUDA;
+        }
+        h->pout = o;
+    }
+    h->prop = *p;
+    return 0;
+}
+extern "C" int pfgpu_gs_get_proposal(pfgpu_gs* h, pfgpu_gs_proposal* p) {
+    if (!h || !p) return PFGPU_ERR_INVALID;
+    *p = h->prop;
+    return 0;
+}
+extern "C" int pfgpu_gs_last_proposal(pfgpu_gs* h, double* matched3, double* eta, uint8_t* took, size_t n) {
+    if (!h || n != h->d.n) return PFGPU_ERR_INVALID;
+    PF_CUDA(cudaSetDevice(h->ctx.device));
+    if (!h->last_prop) {
+        const double nan = std::numeric_limits<double>::quiet_NaN();
+        PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
+        if (matched3) std::fill(matched3, matched3 + 3 * n, nan);
+        if (eta) std::fill(eta, eta + n, nan);
+        if (took) std::fill(took, took + n, (uint8_t)0);
+        return 0;
+    }
+    if (matched3) PF_CUDA(cudaMemcpyAsync(matched3, h->pout.xh, 3 * n * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    if (eta) PF_CUDA(cudaMemcpyAsync(eta, h->pout.eta, n * sizeof(double), cudaMemcpyDeviceToHost, h->ctx.stream));
+    if (took) PF_CUDA(cudaMemcpyAsync(took, h->pout.took, n, cudaMemcpyDeviceToHost, h->ctx.stream));
+    PF_CUDA(cudaStreamSynchronize(h->ctx.stream));
     return 0;
 }

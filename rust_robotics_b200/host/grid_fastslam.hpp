@@ -23,6 +23,21 @@ struct GridFastSlamConfig {
     }
 };
 
+// the scan-matched proposal's parameters (pfgpu_gs_proposal without `enabled`), the defaults of pfgpu_gs_default_proposal
+struct GridFastSlamProposal {
+    double linear_range = 0.1, linear_step = 0.025, angular_range = 0.05, angular_step = 0.0125;
+    uint32_t half_width = 1;
+    double lattice_linear_step = 0.01, lattice_angular_step = 0.005;
+    uint32_t min_hits = 10;
+    pfgpu_gs_proposal to_c() const {
+        pfgpu_gs_proposal c{};
+        c.half_width = half_width; c.linear_range = linear_range; c.linear_step = linear_step; c.angular_range = angular_range;
+        c.angular_step = angular_step; c.lattice_linear_step = lattice_linear_step; c.lattice_angular_step = lattice_angular_step;
+        c.min_hits = min_hits;
+        return c;
+    }
+};
+
 class GridFastSlam {
     pfgpu_gs* h_ = nullptr;
 public:
@@ -84,6 +99,25 @@ public:
         pfgpu_gs_stats s{};
         check(pfgpu_gs_info(h_, nullptr, nullptr, nullptr, nullptr, &s), "stats");
         return s;
+    }
+    // the scan-matched proposal (DESIGN §3.17): enabled with a config, disabled with nullptr; applies from the next step
+    void set_proposal(const GridFastSlamProposal* p) {
+        pfgpu_gs_proposal c{};
+        pfgpu_gs_default_proposal(&c);
+        if (p) { c = p->to_c(); c.enabled = 1; }
+        check(pfgpu_gs_set_proposal(h_, &c), "set_proposal");
+    }
+    pfgpu_gs_proposal proposal() const {
+        pfgpu_gs_proposal c{};
+        check(pfgpu_gs_get_proposal(h_, &c), "proposal");
+        return c;
+    }
+    // the last step's per-slot match winners (n x 3), eta and whether each particle took the proposal
+    struct Proposal { std::vector<double> matched, eta; std::vector<uint8_t> took; };
+    Proposal last_proposal() const {
+        Proposal r{std::vector<double>(3 * config.n_particles), std::vector<double>(config.n_particles), std::vector<uint8_t>(config.n_particles)};
+        check(pfgpu_gs_last_proposal(h_, r.matched.data(), r.eta.data(), r.took.data(), config.n_particles), "last_proposal");
+        return r;
     }
     void sync() { check(pfgpu_gs_sync(h_), "sync"); }
 };

@@ -137,6 +137,22 @@ pub struct pfgpu_gs_stats {
     pub events: u64,
 }
 pub enum pfgpu_gs {}
+/// grid FastSLAM's scan-matched proposal (pfgpu_gs_default_proposal: off, +-0.1 m at 0.025 m, +-0.05 rad at 0.0125 rad, lattice k = 1
+/// at 0.01 m and 0.005 rad, min_hits 10)
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug, PartialEq)]
+pub struct pfgpu_gs_proposal {
+    pub enabled: u32,
+    pub half_width: u32,
+    pub linear_range: f64,
+    pub linear_step: f64,
+    pub angular_range: f64,
+    pub angular_step: f64,
+    pub lattice_linear_step: f64,
+    pub lattice_angular_step: f64,
+    pub min_hits: u32,
+    pub _pad: u32,
+}
 /// CorrelativeScanMatcherConfig (pfgpu_csm_match; the reference's defaults 1.0, 0.2, 0.1, 0.02, 0.05)
 #[repr(C)]
 #[derive(Clone, Copy)]
@@ -232,6 +248,10 @@ extern "C" {
     pub fn pfgpu_gs_info(h: *mut pfgpu_gs, width: *mut usize, height: *mut usize, n: *mut usize, max_used_beams: *mut u64,
                          stats: *mut pfgpu_gs_stats) -> c_int;
     pub fn pfgpu_gs_sync(h: *mut pfgpu_gs) -> c_int;
+    pub fn pfgpu_gs_default_proposal(p: *mut pfgpu_gs_proposal);
+    pub fn pfgpu_gs_set_proposal(h: *mut pfgpu_gs, p: *const pfgpu_gs_proposal) -> c_int;
+    pub fn pfgpu_gs_get_proposal(h: *mut pfgpu_gs, p: *mut pfgpu_gs_proposal) -> c_int;
+    pub fn pfgpu_gs_last_proposal(h: *mut pfgpu_gs, matched3: *mut f64, eta: *mut f64, took: *mut u8, n: usize) -> c_int;
     pub fn pfgpu_csm_create(device: c_int, out: *mut *mut pfgpu_csm) -> c_int;
     pub fn pfgpu_csm_destroy(h: *mut pfgpu_csm);
     pub fn pfgpu_csm_set_reference(h: *mut pfgpu_csm, x: *const f64, y: *const f64, n: usize) -> c_int;

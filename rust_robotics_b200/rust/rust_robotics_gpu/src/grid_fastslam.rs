@@ -100,6 +100,28 @@ impl GridFastSlam {
         status(unsafe { sys::pfgpu_gs_info(self.h, std::ptr::null_mut(), std::ptr::null_mut(), std::ptr::null_mut(), std::ptr::null_mut(), &mut s) })?;
         Ok(s)
     }
+    /// the scan-matched proposal (DESIGN §3.17): `Some(p)` enables it with p's parameters (p.enabled is ignored), `None` disables
+    /// it; applies from the next step
+    pub fn set_proposal(&mut self, p: Option<sys::pfgpu_gs_proposal>) -> RoboticsResult<()> {
+        let mut c = sys::pfgpu_gs_proposal::default();
+        unsafe { sys::pfgpu_gs_default_proposal(&mut c) };
+        if let Some(p) = p { c = p; c.enabled = 1; }
+        status(unsafe { sys::pfgpu_gs_set_proposal(self.h, &c) })
+    }
+    /// the proposal in use, `None` when it is off
+    pub fn proposal(&self) -> RoboticsResult<Option<sys::pfgpu_gs_proposal>> {
+        let mut c = sys::pfgpu_gs_proposal::default();
+        status(unsafe { sys::pfgpu_gs_get_proposal(self.h, &mut c) })?;
+        Ok(if c.enabled != 0 { Some(c) } else { None })
+    }
+    /// the last step's per-slot match winners (x, y, yaw; NaN where no match ran), eta (NaN where no lattice ran) and whether each
+    /// particle took the proposal
+    pub fn last_proposal(&self) -> RoboticsResult<(Vec<[f64; 3]>, Vec<f64>, Vec<bool>)> {
+        let n = self.config.n_particles;
+        let (mut xh, mut eta, mut took) = (vec![0.0f64; 3 * n], vec![0.0f64; n], vec![0u8; n]);
+        status(unsafe { sys::pfgpu_gs_last_proposal(self.h, xh.as_mut_ptr(), eta.as_mut_ptr(), took.as_mut_ptr(), n) })?;
+        Ok((xh.chunks(3).map(|c| [c[0], c[1], c[2]]).collect(), eta, took.into_iter().map(|t| t != 0).collect()))
+    }
 }
 
 impl Drop for GridFastSlam {
